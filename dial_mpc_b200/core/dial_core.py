@@ -46,7 +46,9 @@ def softmax_update(weights, Y0s, sigma, mu_0t):
 
 class MBDPI:
     def __init__(self, args: DialConfig, env, rank: int = 0, world_size: int = 1, process_group=None,
-                 compute_bars: bool = True, plan_factory=None):
+                 compute_bars: bool = True, plan_factory=None, n_instances: int = 1):
+        """``n_instances`` > 1: one plan holds that many independent planner instances (same model,
+        config and annealing schedule; own state, rng and knots), advanced together by ``DeviceLoop``."""
         self.args = args
         self.env = env
         self.nu = env.action_size
@@ -58,6 +60,9 @@ class MBDPI:
         if args.Nsample % world_size != 0:
             raise ValueError("Nsample must be divisible by the number of ranks")
         self.Nlocal = args.Nsample // world_size
+        self.n_instances = int(n_instances)
+        if self.n_instances < 1:
+            raise ValueError("n_instances must be >= 1")
 
         sigma_control = args.horizon_diffuse_factor ** np.arange(args.Hnode + 1)[::-1]
         self.sigma_control_np = (sigma_control * args.sigma_scale).astype(np.float64)
@@ -72,7 +77,7 @@ class MBDPI:
 
         desc = env.plan_desc(Nsample=self.Nlocal, Ntotal=args.Nsample, shard_offset=rank * self.Nlocal,
                              Hsample=args.Hsample, Hnode=args.Hnode, temp_sample=args.temp_sample,
-                             M_n2u=self.M_n2u_np)
+                             M_n2u=self.M_n2u_np, n_inst=self.n_instances)
         # plan_factory exists for the CPU test harness (tests/emul); the product path is Plan
         self.plan = (plan_factory or Plan)(env, desc)
         dev = self.plan.device
@@ -140,6 +145,7 @@ class MBDPI:
     def reverse_once(self, state, rng, Ybar_i, noise_scale, eps=None, _sync_bars=True):
         """One annealing iteration.  ``eps`` (optional, [Nsample,Hnode+1,nu]) injects the noise;
         otherwise it is drawn in-kernel from the Threefry stream keyed by ``split(rng)[1]``."""
+        self._single("reverse_once")
         rng, Y0s_rng = drandom.split(rng)
         Ybar_i = self._t(Ybar_i)
         noise_scale = self._t(noise_scale)
@@ -200,6 +206,11 @@ class MBDPI:
             info["xbar"] = xbar.view(Hs1, m.nbody - 1, 3)
         return rng, Ybar, info
 
+    def _single(self, what: str) -> None:
+        if self.n_instances > 1:
+            raise RuntimeError(f"MBDPI.{what} plans one instance; a plan of {self.n_instances} instances runs "
+                               "through DeviceLoop (one CUDA graph per control step for all instances)")
+
     @property
     def exchange_name(self) -> str:
         if self.world_size == 1:
@@ -211,6 +222,7 @@ class MBDPI:
         """Device time (microseconds, CUDA events on the current stream) of the stages of one
         ``reverse_once``: rollout | rewards exchange | weights + Ybar | bars (+ their allreduce).
         Measurement aid for bench.py; the stages run back to back on one stream here."""
+        self._single("phase_times")
         Ybar_i, noise_scale = self._t(Ybar_i), self._t(noise_scale)
         N, Nl = self.args.Nsample, self.Nlocal
         m = self.env.sys
@@ -246,6 +258,7 @@ class MBDPI:
 
     def reverse_scan(self, state, rng, Y0, factors):
         """``lax.scan(reverse_scan, (rng, Y0, state), factors)`` of dial_core.py:177-180,262-264."""
+        self._single("reverse_scan")
         info = None
         n = factors.shape[0]
         for i in range(n):
@@ -281,41 +294,62 @@ class DeviceLoop:
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
                  compute_bars: bool = True, noise=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
-        deploy planner passes its own, dial_plan.py:199-209)."""
+        deploy planner passes its own, dial_plan.py:199-209).
+
+        Batched ``mbdpi`` (``n_instances`` = B > 1): ``state`` is a sequence of B States, ``rng`` [B,2]
+        uint32 and ``Y0`` [B,Hnode+1,nu] or None.  Every per-instance buffer, ``Y``, ``action``,
+        ``reward``, ``info()`` and ``set_state`` gain a leading [B]; ``state(b)`` materialises
+        instance b.  Instance b computes bitwise what a single-instance loop from its state, rng and
+        knots computes."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
         self.mbdpi, self.plan = mbdpi, mbdpi.plan
         a, pl, dev = mbdpi.args, mbdpi.plan, mbdpi.device
         nmax = int(n_diffuse_max or max(a.Ndiffuse, a.Ndiffuse_init))
-        ps = state.pipeline_state
         f, e = pl.f32, pl.empty
         Hs1 = a.Hsample + 1
         m = mbdpi.env.sys
-        key = np.ascontiguousarray(rng, dtype=np.uint32).view(np.int32)
-        self.info0 = dict(state.info)
+        B = self.n_instances = mbdpi.n_instances
+        states = list(state) if B > 1 else [state]
+        if len(states) != B:
+            raise ValueError(f"a plan of {B} instances needs {B} states, got {len(states)}")
+        if B > 1 and any(s.info.get("randomize_target", False) for s in states):
+            raise RuntimeError("randomize_tasks draws per-instance commands, which a batched DeviceLoop does not "
+                               "support: run one DeviceLoop per instance")
+        lead = (B,) if B > 1 else ()
+        key = np.ascontiguousarray(rng, dtype=np.uint32)
+        if key.shape != lead + (2,):
+            raise ValueError(f"rng must have shape {lead + (2,)}, got {key.shape}")
+        if Y0 is not None and tuple(np.shape(Y0)) != lead + (a.Hnode + 1, mbdpi.nu):
+            raise ValueError(f"Y0 must have shape {lead + (a.Hnode + 1, mbdpi.nu)}, got {tuple(np.shape(Y0))}")
+        ps = [s.pipeline_state for s in states]
+        per = (lambda t: t[0]) if B == 1 else torch.stack   # one instance: the buffers keep their plain shapes
+        counters = [[int(s.info.get("step", 0)), int(s.info.get("contact_stage", 0))] for s in states]
+        self.info0 = dict(state.info) if B == 1 else [dict(s.info) for s in states]
         self.buf = dict(
-            qpos=f(ps.qpos).clone(), qvel=f(ps.qvel).clone(), qacc_warmstart=f(ps.qacc_warmstart).clone(),
-            counters=torch.tensor([int(state.info.get("step", 0)), int(state.info.get("contact_stage", 0))],
-                                  dtype=torch.int32, device=dev),
-            rng=torch.as_tensor(key.copy(), device=dev),
-            Y=(torch.zeros(a.Hnode + 1, mbdpi.nu, device=dev) if Y0 is None else f(Y0).clone()),
-            ctrl=torch.zeros(mbdpi.nu, device=dev), reward=torch.zeros(1, device=dev),
-            rews=torch.zeros(mbdpi.Nlocal + 1, device=dev),
+            qpos=per([f(p.qpos) for p in ps]).clone(), qvel=per([f(p.qvel) for p in ps]).clone(),
+            qacc_warmstart=per([f(p.qacc_warmstart) for p in ps]).clone(),
+            counters=torch.tensor(counters[0] if B == 1 else counters, dtype=torch.int32, device=dev),
+            rng=torch.as_tensor(key.view(np.int32).copy(), device=dev),
+            Y=(torch.zeros(*lead, a.Hnode + 1, mbdpi.nu, device=dev) if Y0 is None else f(Y0).clone()),
+            ctrl=torch.zeros(*lead, mbdpi.nu, device=dev), reward=torch.zeros(B, device=dev),
+            rews=torch.zeros(*lead, mbdpi.Nlocal + 1, device=dev),
             rews_all=(torch.zeros(a.Nsample + 1, device=dev) if mbdpi.world_size > 1 else None),
-            qbar=e(Hs1, m.nq) if compute_bars else None, qdbar=e(Hs1, m.nv) if compute_bars else None,
-            xbar=e(Hs1, m.nbody - 1, 3) if compute_bars else None,
+            qbar=e(*lead, Hs1, m.nq) if compute_bars else None, qdbar=e(*lead, Hs1, m.nv) if compute_bars else None,
+            xbar=e(*lead, Hs1, m.nbody - 1, 3) if compute_bars else None,
             noise=(mbdpi.schedule(nmax) if noise is None else f(noise)).contiguous())
         assert tuple(self.buf["noise"].shape) == (nmax, a.Hnode + 1) or self.buf["noise"].shape[0] >= nmax
         self.n_diffuse_max = nmax
         # randomize_tasks: host mirror of info["step"] / info["rng"] (the env's key chain), from which
         # the one-step random command the horizon may reach is computed ahead (BaseEnv.command_override)
-        self._rand = bool(state.info.get("randomize_target", False))
-        self._env_info = {"randomize_target": self._rand, "step": int(state.info.get("step", 0)),
-                          "rng": np.asarray(state.info.get("rng", np.zeros(2)), dtype=np.uint32).copy()}
+        s0 = states[0]
+        self._rand = bool(s0.info.get("randomize_target", False))
+        self._env_info = {"randomize_target": self._rand, "step": int(s0.info.get("step", 0)),
+                          "rng": np.asarray(s0.info.get("rng", np.zeros(2)), dtype=np.uint32).copy()}
         if self._rand and hasattr(mbdpi.env, "stage_tables"):
             # seq-jump: the jump sequence drawn at reset is constant afterwards; one upload at bind time
-            pl.set_stages(mbdpi.env.stage_tables(state.info))
+            pl.set_stages(mbdpi.env.stage_tables(s0.info))
         pl.mpc_bind(self.buf, mbdpi.M_shift.cpu().numpy())
 
     def step(self, n_diffuse: Optional[int] = None, env_step=True) -> None:
@@ -343,19 +377,22 @@ class DeviceLoop:
     def set_state(self, qpos, qvel, qacc_warmstart=None, step: Optional[int] = None) -> None:
         """Overwrite the planning state (deploy: the state comes from the robot / simulator).  ``step``
         sets ``info["step"]`` only, like the reference's ``update_mjx_state`` (dial_plan.py:149-155):
-        a seq-jump ``contact_stage`` is whatever the bound state carries."""
+        a seq-jump ``contact_stage`` is whatever the bound state carries.  Batched loops: [B,...]
+        arrays and ``step`` an int or [B]."""
         self.buf["qpos"].copy_(self.plan.f32(qpos))
         self.buf["qvel"].copy_(self.plan.f32(qvel))
         if qacc_warmstart is not None:
             self.buf["qacc_warmstart"].copy_(self.plan.f32(qacc_warmstart))
-        if step is not None:
+        if step is not None and self.n_instances > 1:
+            self.buf["counters"][:, 0] = torch.as_tensor(np.asarray(step, dtype=np.int32), device=self.buf["counters"].device)
+        elif step is not None:
             self.buf["counters"][0] = int(step)
             self._env_info["step"] = int(step)
 
     @property
     def action(self) -> torch.Tensor:
-        """``Y0[0]``: the action the next env step applies (device view)."""
-        return self.buf["Y"][0]
+        """``Y0[0]``: the action the next env step applies (device view; batched: [B,nu])."""
+        return self.buf["Y"][:, 0] if self.n_instances > 1 else self.buf["Y"][0]
 
     @property
     def Y(self) -> torch.Tensor:
@@ -363,7 +400,7 @@ class DeviceLoop:
 
     @property
     def reward(self) -> torch.Tensor:
-        return self.buf["reward"][0]
+        return self.buf["reward"] if self.n_instances > 1 else self.buf["reward"][0]
 
     def info(self) -> Dict[str, Any]:
         b = self.buf
@@ -372,18 +409,25 @@ class DeviceLoop:
             d.update(qbar=b["qbar"], qdbar=b["qdbar"], xbar=b["xbar"])
         return d
 
-    def state(self):
-        """Materialise the env ``State`` (synchronises: reads the counters)."""
+    def state(self, i: Optional[int] = None):
+        """Materialise the env ``State`` (synchronises: reads the counters); batched loops: that of
+        instance ``i``."""
         from dial_mpc_b200.envs.base_env import PipelineState, State
-        b = self.buf
+        if self.n_instances > 1:
+            if i is None:
+                raise ValueError("a batched DeviceLoop materialises one instance: state(i)")
+            b = {k: (t[i] if t is not None and k != "noise" else t) for k, t in self.buf.items()}
+            info0, r = self.info0[i], b["reward"]
+        else:
+            b, info0, r = self.buf, self.info0, self.buf["reward"][0]
         c = b["counters"].cpu().numpy()
-        info = dict(self.info0)
+        info = dict(info0)
         info["step"] = int(c[0])
         if "contact_stage" in info:
             info["contact_stage"] = int(c[1])
         info["rng"] = b["rng"].cpu().numpy().view(np.uint32).copy()
         ps = PipelineState(b["qpos"].clone(), b["qvel"].clone(), b["qacc_warmstart"].clone(), b["ctrl"].clone())
-        return State(ps, None, b["reward"][0].clone(), 0.0, {}, info)
+        return State(ps, None, r.clone(), 0.0, {}, info)
 
 
 def save_run(output_dir, rollout, infos, timestamp=None):
@@ -401,6 +445,37 @@ def save_run(output_dir, rollout, infos, timestamp=None):
     return states, preds
 
 
+def run_instances(dial_config, env, B, Nstep):
+    """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
+    plain run with seed ``dial_config.seed + b``."""
+    mbdpi = MBDPI(dial_config, env, n_instances=B)
+    states, rngs = [], []
+    for b in range(B):
+        rng, rng_reset = drandom.split(drandom.PRNGKey(seed=dial_config.seed + b))
+        states.append(env.reset(rng_reset))
+        rngs.append(drandom.split(rng)[1])
+    loop = DeviceLoop(mbdpi, states, np.stack(rngs))
+    buf = loop.buf
+    rews, rollout, infos = [], [], []
+    t0, tlast = time.time(), -1
+    for t in range(Nstep):
+        loop.step(dial_config.Ndiffuse_init if t == 0 else dial_config.Ndiffuse)
+        tt = torch.full((B, 1), float(t), device=mbdpi.device)
+        rollout.append(torch.cat([tt, buf["qpos"], buf["qvel"], buf["ctrl"]], 1))
+        rews.append(buf["reward"].clone())
+        infos.append(buf["xbar"].clone())
+        if t % 10 == 0:
+            r = rews[-1].cpu().numpy()   # synchronises
+            print(f"step {t}: rew={r.mean():.3e} (min {r.min():.3e}, max {r.max():.3e} over {B} instances) "
+                  f"freq={(t - tlast) / (time.time() - t0):.1f} Hz")
+            t0, tlast = time.time(), t
+    rew = torch.stack(rews).mean(0).cpu().numpy()
+    print("mean reward per instance = " + " ".join(f"{r:.2e}" for r in rew))
+    timestamp = time.strftime("%Y%m%d-%H%M%S")
+    for b in range(B):
+        save_run(dial_config.output_dir, [r[b] for r in rollout], [x[b] for x in infos], timestamp=f"{timestamp}_inst{b}")
+
+
 def main():
     """Synchronous MPC loop — dial_core.py:175-268 without the rendering / flask tail."""
     parser = argparse.ArgumentParser()
@@ -412,6 +487,9 @@ def main():
     parser.add_argument("--n-steps", type=int, default=None)
     parser.add_argument("--eager", action="store_true",
                         help="per-call launches (env.step / reverse_scan) instead of the CUDA-graph loop")
+    parser.add_argument("--instances", type=int, default=1,
+                        help="run this many independent closed loops in one CUDA graph per control step; instance b "
+                             "resets from PRNGKey(seed + b) and writes its output files under the prefix <time>_inst<b>")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -427,10 +505,17 @@ def main():
     else:
         config_dict = yaml.safe_load(open(args.config))
     dial_config = load_dataclass_from_dict(DialConfig, config_dict)
+    if args.instances < 1:
+        parser.error("--instances must be at least 1")
+    if args.instances > 1 and args.eager:
+        parser.error("--instances runs on the CUDA-graph loop; it excludes --eager")
     rng = drandom.PRNGKey(seed=dial_config.seed)
     env_config_type = dial_envs.get_config(dial_config.env_name)
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
     env = dial_envs.get_environment(dial_config.env_name, config=env_config)
+    if args.instances > 1:
+        run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps)
+        return
     mbdpi = MBDPI(dial_config, env)
     rng, rng_reset = drandom.split(rng)
     state = env.reset(rng_reset)

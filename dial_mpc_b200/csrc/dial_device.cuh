@@ -121,10 +121,15 @@ struct RolloutArgs {
   int32_t lockstep;     // >=1: warps of a CTA re-converge at every env step (shared instruction fetch); 2: and before the Newton loop
   int32_t sync_every;   // lock-step barrier every this many env steps (>= 1)
   int32_t step0, stage0;
+  // batched plans (dial_plan_desc.n_inst > 1): rows [b * rows_per_inst, (b+1) * rows_per_inst) belong to
+  // instance b, whose state / counters / rng / key / Ybar and final-state outputs sit at instance-major
+  // offsets of the pointers below; per-row outputs are indexed by the global row.  0: one instance.
+  int32_t rows_per_inst;
+  int32_t us_row;       // floats between the action rows of `us` (mode 0); 0: H * nu
   const float* qpos0;
   const float* qvel0;
   const float* warm0;
-  const float* us;      // [nrows,H,nu]               (mode 0)
+  const float* us;      // [nrows,H,nu]               (mode 0), rows us_row floats apart
   const float* eps;     // [Ntotal,Hn+1,nu] or null   (mode 1)
   const float* Ybar;    // [Hn+1,nu]
   const float* noise;   // [Hn+1]
@@ -2821,6 +2826,9 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
   const dial_model_desc& m = M.m;
   const dial_plan_desc& c = Pp->c;
   const int nq = m.nq, nv = m.nv, nu = m.nu, nb = m.nbody;
+  // instance of a batched launch and the row inside it (the sample index)
+  const int inst = A.rows_per_inst > 0 ? row / A.rows_per_inst : 0;
+  const int lrow = row - inst * A.rows_per_inst;
   // ancestor chain of this lane's dof
   w.nch = 0; w.ndesc = 0; w.mylevel = -1; w.parent = -1;
 #pragma unroll
@@ -2852,8 +2860,8 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
     for (int i = lane; i < 32; i += 32) SM(frow)[i] = 0.f;
   }
   // initial state + world body constants
-  for (int i = lane; i < nq; i += 32) SM(qpos)[i] = A.qpos0[i];
-  for (int i = lane; i < nv; i += 32) { SM(qvel)[i] = A.qvel0[i]; SM(warm)[i] = A.warm0[i]; }
+  for (int i = lane; i < nq; i += 32) SM(qpos)[i] = A.qpos0[(size_t)inst * nq + i];
+  for (int i = lane; i < nv; i += 32) { SM(qvel)[i] = A.qvel0[(size_t)inst * nv + i]; SM(warm)[i] = A.warm0[(size_t)inst * nv + i]; }
   if (lane == 0) {
     SM(xpos)[0] = SM(xpos)[1] = SM(xpos)[2] = 0.f;
     SM(xquat)[0] = 1.f; SM(xquat)[1] = SM(xquat)[2] = SM(xquat)[3] = 0.f;
@@ -2872,15 +2880,15 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
 #pragma unroll
   for (int k = 0; k < DIAL_MAXNODE; ++k) Y[k] = 0.f;
   if (A.mode == 1 && lane < nu) {
-    const bool is_mean = row == c.Nsample;
-    const uint32_t gidx = (uint32_t)(c.shard_offset + row);
+    const bool is_mean = lrow == c.Nsample;
+    const uint32_t gidx = (uint32_t)(c.shard_offset + lrow);
     const uint32_t ntot = (uint32_t)c.Ntotal * (uint32_t)Hn1 * (uint32_t)nu;
-    uint32_t key0 = A.key_dev ? A.key_dev[0] : A.key0, key1 = A.key_dev ? A.key_dev[1] : A.key1;
-    if (A.rng_dev) split_key(A.rng_dev[0], A.rng_dev[1], key0, key1);
+    uint32_t key0 = A.key_dev ? A.key_dev[2 * inst] : A.key0, key1 = A.key_dev ? A.key_dev[2 * inst + 1] : A.key1;
+    if (A.rng_dev) split_key(A.rng_dev[2 * inst], A.rng_dev[2 * inst + 1], key0, key1);
 #pragma unroll
     for (int k = 0; k < DIAL_MAXNODE; ++k) {
       if (k < Hn1) {
-        float yb = A.Ybar[k * nu + lane];
+        float yb = A.Ybar[(inst * Hn1 + k) * nu + lane];
         float y = yb;
         if (!is_mean && k > 0) {
           uint32_t idx = (gidx * (uint32_t)Hn1 + (uint32_t)k) * (uint32_t)nu + (uint32_t)lane;
@@ -2892,7 +2900,7 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
     }
   }
 
-  int step = A.counters_in ? A.counters_in[0] : A.step0, stage = A.counters_in ? A.counters_in[1] : A.stage0;
+  int step = A.counters_in ? A.counters_in[2 * inst] : A.step0, stage = A.counters_in ? A.counters_in[2 * inst + 1] : A.stage0;
   float rsum = 0.f;
   const bool fwd_only = A.mode == 2;  // pipeline_init: mjx.forward only, zero ctrl
   const int H = fwd_only ? 1 : A.H;
@@ -2904,7 +2912,7 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
     if (lane < nu && !fwd_only) {
       float u;
       if (A.mode == 0) {
-        u = A.us[((size_t)row * A.H + t) * nu + lane];
+        u = A.us[(size_t)row * (A.us_row ? A.us_row : A.H * nu) + t * nu + lane];
       } else {
         u = 0.f;
 #pragma unroll
@@ -2951,18 +2959,24 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
       if (sample || p == A.xch_rank) A.xch_mbox[p][slot] = val;
   }
 #endif
-  if (row == 0) {
-    if (A.qpos_out) for (int i = lane; i < nq; i += 32) A.qpos_out[i] = SM(qpos)[i];
-    if (A.qvel_out) for (int i = lane; i < nv; i += 32) A.qvel_out[i] = SM(qvel)[i];
-    if (A.warm_out) for (int i = lane; i < nv; i += 32) A.warm_out[i] = SM(warm)[i];
-    if (A.ctrl_out) for (int i = lane; i < nu; i += 32) A.ctrl_out[i] = SM(ctrl)[i];
+  // final state of each instance's first row.  The instance is derived again from a shuffled copy of
+  // `row`, which the compiler cannot equate with the prologue's: inst / lrow are not kept live over
+  // the env-step loop (two registers the star kernels do not have to spare).
+  const int erow = shfl_i(row, 0), einst = A.rows_per_inst > 0 ? erow / A.rows_per_inst : 0;
+  if (erow == einst * A.rows_per_inst) {
+    const int inst = einst;
+    if (A.qpos_out) for (int i = lane; i < nq; i += 32) A.qpos_out[(size_t)inst * nq + i] = SM(qpos)[i];
+    if (A.qvel_out) for (int i = lane; i < nv; i += 32) A.qvel_out[(size_t)inst * nv + i] = SM(qvel)[i];
+    if (A.warm_out) for (int i = lane; i < nv; i += 32) A.warm_out[(size_t)inst * nv + i] = SM(warm)[i];
+    if (A.ctrl_out) for (int i = lane; i < nu; i += 32) A.ctrl_out[(size_t)inst * nu + i] = SM(ctrl)[i];
     if (A.kin_out && lane == 0) {   // what the envs' _get_obs reads of pipeline_state.x / xd (kinematics of the last forward pass)
       const BaseKin bk = base_kin(w, c.torso_body);
-      A.kin_out[0] = bk.pos.x; A.kin_out[1] = bk.pos.y; A.kin_out[2] = bk.pos.z;
-      A.kin_out[3] = bk.rot.w; A.kin_out[4] = bk.rot.x; A.kin_out[5] = bk.rot.y; A.kin_out[6] = bk.rot.z;
-      A.kin_out[7] = bk.vb.x; A.kin_out[8] = bk.vb.y; A.kin_out[9] = bk.vb.z;
-      A.kin_out[10] = bk.ab.x; A.kin_out[11] = bk.ab.y; A.kin_out[12] = bk.ab.z;
+      float* ko = A.kin_out + 13 * inst;
+      ko[0] = bk.pos.x; ko[1] = bk.pos.y; ko[2] = bk.pos.z;
+      ko[3] = bk.rot.w; ko[4] = bk.rot.x; ko[5] = bk.rot.y; ko[6] = bk.rot.z;
+      ko[7] = bk.vb.x; ko[8] = bk.vb.y; ko[9] = bk.vb.z;
+      ko[10] = bk.ab.x; ko[11] = bk.ab.y; ko[12] = bk.ab.z;
     }
-    if (A.counters_out && lane == 0) { A.counters_out[0] = step; A.counters_out[1] = stage; }
+    if (A.counters_out && lane == 0) { A.counters_out[2 * inst] = step; A.counters_out[2 * inst + 1] = stage; }
   }
 }

@@ -286,6 +286,8 @@ __global__ void __launch_bounds__(YBAR_THREADS) ybar_kernel(const float* __restr
 // divides, normalises the stored weights, and advances the planner rng.  Two graph nodes fewer per
 // reverse_once (a launch boundary inside a graph costs about a microsecond, so this is about graph
 // size and the host-visible weights dependency more than time).
+// Batched plans: blockIdx.y is the instance; each instance runs the single-instance grid on its own
+// slices of rews / weights / rng / Ybar / partials / counter, so its arithmetic and order are unchanged.
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __restrict__ rews, int n, float temp,
                                                                float* __restrict__ weights, const XchWait X,
@@ -297,6 +299,11 @@ __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __res
   __shared__ float acc[YBAR_THREADS];
   __shared__ bool is_last;
   const int tid = threadIdx.x;
+  {
+    const size_t b = blockIdx.y, ne1 = (size_t)Hn1 * nu;
+    rews += b * n; weights += b * n; rng += 2 * b; Ybar += b * ne1; Ybar_out += b * ne1;
+    partial += b * gridDim.x * (ne1 + 1); counter += b;
+  }
   if (X.mbox) {
     const uint32_t seq = *X.seq, buf = seq & 1u;
     xch_wait_flags(X.flags + buf * DIAL_MAXRANK, seq + 1u, X.world, X.err, blockIdx.x == 0 ? X.err + 2 : nullptr);
@@ -397,10 +404,11 @@ __global__ void mpc_split_kernel(uint32_t* __restrict__ rng, uint32_t* __restric
 }
 
 // Y <- shift(Y) = u2node(roll(node2u(Y), -1), last row 0)  (dial_core.py:160-165) as one constant
-// (Hn+1)x(Hn+1) matrix; one thread per output element
+// (Hn+1)x(Hn+1) matrix; one thread per output element, one CTA per instance
 __global__ void mpc_shift_kernel(const float* __restrict__ Msh, const float* __restrict__ Yin,
                                  float* __restrict__ Yout, int n1, int nu) {
   const int i = threadIdx.x;
+  Yin += (size_t)blockIdx.x * n1 * nu; Yout += (size_t)blockIdx.x * n1 * nu;
   if (i < n1 * nu) {
     const int k = i / nu, a = i - k * nu;
     float s = 0.f;
@@ -416,6 +424,8 @@ __global__ void mpc_shift_kernel(const float* __restrict__ Msh, const float* __r
 //   stage 1: grid (ceil(max_j / 256), TB_CHUNKS row chunks, 3 arrays): per-chunk partials, rows in
 //            order, 8 independent loads in flight per thread
 //   stage 2: grid H: partials summed in fixed chunk order (bitwise deterministic)
+// Batched plans add an instance dimension (stage 1: z = 3 * instance + array, stage 2: y = instance)
+// over instance-major trajectories, weights, partials and outputs.
 // The only bandwidth-shaped kernel of the path: rows * H * (nq + nv + 3 (nbody-1)) * 4 bytes read
 // once from L2 / HBM (cfg1: 16 MB, cfg4 shard: 65 MB).
 // ---------------------------------------------------------------------------------
@@ -431,13 +441,17 @@ struct TrajArgs {
 };
 
 // (32 registers: one CTA fits beside the 448-thread rollout CTA of the next iteration, which the bars overlap)
+// BATCH = false (single-instance plans) compiles to the instance-free code: the bars of a plain plan
+// pay nothing for the instance dimension
+template <bool BATCH>
 __global__ void __launch_bounds__(256, 8) trajbar_partial_kernel(const TrajArgs T) {
-  const int chunk = blockIdx.y, arr = blockIdx.z;
+  const int chunk = blockIdx.y, arr = BATCH ? blockIdx.z % 3 : blockIdx.z, inst = BATCH ? blockIdx.z / 3 : 0;
   const int ncol = arr == 0 ? T.ncol[0] : (arr == 1 ? T.ncol[1] : T.ncol[2]), len = T.H * ncol;
   const int coloff = arr == 0 ? T.coloff[0] : (arr == 1 ? T.coloff[1] : T.coloff[2]);
   const int j = blockIdx.x * 256 + threadIdx.x;
   if (blockIdx.x * 256 >= len) return;
-  const float* __restrict__ traj = arr == 0 ? T.traj[0] : (arr == 1 ? T.traj[1] : T.traj[2]);
+  const float* __restrict__ traj = (arr == 0 ? T.traj[0] : (arr == 1 ? T.traj[1] : T.traj[2])) + (size_t)inst * T.nrows * len;
+  const float* wts = BATCH ? T.weights + (size_t)inst * (T.mean_weight_index + 1) : T.weights;
   const int per = (T.nrows + TB_CHUNKS - 1) / TB_CHUNKS;
   const int r0 = chunk * per, r1 = min(T.nrows, r0 + per);
   const int jj = j < len ? j : len - 1;
@@ -449,8 +463,8 @@ __global__ void __launch_bounds__(256, 8) trajbar_partial_kernel(const TrajArgs 
       const int rr = r + k;
       float wgt = 0.f;
       if (rr < r1) {
-        if (rr == T.mean_row) wgt = T.include_mean ? T.weights[T.mean_weight_index] : 0.f;
-        else wgt = T.weights[T.w_offset + rr];
+        if (rr == T.mean_row) wgt = T.include_mean ? wts[T.mean_weight_index] : 0.f;
+        else wgt = wts[T.w_offset + rr];
       }
       wv[k] = wgt;
     }
@@ -462,21 +476,23 @@ __global__ void __launch_bounds__(256, 8) trajbar_partial_kernel(const TrajArgs 
   }
   if (j < len) {
     const int t = j / ncol, c = j - t * ncol;
-    T.partial[((size_t)chunk * T.H + t) * T.coltot + coloff + c] = a;
+    T.partial[(((size_t)inst * TB_CHUNKS + chunk) * T.H + t) * T.coltot + coloff + c] = a;
   }
 }
 
+template <bool BATCH>
 __global__ void __launch_bounds__(128, 8) trajbar_final_kernel(const TrajArgs T) {
-  const int t = blockIdx.x;
+  const int t = blockIdx.x, inst = BATCH ? blockIdx.y : 0;
+  const float* partial = T.partial + (size_t)inst * TB_CHUNKS * T.H * T.coltot;
   for (int col = threadIdx.x; col < T.coltot; col += blockDim.x) {
     float s = 0.f;
 #pragma unroll 8
-    for (int ch = 0; ch < TB_CHUNKS; ++ch) s += T.partial[((size_t)ch * T.H + t) * T.coltot + col];
+    for (int ch = 0; ch < TB_CHUNKS; ++ch) s += partial[((size_t)ch * T.H + t) * T.coltot + col];
     float* out; int ncol, off;   // (no dynamic indexing of the kernel parameter: it would be copied to the stack)
     if (col >= T.coloff[2]) { out = T.out[2]; ncol = T.ncol[2]; off = T.coloff[2]; }
     else if (col >= T.coloff[1]) { out = T.out[1]; ncol = T.ncol[1]; off = T.coloff[1]; }
     else { out = T.out[0]; ncol = T.ncol[0]; off = T.coloff[0]; }
-    if (out) out[(size_t)t * ncol + (col - off)] = s;
+    if (out) out[((size_t)inst * T.H + t) * ncol + (col - off)] = s;
   }
 }
 
@@ -489,6 +505,7 @@ struct dial_plan {
   DevModel* dM = nullptr;
   DevPlan* dP = nullptr;
   int variant = 0;
+  int n_inst = 1;               // independent planner instances (dial_plan_desc.n_inst)
   int num_sms = 132;
   size_t smem_bytes = 0;
   // workspaces
@@ -671,6 +688,16 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
   }
 #endif
   if (c.n_user < 0 || c.n_user > DIAL_MAXUSER) { g_err = "n_user out of range"; delete p; return nullptr; }
+  if (c.n_inst < 0) { g_err = "n_inst must be >= 0 (0 or 1: a single instance)"; delete p; return nullptr; }
+  if (c.n_inst > 1) {
+    if (c.Ntotal != c.Nsample) { g_err = "a batched plan (n_inst > 1) cannot be sharded (Ntotal must equal Nsample)"; delete p; return nullptr; }
+    if (c.Nsample + 1 > (1 << 17)) { g_err = "a batched plan (n_inst > 1) needs Nsample + 1 <= 131072 (the fused update)"; delete p; return nullptr; }
+    // the instance is grid dimension z / 3 of the bars kernel (<= 65535) and rows are int32
+    if (c.n_inst > 65535 / 3 || (int64_t)c.n_inst * (c.Nsample + 1) > 0x7fffffff) {
+      g_err = "n_inst too large: at most 21845 instances and 2^31 - 1 rows per rollout launch"; delete p; return nullptr;
+    }
+  }
+  p->n_inst = c.n_inst > 1 ? c.n_inst : 1;
   auto bad = [&](cudaError_t e, const char* what) {
     g_err = std::string(what) + ": " + cudaGetErrorString(e);
     dial_plan_destroy(p);
@@ -681,15 +708,15 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
   if ((e = cudaMalloc(&p->dP, sizeof(DevPlan))) != cudaSuccess) return bad(e, "cudaMalloc(plan)");
   if ((e = cudaMemcpy(p->dM, &p->hM, sizeof(DevModel), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(model)");
   if ((e = cudaMemcpy(p->dP, &p->hP, sizeof(DevPlan), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(plan)");
-  const size_t rows = (size_t)c.Nsample + 1, H = (size_t)c.Hsample + 1;
+  const size_t B = (size_t)p->n_inst, rows = B * ((size_t)c.Nsample + 1), H = (size_t)c.Hsample + 1;
   const dial_model_desc& m = *model;
   for (int b = 0; b < 2; ++b) {
     if ((e = cudaMalloc(&p->traj_q[b], rows * H * m.nq * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_q)");
     if ((e = cudaMalloc(&p->traj_qd[b], rows * H * m.nv * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_qd)");
     if ((e = cudaMalloc(&p->traj_x[b], rows * H * 3 * (m.nbody - 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_x)");
   }
-  if ((e = cudaMalloc(&p->weights, ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
-  if ((e = cudaMalloc(&p->weights2, ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
+  if ((e = cudaMalloc(&p->weights, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
+  if ((e = cudaMalloc(&p->weights2, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
   if ((e = cudaStreamCreateWithFlags(&p->side, cudaStreamNonBlocking)) != cudaSuccess) return bad(e, "cudaStreamCreate(side)");
   for (int i = 0; i < 2; ++i) {
     if ((e = cudaEventCreateWithFlags(&p->ev_main[i], cudaEventDisableTiming)) != cudaSuccess) return bad(e, "cudaEventCreate");
@@ -702,10 +729,10 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     int gu = (c.Ntotal + 1 + slots * 8 - 1) / (slots * 8);
     p->upd_grid = gu < 1 ? 1 : (gu > p->ybar_grid ? p->ybar_grid : gu);
   }
-  if ((e = cudaMalloc(&p->partial, (size_t)p->ybar_grid * (ne + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(partial)");
-  if ((e = cudaMalloc(&p->tb_partial, (size_t)TB_CHUNKS * H * (m.nq + m.nv + 3 * (m.nbody - 1)) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(tb_partial)");
-  if ((e = cudaMalloc(&p->counter, sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMalloc(counter)");
-  if ((e = cudaMemset(p->counter, 0, sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMemset(counter)");
+  if ((e = cudaMalloc(&p->partial, B * p->ybar_grid * (ne + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(partial)");
+  if ((e = cudaMalloc(&p->tb_partial, B * TB_CHUNKS * H * (m.nq + m.nv + 3 * (m.nbody - 1)) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(tb_partial)");
+  if ((e = cudaMalloc(&p->counter, B * sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMalloc(counter)");
+  if ((e = cudaMemset(p->counter, 0, B * sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMemset(counter)");
   if ((e = cudaMalloc(&p->row_counter, sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMalloc(row_counter)");
   if (getenv("DIAL_DEBUG_COUNTERS")) {
     if ((e = cudaMalloc(&p->dbg, 8 * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(dbg)");
@@ -813,6 +840,7 @@ extern "C" int dial_pipeline_init(dial_plan* p, const float* qpos, const float* 
 extern "C" int dial_reverse_rollout(dial_plan* p, const dial_state* s, const float* eps, const uint32_t key[2],
                                     const float* Ybar, const float* noise_scale, float* rews_local, void* stream) {
   if (!p || !s || !Ybar || !noise_scale || !rews_local) return fail("dial_reverse_rollout: null argument");
+  if (p->n_inst > 1) return fail("dial_reverse_rollout: batched plans run through dial_mpc_step");
   if (!eps && !key) return fail("dial_reverse_rollout: need eps or key");
   RolloutArgs A; memset(&A, 0, sizeof(A));
   fill_state(A, s);
@@ -838,6 +866,7 @@ extern "C" int dial_reverse_update_x(dial_plan* p, const float* eps, const uint3
                                      const float* noise_scale, const float* rews_all, float* Ybar_out,
                                      float* weights, float* rews_gathered, void* stream) {
   if (!p || !Ybar || !noise_scale || !Ybar_out) return fail("dial_reverse_update: null argument");
+  if (p->n_inst > 1) return fail("dial_reverse_update: batched plans run through dial_mpc_step");
   if (!rews_all && !p->xch.on) return fail("dial_reverse_update: rews_all may be NULL only with a connected exchange");
   if (!eps && !key) return fail("dial_reverse_update: need eps or key");
   const dial_plan_desc& c = p->hP.c;
@@ -859,12 +888,11 @@ extern "C" int dial_reverse_update_x(dial_plan* p, const float* eps, const uint3
   return 0;
 }
 
-extern "C" int dial_reverse_trajbar(dial_plan* p, const float* weights, int rank, float* qbar, float* qdbar,
-                                    float* xbar, void* stream) {
-  if (!p) return fail("dial_reverse_trajbar: null plan");
+// the bars of every instance of the plan (the control-step graph; the public call below is single-instance)
+static int enqueue_trajbar(dial_plan* p, const float* weights, int rank, float* qbar, float* qdbar, float* xbar,
+                           cudaStream_t st) {
   const dial_plan_desc& c = p->hP.c;
   const dial_model_desc& m = p->hM.m;
-  cudaStream_t st = (cudaStream_t)stream;
   const float* w = weights ? weights : p->weights;
   const int H = c.Hsample + 1, rows = c.Nsample + 1;
   TrajArgs T;
@@ -880,10 +908,13 @@ extern "C" int dial_reverse_trajbar(dial_plan* p, const float* weights, int rank
   T.nrows = rows; T.H = H; T.weights = w; T.w_offset = c.shard_offset; T.mean_row = c.Nsample;
   T.mean_weight_index = c.Ntotal; T.include_mean = rank == 0 ? 1 : 0; T.partial = p->tb_partial;
   const int maxlen = H * (T.ncol[2] > T.ncol[0] ? T.ncol[2] : T.ncol[0]);   // nq = nv + 1 > nv always
-  trajbar_partial_kernel<<<dim3((maxlen + 255) / 256, TB_CHUNKS, 3), 256, 0, st>>>(T);
+  const dim3 g1((maxlen + 255) / 256, TB_CHUNKS, 3 * p->n_inst), g2(H, p->n_inst);
+  if (p->n_inst > 1) trajbar_partial_kernel<true><<<g1, 256, 0, st>>>(T);
+  else trajbar_partial_kernel<false><<<g1, 256, 0, st>>>(T);
   p->launches++;
   CUDA_OK(cudaGetLastError());
-  trajbar_final_kernel<<<H, 128, 0, st>>>(T);
+  if (p->n_inst > 1) trajbar_final_kernel<true><<<g2, 128, 0, st>>>(T);
+  else trajbar_final_kernel<false><<<g2, 128, 0, st>>>(T);
   p->launches++;
   CUDA_OK(cudaGetLastError());
   if (xsum) {
@@ -897,6 +928,13 @@ extern "C" int dial_reverse_trajbar(dial_plan* p, const float* weights, int rank
     CUDA_OK(cudaGetLastError());
   }
   return 0;
+}
+
+extern "C" int dial_reverse_trajbar(dial_plan* p, const float* weights, int rank, float* qbar, float* qdbar,
+                                    float* xbar, void* stream) {
+  if (!p) return fail("dial_reverse_trajbar: null plan");
+  if (p->n_inst > 1) return fail("dial_reverse_trajbar: batched plans run through dial_mpc_step");
+  return enqueue_trajbar(p, weights, rank, qbar, qdbar, xbar, (cudaStream_t)stream);
 }
 
 // ---- multi-GPU exchange over NVLink peer memory -------------------------------------------------
@@ -956,6 +994,7 @@ extern "C" int dial_exchange_status(dial_plan* p, uint32_t out[6]) {
 
 extern "C" int dial_reverse_trajectories(dial_plan* p, float* q, float* qd, float* xpos, void* stream) {
   if (!p) return fail("dial_reverse_trajectories: null plan");
+  if (p->n_inst > 1) return fail("dial_reverse_trajectories: batched plans run through dial_mpc_step");
   const dial_plan_desc& c = p->hP.c;
   const dial_model_desc& m = p->hM.m;
   const size_t n = ((size_t)c.Nsample + 1) * (c.Hsample + 1) * sizeof(float);
@@ -976,11 +1015,12 @@ extern "C" int dial_mpc_bind(dial_plan* p, const dial_mpc_buffers* b, const floa
   if (c.Ntotal != c.Nsample && !p->xch.on)
     return fail("dial_mpc_bind: a sharded plan needs a connected exchange (dial_exchange_create / dial_exchange_connect) for the device-resident loop");
   if (c.Ntotal != c.Nsample && !b->rews_all) return fail("dial_mpc_bind: sharded plans need rews_all [Ntotal+1]");
+  if (p->n_inst > 1 && b->rews_all) return fail("dial_mpc_bind: rews_all must be NULL on a batched plan");
   const int n1 = c.Hnode + 1, nu = p->hM.m.nu;
   for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   p->mpc_graphs.clear();
   if (!p->mpc_Msh) CUDA_OK(cudaMalloc(&p->mpc_Msh, DIAL_MAXNODE * DIAL_MAXNODE * sizeof(float)));
-  if (!p->mpc_Y1) CUDA_OK(cudaMalloc(&p->mpc_Y1, DIAL_MAXNODE * DIAL_MAXU * sizeof(float)));
+  if (!p->mpc_Y1) CUDA_OK(cudaMalloc(&p->mpc_Y1, (size_t)p->n_inst * DIAL_MAXNODE * DIAL_MAXU * sizeof(float)));
   if (!p->mpc_key) CUDA_OK(cudaMalloc(&p->mpc_key, 2 * sizeof(uint32_t)));
   CUDA_OK(cudaMemcpy(p->mpc_Msh, M_shift, (size_t)n1 * n1 * sizeof(float), cudaMemcpyHostToDevice));
   (void)nu;
@@ -993,21 +1033,24 @@ extern "C" int dial_mpc_bind(dial_plan* p, const dial_mpc_buffers* b, const floa
 static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t st) {
   const dial_plan_desc& c = p->hP.c;
   const dial_mpc_buffers& B = p->mpc;
-  const int n1 = c.Hnode + 1, nu = p->hM.m.nu;
+  const int n1 = c.Hnode + 1, nu = p->hM.m.nu, ni = p->n_inst;
+  const bool batched = ni > 1;
   float* Y[2] = {B.Y, p->mpc_Y1};
   int cur = 0;
   if (env_step == 1) {
-    // state = step_env(state, Y0[0])  (dial_core.py:245): in place, counters advanced by the kernel
+    // state = step_env(state, Y0[0])  (dial_core.py:245): in place, counters advanced by the kernel;
+    // batched: row b is instance b, its action Y[b][0]
     RolloutArgs A; memset(&A, 0, sizeof(A));
     A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart;
     A.counters_in = B.counters; A.counters_out = B.counters;
-    A.nrows = 1; A.H = 1; A.mode = 0; A.us = Y[cur]; A.rewss = B.reward;
+    A.nrows = ni; A.H = 1; A.mode = 0; A.us = Y[cur]; A.rewss = B.reward;
+    if (batched) { A.rows_per_inst = 1; A.us_row = n1 * nu; }
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
     CUDA_OK(launch_rollout(p, A, 1, st));
   }
   if (env_step == 1 || env_step == 2) {
     // Y0 = shift(Y0)  (dial_core.py:252)
-    mpc_shift_kernel<<<1, DIAL_MAXNODE * DIAL_MAXU, 0, st>>>(p->mpc_Msh, Y[cur], Y[cur ^ 1], n1, nu);
+    mpc_shift_kernel<<<ni, DIAL_MAXNODE * DIAL_MAXU, 0, st>>>(p->mpc_Msh, Y[cur], Y[cur ^ 1], n1, nu);
     p->launches++;
     CUDA_OK(cudaGetLastError());
     cur ^= 1;
@@ -1018,6 +1061,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
   // iteration i+1 rolls into the other pair; iteration i+2 waits for them.
   const bool bars = B.qbar && B.qdbar && B.xbar;
   float* wts[2] = {p->weights, p->weights2};
+  const size_t nw = (size_t)ni * (c.Ntotal + 1);   // weights of all instances
   for (int i = 0; i < n_diffuse; ++i) {
     const float* noise = B.noise + (size_t)i * n1;
     // rng split folded into the rollout (key = split(rng)[1]) and the fused update kernel (which also
@@ -1031,7 +1075,8 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     if (bars && i >= 2) CUDA_OK(cudaStreamWaitEvent(st, p->ev_side[i & 1], 0));
     RolloutArgs A; memset(&A, 0, sizeof(A));
     A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart; A.counters_in = B.counters;
-    A.nrows = c.Nsample + 1; A.H = c.Hsample + 1; A.mode = 1;
+    A.nrows = ni * (c.Nsample + 1); A.H = c.Hsample + 1; A.mode = 1;
+    if (batched) A.rows_per_inst = c.Nsample + 1;
     A.Ybar = Y[cur]; A.noise = noise;
     if (fused) A.rng_dev = B.rng; else A.key_dev = p->mpc_key;
     p->cur ^= 1;
@@ -1042,7 +1087,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     float* w = wts[i & 1];
     XchWait X = xch_wait_args(p, B.rews_all);
     if (fused) {
-      update_kernel<<<p->upd_grid, YBAR_THREADS, 0, st>>>(B.rews, c.Ntotal + 1, c.temp_sample, w, X, B.rng, Y[cur], noise, c.Ntotal,
+      update_kernel<<<dim3(p->upd_grid, ni), YBAR_THREADS, 0, st>>>(B.rews, c.Ntotal + 1, c.temp_sample, w, X, B.rng, Y[cur], noise, c.Ntotal,
                                                           n1, nu, p->partial, p->counter, Y[cur ^ 1]);
       p->launches++;
       CUDA_OK(cudaGetLastError());
@@ -1059,18 +1104,18 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     if (bars) {
       CUDA_OK(cudaEventRecord(p->ev_main[i & 1], st));
       CUDA_OK(cudaStreamWaitEvent(p->side, p->ev_main[i & 1], 0));
-      int rc = dial_reverse_trajbar(p, w, p->xch.on ? p->xch.rank : 0, B.qbar, B.qdbar, B.xbar, (void*)p->side);
+      int rc = enqueue_trajbar(p, w, p->xch.on ? p->xch.rank : 0, B.qbar, B.qdbar, B.xbar, p->side);
       if (rc) return rc;
       CUDA_OK(cudaEventRecord(p->ev_side[i & 1], p->side));
     }
   }
-  if (cur != 0) CUDA_OK(cudaMemcpyAsync(Y[0], Y[1], (size_t)n1 * nu * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (cur != 0) CUDA_OK(cudaMemcpyAsync(Y[0], Y[1], (size_t)ni * n1 * nu * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (bars && n_diffuse > 0) {   // join the bars branch (both outstanding iterations)
     if (n_diffuse >= 2) CUDA_OK(cudaStreamWaitEvent(st, p->ev_side[(n_diffuse - 2) & 1], 0));
     CUDA_OK(cudaStreamWaitEvent(st, p->ev_side[(n_diffuse - 1) & 1], 0));
   }
   if (n_diffuse > 0 && wts[(n_diffuse - 1) & 1] != p->weights)   // p->weights always holds the last iteration's weights
-    CUDA_OK(cudaMemcpyAsync(p->weights, p->weights2, ((size_t)c.Ntotal + 1) * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(p->weights, p->weights2, nw * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -1079,6 +1124,8 @@ extern "C" int dial_mpc_step(dial_plan* p, int n_diffuse, int env_step, void* st
   if (!p->mpc_bound) return fail("dial_mpc_step: call dial_mpc_bind first");
   if (n_diffuse < 0 || n_diffuse > 64) return fail("dial_mpc_step: n_diffuse out of range");
   if (env_step < 0 || env_step > 2) return fail("dial_mpc_step: env_step must be 0 (plan only), 1 (env step + shift) or 2 (shift only)");
+  // batched plans use the fused update only (plan creation guarantees Nsample + 1 <= 2^17)
+  if (p->n_inst > 1 && getenv("DIAL_NO_FUSED_UPDATE")) return fail("dial_mpc_step: batched plans need the fused update (unset DIAL_NO_FUSED_UPDATE)");
   cudaStream_t st = (cudaStream_t)stream;
   dial_plan::MpcGraph* g = nullptr;
   for (auto& e : p->mpc_graphs) if (e.n_diffuse == n_diffuse && e.env_step == env_step) g = &e;

@@ -149,7 +149,9 @@ class BaseEnv:
         raise NotImplementedError
 
     def plan_desc(self, Nsample=1, Hsample=1, Hnode=2, temp_sample=1.0, M_n2u=None,
-                  Ntotal=None, shard_offset=0) -> "_capi.dial_plan_desc":
+                  Ntotal=None, shard_offset=0, n_inst=1) -> "_capi.dial_plan_desc":
+        """``n_inst``: independent planner instances sharing this descriptor (batched control-step
+        graph, ``DeviceLoop`` on an ``MBDPI(..., n_instances=n_inst)``)."""
         d = _capi.dial_plan_desc()
         d.env_id = self.env_id
         d.Nsample, d.Ntotal, d.shard_offset = int(Nsample), int(Ntotal or Nsample), int(shard_offset)
@@ -172,6 +174,7 @@ class BaseEnv:
         if M_n2u is not None:
             _capi._set(d.M_n2u, M_n2u)
         d.cmd_step = -1
+        d.n_inst = int(n_inst)
         self._fill_reward_desc(d)
         return d
 

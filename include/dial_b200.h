@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define DIAL_ABI_VERSION 8
+#define DIAL_ABI_VERSION 9
 
 /* capacities of the fixed-size device model */
 #define DIAL_MAXB 24   /* bodies incl. world            */
@@ -131,6 +131,12 @@ typedef struct dial_plan_desc {
    * Set through dial_plan_set_command only (dial_plan_create ignores the value and starts at -1). */
   int32_t cmd_step;
   float cmd_vel[3], cmd_ang[3];
+  /* independent planner instances of one plan (0 or 1: a single instance).  B > 1 instances share
+   * the model, every constant above and the annealing schedule; each has its own state, counters,
+   * rng, control knots and outputs (see dial_mpc_buffers).  Batched plans run through dial_mpc_step
+   * only, with the fused update; they cannot be sharded (Ntotal == Nsample) and need
+   * Nsample + 1 <= 2^17. */
+  int32_t n_inst;
 } dial_plan_desc;
 
 /* State handed to the planner: Brax `State.pipeline_state` (qpos, qvel,
@@ -285,10 +291,16 @@ typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound 
   float* qdbar;           /* [Hs+1,nv]        reverse_once                                    */
   float* xbar;            /* [Hs+1,nbody-1,3]                                                 */
   const float* noise;     /* [>= n_diffuse][Hn+1] annealing schedule (dial_core.py:259-261)  */
+  /* Batched plans (n_inst = B > 1): every array above except noise gains a leading [B] dimension,
+   * instance-major: qpos [B,nq], qvel/qacc_warmstart [B,nv], counters [B,2], rng [B,2],
+   * Y [B,Hn+1,nu], ctrl [B,nu], reward [B], rews [B,Nsample+1], qbar [B,Hs+1,nq],
+   * qdbar [B,Hs+1,nv], xbar [B,Hs+1,nbody-1,3].  rews_all must be NULL.  Instance b's results are
+   * bitwise those of a single-instance plan bound to instance b's slices. */
 } dial_mpc_buffers;
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
- * (MBDPI.shift, core/dial_core.py:160-165).  Drops previously captured graphs. */
+ * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops
+ * previously captured graphs. */
 int dial_mpc_bind(dial_plan* plan, const dial_mpc_buffers* buffers, const float* M_shift);
 
 /* One control step on `stream`: [env_step == 1: state <- env.step(state, Y[0])], [env_step == 1
@@ -297,6 +309,11 @@ int dial_mpc_bind(dial_plan* plan, const dial_mpc_buffers* buffers, const float*
  * the robot); env_step = 2 shifts and plans without advancing the state (a planner whose state
  * is written by somebody else once per control period). */
 int dial_mpc_step(dial_plan* plan, int n_diffuse, int env_step, void* stream);
+/* A batched plan advances all B loops in the same graph: the env step rolls B rows, the shift runs
+ * one CTA per instance, every reverse_once is one rollout launch over B (Nsample+1) rows and one
+ * fused update launch over B instances.  DIAL_NO_FUSED_UPDATE is an error on a batched plan.  The
+ * eager dial_reverse_rollout / _update(_x) / _trajbar / _trajectories reject batched plans;
+ * dial_rollout, dial_env_step(_kin) and dial_pipeline_init keep their single-instance meaning. */
 
 /* jax.random.split(rng) / the planner's key threading (core/dial_core.py:106,145):
  * host-side Threefry-2x32; out[0] is the new rng, out[1] the sampling key. */
