@@ -66,6 +66,80 @@ dial_model_desc = _mk("dial_model_desc")
 dial_plan_desc = _mk("dial_plan_desc")
 dial_state = _mk("dial_state")
 dial_mpc_buffers = _mk("dial_mpc_buffers")
+dial_task = _mk("dial_task")
+
+TASK_FIELDS = tuple(name for name, _ in _STRUCTS["dial_task"])
+# the plan descriptor's task block has the layout of dial_task (a plan's own task is read through it)
+_T0 = getattr(dial_plan_desc, TASK_FIELDS[0]).offset
+if any(getattr(dial_plan_desc, f).offset - _T0 != getattr(dial_task, f).offset for f in TASK_FIELDS):
+    raise RuntimeError("include/dial_b200.h: the task block of dial_plan_desc does not have the layout of dial_task")
+
+
+def task_from_desc(d: dial_plan_desc) -> dial_task:
+    """The task fields of a plan descriptor (the reward inputs that differ between tasks), checked."""
+    t = dial_task()
+    for name in TASK_FIELDS:
+        v = getattr(d, name)
+        if isinstance(v, C.Array):
+            C.memmove(C.addressof(getattr(t, name)), C.addressof(v), C.sizeof(v))
+        else:
+            setattr(t, name, v)
+    return check_task(t)
+
+
+def task_set_command(t: dial_task, override):
+    """Write a randomize_tasks one-step command (``BaseEnv.command_override``: (step, vel[3], ang[3]) or
+    None) into ``t`` as ``dial_plan_set_command`` writes it into a plan; returns a key of the values."""
+    if override is None:
+        t.cmd_step = -1
+        _set(t.cmd_vel, np.zeros(3, np.float32))
+        _set(t.cmd_ang, np.zeros(3, np.float32))
+        return None
+    vel, ang = np.float32(override[1]).reshape(3), np.float32(override[2]).reshape(3)
+    t.cmd_step = int(override[0])
+    _set(t.cmd_vel, vel)
+    _set(t.cmd_ang, ang)
+    return (int(override[0]), tuple(vel.tolist()), tuple(ang.tolist()))
+
+
+def task_set_stages(t: dial_task, tables) -> dial_task:
+    """Write a jump sequence (pose [n,3], yaw [n], contact_targets [n,4,3], contact_radius [n,4]) into
+    ``t`` as ``dial_plan_set_stages`` writes it into a plan (unused rows zeroed)."""
+    pose, yaw, tgt, rad = (np.ascontiguousarray(x, dtype=np.float32) for x in tables)
+    n = int(pose.shape[0])
+    if not 1 <= n <= DEFINES["DIAL_MAXSTAGE"]:
+        raise ValueError(f"a jump sequence of {n} stages is out of range (1..{DEFINES['DIAL_MAXSTAGE']})")
+    if yaw.shape != (n,) or tgt.shape != (n, 4, 3) or rad.shape != (n, 4):
+        raise ValueError("stage tables must have shapes [n,3], [n], [n,4,3], [n,4]")
+    t.n_stage = n
+    for name, v in (("pose_seq", pose), ("yaw_seq", yaw), ("contact_targets", tgt), ("contact_radius", rad)):
+        np.ctypeslib.as_array(getattr(t, name))[...] = 0
+        _set(getattr(t, name), v)
+    return t
+
+
+def first_shared_difference(a: dial_plan_desc, b: dial_plan_desc) -> Optional[str]:
+    """The first field outside the task (shared by every instance of a plan) in which two plan
+    descriptors differ, or None."""
+    for name, _ in dial_plan_desc._fields_:
+        if name in TASK_FIELDS:
+            continue
+        va, vb = getattr(a, name), getattr(b, name)
+        if isinstance(va, C.Array):
+            if bytes(va) != bytes(vb):
+                return name
+        elif va != vb:
+            return name
+    return None
+
+
+def check_task(t: dial_task) -> dial_task:
+    """Raise unless the counts the kernels index the tables with are in range (include/dial_b200.h)."""
+    if not 1 <= t.n_stage <= DEFINES["DIAL_MAXSTAGE"]:
+        raise ValueError(f"dial_task.n_stage = {t.n_stage} is out of range (1..{DEFINES['DIAL_MAXSTAGE']})")
+    if not 0 <= t.n_user <= DEFINES["DIAL_MAXUSER"]:
+        raise ValueError(f"dial_task.n_user = {t.n_user} is out of range (0..{DEFINES['DIAL_MAXUSER']})")
+    return t
 
 ENV_IDS = {"unitree_go2_walk": 0, "unitree_go2_seq_jump": 1, "unitree_h1_walk": 2, "allegro_reorient": 3, "unitree_h1_loco": 4,
            "custom": 5}
@@ -159,13 +233,15 @@ def _bind(path: str) -> C.CDLL:
     lib.dial_mpc_bind.restype = C.c_int
     lib.dial_mpc_step.argtypes = [V, I, I, V]
     lib.dial_mpc_step.restype = C.c_int
+    lib.dial_plan_get_task.argtypes = [V, C.POINTER(dial_task)]
+    lib.dial_plan_get_task.restype = C.c_int
     for fn in ("dial_rollout", "dial_env_step", "dial_env_step_kin", "dial_plan_set_command", "dial_plan_set_stages", "dial_pipeline_init", "dial_reverse_rollout",
                "dial_reverse_update", "dial_reverse_update_x", "dial_reverse_trajbar", "dial_reverse_trajectories",
                "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status"):
         getattr(lib, fn).restype = C.c_int
     if lib.dial_abi_version() != DEFINES["DIAL_ABI_VERSION"]:
         raise RuntimeError(f"{os.path.basename(path)} ABI version does not match include/dial_b200.h")
-    for i, t in enumerate((dial_model_desc, dial_plan_desc, dial_state, dial_mpc_buffers)):
+    for i, t in enumerate((dial_model_desc, dial_plan_desc, dial_state, dial_mpc_buffers, dial_task)):
         if lib.dial_sizeof(i) != C.sizeof(t):
             raise RuntimeError(f"struct layout mismatch for {t.__name__}: C {lib.dial_sizeof(i)} vs ctypes {C.sizeof(t)}")
     return lib
@@ -192,4 +268,4 @@ EXPORTS = ["dial_abi_version", "dial_last_error", "dial_sizeof", "dial_plan_crea
            "dial_env_step", "dial_env_step_kin", "dial_plan_set_command", "dial_plan_set_stages", "dial_pipeline_init", "dial_reverse_rollout", "dial_reverse_update", "dial_reverse_update_x",
            "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status",
            "dial_reverse_trajbar", "dial_reverse_trajectories", "dial_key_split", "dial_fp32_peak", "dial_launch_count", "dial_rollout_wpc", "dial_debug_counters",
-           "dial_solver_variant", "dial_custom_reward_id", "dial_mpc_bind", "dial_mpc_step"]
+           "dial_solver_variant", "dial_custom_reward_id", "dial_mpc_bind", "dial_mpc_step", "dial_plan_get_task"]

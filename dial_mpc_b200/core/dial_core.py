@@ -9,6 +9,7 @@ sharded over several GPUs (one process per GPU).
 from __future__ import annotations
 
 import argparse
+import dataclasses
 import importlib
 import os
 import sys
@@ -20,6 +21,7 @@ import torch
 import yaml
 
 import dial_mpc_b200.envs as dial_envs
+from dial_mpc_b200 import _capi
 from dial_mpc_b200 import random as drandom
 from dial_mpc_b200.core.dial_config import DialConfig
 from dial_mpc_b200.plan import Plan
@@ -292,7 +294,7 @@ class DeviceLoop:
     the GPUs inside the kernels (peer-memory exchange), so no host collective sits in the step."""
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
-                 compute_bars: bool = True, noise=None):
+                 compute_bars: bool = True, noise=None, envs=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -300,7 +302,14 @@ class DeviceLoop:
         uint32 and ``Y0`` [B,Hnode+1,nu] or None.  Every per-instance buffer, ``Y``, ``action``,
         ``reward``, ``info()`` and ``set_state`` gain a leading [B]; ``state(b)`` materialises
         instance b.  Instance b computes bitwise what a single-instance loop from its state, rng and
-        knots computes."""
+        knots computes.
+
+        ``envs``: B env objects of ``mbdpi.env``'s class, one task per instance (commands, gait, jump
+        sequence, custom-reward user constants; ``BaseEnv.task``).  Every other field of their plan
+        descriptors must equal ``mbdpi.env``'s: the plan shares it.  Instance b then computes bitwise
+        what a single-instance loop on ``envs[b]`` computes.  A batched loop whose states all carry
+        ``randomize_target`` binds per-instance tasks as well: each instance draws its own commands
+        (and seq-jump its own jump sequence, from its state's info)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -314,9 +323,16 @@ class DeviceLoop:
         states = list(state) if B > 1 else [state]
         if len(states) != B:
             raise ValueError(f"a plan of {B} instances needs {B} states, got {len(states)}")
-        if B > 1 and any(s.info.get("randomize_target", False) for s in states):
-            raise RuntimeError("randomize_tasks draws per-instance commands, which a batched DeviceLoop does not "
-                               "support: run one DeviceLoop per instance")
+        rand = [bool(s.info.get("randomize_target", False)) for s in states]
+        if any(rand) and not all(rand):
+            raise RuntimeError("randomize_tasks draws per-instance commands: in a batched DeviceLoop either every "
+                               "state carries randomize_target or none does")
+        if envs is not None:
+            envs = list(envs)
+            if len(envs) != B:
+                raise ValueError(f"a plan of {B} instances needs {B} envs, got {len(envs)}")
+            for env_b in envs:
+                self._check_shared(mbdpi.env, env_b)
         lead = (B,) if B > 1 else ()
         key = np.ascontiguousarray(rng, dtype=np.uint32)
         if key.shape != lead + (2,):
@@ -341,16 +357,65 @@ class DeviceLoop:
             noise=(mbdpi.schedule(nmax) if noise is None else f(noise)).contiguous())
         assert tuple(self.buf["noise"].shape) == (nmax, a.Hnode + 1) or self.buf["noise"].shape[0] >= nmax
         self.n_diffuse_max = nmax
-        # randomize_tasks: host mirror of info["step"] / info["rng"] (the env's key chain), from which
-        # the one-step random command the horizon may reach is computed ahead (BaseEnv.command_override)
-        s0 = states[0]
-        self._rand = bool(s0.info.get("randomize_target", False))
-        self._env_info = {"randomize_target": self._rand, "step": int(s0.info.get("step", 0)),
-                          "rng": np.asarray(s0.info.get("rng", np.zeros(2)), dtype=np.uint32).copy()}
-        if self._rand and hasattr(mbdpi.env, "stage_tables"):
+        # randomize_tasks: per instance, a host mirror of info["step"] / info["rng"] (the env's key chain),
+        # from which the one-step random command the horizon may reach is computed ahead
+        # (BaseEnv.command_override)
+        self._rand = rand[0]
+        self._env_info = [{"randomize_target": self._rand, "step": int(s.info.get("step", 0)),
+                           "rng": np.asarray(s.info.get("rng", np.zeros(2)), dtype=np.uint32).copy()} for s in states]
+        # per-instance tasks: an explicit env per instance, or per-instance random commands
+        self._envs = envs if envs is not None else [mbdpi.env] * B
+        self._tasks_host = None
+        if envs is not None or (B > 1 and self._rand):
+            self._tasks_host = [e.task() for e in self._envs]
+            if self._rand and hasattr(mbdpi.env, "stage_tables"):
+                # seq-jump: the jump sequence drawn at reset is constant afterwards
+                for b, s in enumerate(states):
+                    _capi.task_set_stages(self._tasks_host[b], self._envs[b].stage_tables(s.info))
+            self._task_cmd = [()] * B       # command override last uploaded per instance (() = none yet)
+            self.buf["tasks"] = torch.from_numpy(
+                np.stack([np.frombuffer(bytes(t), np.uint8) for t in self._tasks_host])).to(dev)
+        elif self._rand and hasattr(mbdpi.env, "stage_tables"):
             # seq-jump: the jump sequence drawn at reset is constant afterwards; one upload at bind time
-            pl.set_stages(mbdpi.env.stage_tables(s0.info))
+            pl.set_stages(mbdpi.env.stage_tables(states[0].info))
         pl.mpc_bind(self.buf, mbdpi.M_shift.cpu().numpy())
+
+    @staticmethod
+    def _check_shared(ref_env, env) -> None:
+        """``env`` may give an instance of ``ref_env``'s plan its task: same class, and the same plan
+        descriptor outside the task fields."""
+        if type(env) is not type(ref_env):
+            raise ValueError(f"every instance's env must be a {type(ref_env).__name__}, got {type(env).__name__}")
+        diff = _capi.first_shared_difference(ref_env.plan_desc(), env.plan_desc())
+        if diff is not None:
+            raise ValueError(f"plan descriptor field '{diff}' differs between the instances' envs; it is shared "
+                             "by every instance of a plan (only the dial_task fields may differ)")
+
+    def _upload_task(self, b: int) -> None:
+        """Stream-ordered copy of instance b's host task into the bound tasks (no host synchronisation)."""
+        t = self._tasks_host[b]
+        src = torch.from_numpy(np.frombuffer(bytes(t), np.uint8).copy())
+        self.buf["tasks"][b].copy_(src, non_blocking=True)
+
+    def set_task(self, b: int, env_or_task) -> None:
+        """Replace instance b's task before the next ``step``: an env of ``mbdpi.env``'s class (its
+        ``task()``; the shared fields must match) or a ``_capi.dial_task``.  A stream-ordered copy on
+        the current stream, no host synchronisation.  Needs a loop with per-instance tasks bound
+        (``envs=`` or batched ``randomize_tasks``); randomize_tasks loops keep applying each instance's
+        one-step random command on top."""
+        if self._tasks_host is None:
+            raise RuntimeError("set_task needs per-instance tasks: build the DeviceLoop with envs=[...]")
+        b = int(b)
+        if not 0 <= b < self.n_instances:
+            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        if isinstance(env_or_task, _capi.dial_task):
+            t = _capi.check_task(_capi.dial_task.from_buffer_copy(env_or_task))
+        else:
+            self._check_shared(self.mbdpi.env, env_or_task)
+            t = env_or_task.task()
+        self._tasks_host[b] = t
+        self._task_cmd[b] = ()
+        self._upload_task(b)
 
     def step(self, n_diffuse: Optional[int] = None, env_step=True) -> None:
         """One control step (asynchronous on the current stream).  env_step: True = env step + shift
@@ -361,14 +426,22 @@ class DeviceLoop:
         stepping = env_step is True or env_step == 1
         if self._rand:
             # the env step (if any) runs at info["step"], the rollouts cover the Hsample+1 steps after it
-            self.plan.set_command(self.mbdpi.env.command_override(
-                self._env_info, self.mbdpi.args.Hsample + (2 if stepping else 1)))
+            horizon = self.mbdpi.args.Hsample + (2 if stepping else 1)
+            if self._tasks_host is None:
+                self.plan.set_command(self.mbdpi.env.command_override(self._env_info[0], horizon))
+            else:
+                for b, info in enumerate(self._env_info):
+                    ov = self._envs[b].command_override(info, horizon)
+                    key = _capi.task_set_command(self._tasks_host[b], ov)
+                    if key != self._task_cmd[b]:      # upload only the instances whose command changed
+                        self._upload_task(b)
+                        self._task_cmd[b] = key
         self.plan.mpc_step(n, env_step)
         if stepping:
-            self._env_info["step"] += 1
-            if self._rand:
-                from dial_mpc_b200 import random as drandom
-                self._env_info["rng"] = drandom.split(self._env_info["rng"])[0]
+            for info in self._env_info:
+                info["step"] += 1
+                if self._rand:
+                    info["rng"] = drandom.split(info["rng"])[0]
 
     def rng_host(self) -> np.ndarray:
         """The planner rng after the steps launched so far (synchronises)."""
@@ -384,10 +457,13 @@ class DeviceLoop:
         if qacc_warmstart is not None:
             self.buf["qacc_warmstart"].copy_(self.plan.f32(qacc_warmstart))
         if step is not None and self.n_instances > 1:
-            self.buf["counters"][:, 0] = torch.as_tensor(np.asarray(step, dtype=np.int32), device=self.buf["counters"].device)
+            steps = np.broadcast_to(np.asarray(step, dtype=np.int32), (self.n_instances,))
+            self.buf["counters"][:, 0] = torch.as_tensor(steps.copy(), device=self.buf["counters"].device)
+            for info, s in zip(self._env_info, steps):
+                info["step"] = int(s)
         elif step is not None:
             self.buf["counters"][0] = int(step)
-            self._env_info["step"] = int(step)
+            self._env_info[0]["step"] = int(step)
 
     @property
     def action(self) -> torch.Tensor:
@@ -445,16 +521,17 @@ def save_run(output_dir, rollout, infos, timestamp=None):
     return states, preds
 
 
-def run_instances(dial_config, env, B, Nstep):
+def run_instances(dial_config, env, B, Nstep, envs=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
-    plain run with seed ``dial_config.seed + b``."""
+    plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task, when given).  With
+    ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key."""
     mbdpi = MBDPI(dial_config, env, n_instances=B)
     states, rngs = [], []
     for b in range(B):
         rng, rng_reset = drandom.split(drandom.PRNGKey(seed=dial_config.seed + b))
-        states.append(env.reset(rng_reset))
+        states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
-    loop = DeviceLoop(mbdpi, states, np.stack(rngs))
+    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -490,6 +567,9 @@ def main():
     parser.add_argument("--instances", type=int, default=1,
                         help="run this many independent closed loops in one CUDA graph per control step; instance b "
                              "resets from PRNGKey(seed + b) and writes its output files under the prefix <time>_inst<b>")
+    parser.add_argument("--instance-overrides", type=str, default=None, metavar="FILE.yaml",
+                        help="a YAML list of one mapping of env-config fields per instance (--instances of them): "
+                             "instance b runs the config updated by mapping b (its own commands, gait, targets, ...)")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -513,8 +593,29 @@ def main():
     env_config_type = dial_envs.get_config(dial_config.env_name)
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
     env = dial_envs.get_environment(dial_config.env_name, config=env_config)
+    envs = None
+    if args.instance_overrides is not None:
+        if args.instances < 2:
+            parser.error("--instance-overrides needs --instances B with B >= 2")
+        overrides = yaml.safe_load(open(args.instance_overrides))
+        if not isinstance(overrides, list) or len(overrides) != args.instances:
+            parser.error(f"--instance-overrides must hold a list of {args.instances} mappings (one per instance), "
+                         f"got {len(overrides) if isinstance(overrides, list) else type(overrides).__name__}")
+        known = {f.name for f in dataclasses.fields(env_config_type)}
+        envs = []
+        for b, ov in enumerate(overrides):
+            ov = ov or {}
+            if not isinstance(ov, dict) or set(ov) - known:
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, got "
+                             f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
+            cfg_b = load_dataclass_from_dict(env_config_type, dict(config_dict, **ov), convert_list_to_array=True)
+            envs.append(dial_envs.get_environment(dial_config.env_name, config=cfg_b))
+            try:
+                DeviceLoop._check_shared(env, envs[-1])
+            except ValueError as e:
+                parser.error(f"--instance-overrides entry {b}: {e}")
     if args.instances > 1:
-        run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps)
+        run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs)
         return
     mbdpi = MBDPI(dial_config, env)
     rng, rng_reset = drandom.split(rng)

@@ -113,6 +113,21 @@ struct alignas(16) DevPlan {
   int32_t pad_[3];
 };
 
+// The block vel_cmd .. user of dial_plan_desc has the layout of dial_task (include/dial_b200.h): a
+// launch without per-instance tasks reads the plan's own task through a view of it.
+#define DIAL_TASK_AT(f) (offsetof(dial_plan_desc, f) - offsetof(dial_plan_desc, vel_cmd) == offsetof(dial_task, f))
+static_assert(DIAL_TASK_AT(vel_cmd) && DIAL_TASK_AT(ang_cmd) && DIAL_TASK_AT(pos_tar) && DIAL_TASK_AT(gait_duty) &&
+              DIAL_TASK_AT(gait_cadence) && DIAL_TASK_AT(gait_amplitude) && DIAL_TASK_AT(gait_phase) &&
+              DIAL_TASK_AT(cmd_step) && DIAL_TASK_AT(cmd_vel) && DIAL_TASK_AT(cmd_ang) && DIAL_TASK_AT(n_stage) &&
+              DIAL_TASK_AT(jump_dt) && DIAL_TASK_AT(pose_seq) && DIAL_TASK_AT(yaw_seq) &&
+              DIAL_TASK_AT(contact_targets) && DIAL_TASK_AT(contact_radius) && DIAL_TASK_AT(n_user) &&
+              DIAL_TASK_AT(user) &&
+              offsetof(dial_plan_desc, user) + sizeof(float) * DIAL_MAXUSER - offsetof(dial_plan_desc, vel_cmd) == sizeof(dial_task),
+              "dial_plan_desc's task block must have the layout of dial_task");
+#undef DIAL_TASK_AT
+
+HD const dial_task& plan_task(const dial_plan_desc& c) { return *reinterpret_cast<const dial_task*>(c.vel_cmd); }
+
 // arguments of one rollout launch
 struct RolloutArgs {
   int32_t nrows;        // sample rows rolled by this launch
@@ -126,6 +141,10 @@ struct RolloutArgs {
   // offsets of the pointers below; per-row outputs are indexed by the global row.  0: one instance.
   int32_t rows_per_inst;
   int32_t us_row;       // floats between the action rows of `us` (mode 0); 0: H * nu
+  // per-instance reward inputs (dial_mpc_buffers.tasks): row r reads tasks[r / task_rows], or tasks[0]
+  // for every row when task_rows == 0; null: every row reads the plan's own task (plan_task)
+  int32_t task_rows;
+  const dial_task* tasks;
   const float* qpos0;
   const float* qvel0;
   const float* warm0;
@@ -2682,7 +2701,8 @@ DEV BaseKin base_kin(WarpCtx& w, int bid) {
 
 // Per-foot / per-contact terms of the built-in rewards, one lane each (lanes 0..3), summed into
 // lane 0 by two xor-shuffles: [0] gait term (walk envs) or contact bonus (seq-jump), [1] penalty.
-DEV void reward_partials(WarpCtx& w, int step, int stage, float& p0, float& p1) {
+// The task fields (commands, gait, stage tables, user constants) come from `T`, the rest from the plan.
+DEV void reward_partials(WarpCtx& w, const dial_task& T, int step, int stage, float& p0, float& p1) {
   const DevModel& M = *w.M;
   const dial_plan_desc& c = w.P->c;
   const dial_model_desc& m = M.m;
@@ -2691,7 +2711,7 @@ DEV void reward_partials(WarpCtx& w, int step, int stage, float& p0, float& p1) 
   p0 = 0.f; p1 = 0.f;
   if (c.env_id == DIAL_ENV_GO2_WALK || c.env_id == DIAL_ENV_H1_WALK || c.env_id == DIAL_ENV_H1_LOCO) {
     if (f < c.nfeet) {
-      float zt = foot_step(c.gait_duty, c.gait_cadence, c.gait_amplitude, c.gait_phase[f], stepf * c.dt);
+      float zt = foot_step(T.gait_duty, T.gait_cadence, T.gait_amplitude, T.gait_phase[f], stepf * c.dt);
       float z;
       if (c.env_id == DIAL_ENV_GO2_WALK) {
         int sid = c.feet_site[f], sb = m.site_bodyid[sid];
@@ -2713,9 +2733,9 @@ DEV void reward_partials(WarpCtx& w, int step, int stage, float& p0, float& p1) 
       float dist = SM(cdist)[i];
       bool penal = dist <= 0.001f;
       float px = SM(cpos)[3 * i], py = SM(cpos)[3 * i + 1];
-      for (int j = 0; j < c.n_stage; ++j) {
-        float dx = px - c.contact_targets[j][i][0], dyy = py - c.contact_targets[j][i][1];
-        bool cond = dx * dx + dyy * dyy <= c.contact_radius[j][i] * c.contact_radius[j][i];
+      for (int j = 0; j < T.n_stage; ++j) {
+        float dx = px - T.contact_targets[j][i][0], dyy = py - T.contact_targets[j][i][1];
+        bool cond = dx * dx + dyy * dyy <= T.contact_radius[j][i] * T.contact_radius[j][i];
         if (cond && j == stage) p0 += fminf(fmaxf(1.f - dist, 0.f), 1.f);
         penal = penal && !cond;
       }
@@ -2729,7 +2749,7 @@ DEV void reward_partials(WarpCtx& w, int step, int stage, float& p0, float& p1) 
   p0 += shfl_xor(p0, 2); p1 += shfl_xor(p1, 2);
 }
 
-DEV float reward_lane0(WarpCtx& w, int step, int& stage, float part0, float part1) {
+DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, float part0, float part1) {
   const DevModel& M = *w.M;
   const dial_plan_desc& c = w.P->c;
   const dial_model_desc& m = M.m;
@@ -2739,13 +2759,13 @@ DEV float reward_lane0(WarpCtx& w, int step, int& stage, float part0, float part
   if (c.env_id == DIAL_ENV_CUSTOM) {
     dial_reward_ctx x;
     x.step = step; x.dt = c.dt;
-    x.nq = m.nq; x.nv = m.nv; x.nu = m.nu; x.nbody = m.nbody; x.ncon = m.ncon; x.nsite = m.nsite; x.n_user = c.n_user;
+    x.nq = m.nq; x.nv = m.nv; x.nu = m.nu; x.nbody = m.nbody; x.ncon = m.ncon; x.nsite = m.nsite; x.n_user = T.n_user;
     x.qpos = SM(qpos); x.qvel = SM(qvel); x.ctrl = SM(ctrl);
     x.xpos = SM(xpos); x.xquat = SM(xquat); x.xmat = SM(xmat); x.cvel = SM(cvel);
     x.subtree_com = SM(rcom); x.body_rootidx = M.body_rootidx;
     x.contact_dist = SM(cdist); x.contact_pos = SM(cpos);
     x.site_bodyid = m.site_bodyid; x.site_pos = &m.site_pos[0][0];
-    x.user = c.user;
+    x.user = T.user;
     return dial_custom_reward(&x);
   }
 #endif
@@ -2757,17 +2777,17 @@ DEV float reward_lane0(WarpCtx& w, int step, int& stage, float part0, float part
     // manipulation.py:75-84: ball angular velocity / position tracking + joint deviation
     const int ob = c.torso_body;
     V3 wv = ld3(SM(cvel) + 6 * ob) * (3.14159265358979f / 180.f);
-    V3 dw = wv - ld3(c.ang_cmd);
-    V3 dp = ld3(SM(xpos) + 3 * ob) - ld3(c.pos_tar);
+    V3 dw = wv - ld3(T.ang_cmd);
+    V3 dp = ld3(SM(xpos) + 3 * ob) - ld3(T.pos_tar);
     float rj = 0.f;
     for (int a = 0; a < m.nu; ++a) { float e = SM(qpos)[7 + a] - c.joint_offset[a]; rj -= e * e; }
     return -dot(dw, dw) - 5.f * dot(dp, dp) + 0.1f * rj;
   }
   if (c.env_id == DIAL_ENV_GO2_WALK || c.env_id == DIAL_ENV_H1_WALK || c.env_id == DIAL_ENV_H1_LOCO) {
     float ramp = stepf * c.dt / c.ramp_up_time;
-    // randomize_tasks: a one-step command override (dial_plan_set_command)
-    const float* vel_cmd = step == c.cmd_step ? c.cmd_vel : c.vel_cmd;
-    const float* ang_cmd = step == c.cmd_step ? c.cmd_ang : c.ang_cmd;
+    // randomize_tasks: a one-step command override (dial_plan_set_command / the task's cmd_step)
+    const float* vel_cmd = step == T.cmd_step ? T.cmd_vel : T.vel_cmd;
+    const float* ang_cmd = step == T.cmd_step ? T.cmd_ang : T.ang_cmd;
     float vtx = fminf(vel_cmd[0] * ramp, vel_cmd[0]), vty = fminf(vel_cmd[1] * ramp, vel_cmd[1]);
     float atz = fminf(ang_cmd[2] * ramp, ang_cmd[2]);
     const float r_gaits = part0;   // per-foot terms: reward_partials
@@ -2778,7 +2798,7 @@ DEV float reward_lane0(WarpCtx& w, int step, int& stage, float part0, float part
     float r_yaw = -wy * wy;
     float r_vel = -((bk.vb.x - vtx) * (bk.vb.x - vtx) + (bk.vb.y - vty) * (bk.vb.y - vty));
     float r_ang = -(bk.ab.z - atz) * (bk.ab.z - atz);
-    float r_h = -(bk.pos.z - c.pos_tar[2]) * (bk.pos.z - c.pos_tar[2]);
+    float r_h = -(bk.pos.z - T.pos_tar[2]) * (bk.pos.z - T.pos_tar[2]);
     if (c.env_id == DIAL_ENV_GO2_WALK) {
       rew = 0.1f * r_gaits + 0.5f * r_upright + 0.3f * r_yaw + r_vel + r_ang + r_h;
     } else if (c.env_id == DIAL_ENV_H1_LOCO) {
@@ -2799,14 +2819,14 @@ DEV float reward_lane0(WarpCtx& w, int step, int& stage, float part0, float part
       rew = 5.f * r_gaits + 0.5f * r_upright + 0.1f * r_yaw + r_vel + r_ang + 0.5f * r_h + 0.01f * r_energy;
     }
   } else {  // DIAL_ENV_GO2_SEQJUMP
-    V3 dp = bk.pos - ld3(c.pose_seq[stage]);
+    V3 dp = bk.pos - ld3(T.pose_seq[stage]);
     float r_pos = -dot(dp, dp);
-    float dy = quat_yaw(bk.rot) - c.yaw_seq[stage];
+    float dy = quat_yaw(bk.rot) - T.yaw_seq[stage];
     float r_yaw = -dy * dy;
     const float r_contact = part0, pen = part1;   // per-contact terms: reward_partials
     rew = r_pos + r_upright + 0.3f * r_yaw + 0.1f * r_contact - 0.1f * pen + 10.f;
-    int ns = (int)floorf((float)(step + 1) * c.dt / c.jump_dt);
-    stage = ns < c.n_stage - 1 ? ns : c.n_stage - 1;
+    int ns = (int)floorf((float)(step + 1) * c.dt / T.jump_dt);
+    stage = ns < T.n_stage - 1 ? ns : T.n_stage - 1;
   }
   return rew;
 }
@@ -2933,8 +2953,11 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
     for (int f = 0; f < nfr; ++f) physics_step<NL, NR>(w, !fwd_only);
     if (fwd_only) break;
     float rew = 0.f, part0, part1;
-    reward_partials(w, step, stage, part0, part1);
-    if (lane == 0) rew = reward_lane0(w, step, stage, part0, part1);
+    // the task of this row, derived here from `row` (live anyway) and the launch arguments so that no
+    // register holds it over the physics step
+    const dial_task& T = A.tasks ? A.tasks[A.task_rows > 0 ? row / A.task_rows : 0] : plan_task(c);
+    reward_partials(w, T, step, stage, part0, part1);
+    if (lane == 0) rew = reward_lane0(w, T, step, stage, part0, part1);
     stage = shfl_i(stage, 0);
     step += 1;
     rsum += rew;

@@ -296,6 +296,11 @@ static inline bool derive_model(const dial_model_desc& m, DevModel& D, std::stri
   return true;
 }
 
+// The counts the reward loops over, in range (the kernel indexes the tables with them unchecked).
+static inline bool task_valid(const dial_task& t) {
+  return t.n_stage >= 1 && t.n_stage <= DIAL_MAXSTAGE && t.n_user >= 0 && t.n_user <= DIAL_MAXUSER;
+}
+
 static inline int star_variant(const DevModel& D) {
   if (D.dense) return D.m.nv == DIAL_DENSE_NV ? 3 : -1;   // dense path: one instantiation per library build
   if (D.star_nchain >= 1 && D.star_nchain <= 4) {

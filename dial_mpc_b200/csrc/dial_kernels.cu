@@ -572,7 +572,7 @@ extern "C" int dial_abi_version(void) { return DIAL_ABI_VERSION; }
 extern "C" const char* dial_last_error(void) { return g_err.c_str(); }
 extern "C" size_t dial_sizeof(int which) {
   return which == 0 ? sizeof(dial_model_desc) : which == 1 ? sizeof(dial_plan_desc) : which == 2 ? sizeof(dial_state)
-       : which == 3 ? sizeof(dial_mpc_buffers) : 0;
+       : which == 3 ? sizeof(dial_mpc_buffers) : which == 4 ? sizeof(dial_task) : 0;
 }
 
 // solver instantiation by tree shape: star<3,6> (quadruped), star<5,7> (humanoid), star<5,6>,
@@ -807,6 +807,14 @@ extern "C" int dial_plan_set_stages(dial_plan* p, int n_stage, const float* pose
   const size_t off = offsetof(dial_plan_desc, n_stage), end = offsetof(dial_plan_desc, n_user);
   CUDA_OK(cudaMemcpyAsync((char*)p->dP + off, (const char*)&p->hP.c + off, end - off, cudaMemcpyHostToDevice,
                           (cudaStream_t)stream));
+  return 0;
+}
+
+extern "C" int dial_plan_get_task(const dial_plan* p, dial_task* out) {
+  if (!p || !out) return fail("dial_plan_get_task: null argument");
+  const dial_task& t = plan_task(p->hP.c);   // the plan's task block (include/dial_b200.h)
+  if (!task_valid(t)) return fail("dial_plan_get_task: the plan's n_stage / n_user are out of range (1..DIAL_MAXSTAGE / 0..DIAL_MAXUSER)");
+  *out = t;
   return 0;
 }
 
@@ -1045,6 +1053,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     A.counters_in = B.counters; A.counters_out = B.counters;
     A.nrows = ni; A.H = 1; A.mode = 0; A.us = Y[cur]; A.rewss = B.reward;
     if (batched) { A.rows_per_inst = 1; A.us_row = n1 * nu; }
+    if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
     CUDA_OK(launch_rollout(p, A, 1, st));
   }
@@ -1077,6 +1086,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart; A.counters_in = B.counters;
     A.nrows = ni * (c.Nsample + 1); A.H = c.Hsample + 1; A.mode = 1;
     if (batched) A.rows_per_inst = c.Nsample + 1;
+    if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? c.Nsample + 1 : 0; }
     A.Ybar = Y[cur]; A.noise = noise;
     if (fused) A.rng_dev = B.rng; else A.key_dev = p->mpc_key;
     p->cur ^= 1;

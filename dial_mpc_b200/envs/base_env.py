@@ -175,8 +175,15 @@ class BaseEnv:
             _capi._set(d.M_n2u, M_n2u)
         d.cmd_step = -1
         d.n_inst = int(n_inst)
+        d.n_stage = 1         # one (unused) stage unless the env has a jump sequence
         self._fill_reward_desc(d)
         return d
+
+    def task(self) -> "_capi.dial_task":
+        """The reward inputs of this env's configuration that may differ between the instances of one
+        plan (commands, gait, jump sequence, custom-reward user constants): the task fields of
+        ``plan_desc()``, for ``DeviceLoop(..., envs=...)`` / ``DeviceLoop.set_task``."""
+        return _capi.task_from_desc(self.plan_desc())
 
     # -- reset / step through the CUDA core ---------------------------------------------------
     def _get_plan(self):

@@ -209,9 +209,10 @@ class Plan:
     # -- device-resident MPC loop (one CUDA graph per control step) ---------------------------------
     def mpc_bind(self, bufs: dict, M_shift) -> None:
         """``bufs``: name -> CUDA tensor for every field of ``dial_mpc_buffers`` (qbar/qdbar/xbar may be
-        None).  The tensors must stay alive and in place while bound (kept on ``self``)."""
+        None; ``tasks``, [B, sizeof(dial_task)] bytes, may be None or absent).  The tensors must stay alive
+        and in place while bound (kept on ``self``)."""
         b = _capi.dial_mpc_buffers()
-        want = {"counters": torch.int32, "rng": torch.int32}
+        want = {"counters": torch.int32, "rng": torch.int32, "tasks": torch.uint8}
         for name, _ in _capi.dial_mpc_buffers._fields_:
             t = bufs.get(name)
             if t is None:

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define DIAL_ABI_VERSION 9
+#define DIAL_ABI_VERSION 10
 
 /* capacities of the fixed-size device model */
 #define DIAL_MAXB 24   /* bodies incl. world            */
@@ -116,8 +116,16 @@ typedef struct dial_plan_desc {
   int32_t torso_body;       /* MuJoCo body id of the torso (x index + 1)          */
   int32_t nfeet;
   int32_t feet_site[4];
+  float ramp_up_time;
+  /* ---- the task: vel_cmd .. user is laid out exactly as dial_task below (the kernels read a plan's
+   * own task through a dial_task view of this block) ---- */
+  float vel_cmd[3], ang_cmd[3], pos_tar[3];
   float gait_duty, gait_cadence, gait_amplitude, gait_phase[4];
-  float vel_cmd[3], ang_cmd[3], ramp_up_time, pos_tar[3];
+  /* randomize_tasks (unitree_go2_env.py:141-155, unitree_h1_env.py:198-212): the env step whose
+   * info["step"] equals cmd_step uses (cmd_vel, cmd_ang) instead of (vel_cmd, ang_cmd); -1 = none.
+   * Set through dial_plan_set_command only (dial_plan_create ignores the value and starts at -1). */
+  int32_t cmd_step;
+  float cmd_vel[3], cmd_ang[3];
   /* seq-jump */
   int32_t n_stage;
   float jump_dt;
@@ -126,11 +134,7 @@ typedef struct dial_plan_desc {
   /* DIAL_ENV_CUSTOM: constants handed to dial_custom_reward() (ctx->user) */
   int32_t n_user;
   float user[DIAL_MAXUSER];
-  /* randomize_tasks (unitree_go2_env.py:141-155, unitree_h1_env.py:198-212): the env step whose
-   * info["step"] equals cmd_step uses (cmd_vel, cmd_ang) instead of (vel_cmd, ang_cmd); -1 = none.
-   * Set through dial_plan_set_command only (dial_plan_create ignores the value and starts at -1). */
-  int32_t cmd_step;
-  float cmd_vel[3], cmd_ang[3];
+  /* ---- end of the task ---- */
   /* independent planner instances of one plan (0 or 1: a single instance).  B > 1 instances share
    * the model, every constant above and the annealing schedule; each has its own state, counters,
    * rng, control knots and outputs (see dial_mpc_buffers).  Batched plans run through dial_mpc_step
@@ -138,6 +142,25 @@ typedef struct dial_plan_desc {
    * Nsample + 1 <= 2^17. */
   int32_t n_inst;
 } dial_plan_desc;
+
+/* The task of one planner instance: exactly the reward inputs that differ between tasks of one model,
+ * with the names, meanings and layout of the dial_plan_desc block vel_cmd .. user above.  Everything else (model, gains, joint
+ * ranges, dt, ramp_up_time, torso body, feet sites, Nsample, annealing schedule) stays in the plan.
+ * The kernels trust the counts: a task must hold 1 <= n_stage <= DIAL_MAXSTAGE and
+ * 0 <= n_user <= DIAL_MAXUSER (dial_plan_get_task and the Python helpers check this; a caller that
+ * writes tasks itself must too). */
+typedef struct dial_task {
+  float vel_cmd[3], ang_cmd[3], pos_tar[3];
+  float gait_duty, gait_cadence, gait_amplitude, gait_phase[4];
+  int32_t cmd_step;                 /* randomize_tasks one-step command; -1 = none */
+  float cmd_vel[3], cmd_ang[3];
+  int32_t n_stage;                  /* 1..DIAL_MAXSTAGE */
+  float jump_dt;
+  float pose_seq[DIAL_MAXSTAGE][3], yaw_seq[DIAL_MAXSTAGE];
+  float contact_targets[DIAL_MAXSTAGE][4][3], contact_radius[DIAL_MAXSTAGE][4];
+  int32_t n_user;
+  float user[DIAL_MAXUSER];
+} dial_task;
 
 /* State handed to the planner: Brax `State.pipeline_state` (qpos, qvel,
  * qacc_warmstart) + `State.info` counters the rewards read
@@ -155,7 +178,7 @@ typedef struct dial_plan dial_plan;
 int dial_abi_version(void);
 const char* dial_last_error(void);
 /* sizeof() of the descriptor structs as compiled into the library: which = 0 model, 1 plan,
- * 2 state, 3 mpc buffers (lets foreign-language bindings verify their struct layout). */
+ * 2 state, 3 mpc buffers, 4 task (lets foreign-language bindings verify their struct layout). */
 size_t dial_sizeof(int which);
 
 /* Create / destroy a plan (uploads model + config, allocates all workspaces). */
@@ -189,6 +212,11 @@ int dial_plan_set_command(dial_plan* plan, int cmd_step, const float vel[3], con
  * dial_plan_set_command. */
 int dial_plan_set_stages(dial_plan* plan, int n_stage, const float* pose_seq, const float* yaw_seq,
                          const float* contact_targets, const float* contact_radius, void* stream);
+
+/* The plan's current task (its dial_plan_desc reward inputs, including what dial_plan_set_command /
+ * _set_stages last put there) as a dial_task [host]: a starting point for per-instance tasks
+ * (dial_mpc_buffers.tasks).  Fails if the plan's counts are out of range. */
+int dial_plan_get_task(const dial_plan* plan, dial_task* out);
 
 /* The same step, also returning what the envs' `_get_obs` (envs/unitree_go2_env.py:263-286,
  * unitree_h1_env.py:323-346) reads of pipeline_state.x / xd: kin_out [dev][13] = x.pos(3),
@@ -296,6 +324,14 @@ typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound 
    * Y [B,Hn+1,nu], ctrl [B,nu], reward [B], rews [B,Nsample+1], qbar [B,Hs+1,nq],
    * qdbar [B,Hs+1,nv], xbar [B,Hs+1,nbody-1,3].  rews_all must be NULL.  Instance b's results are
    * bitwise those of a single-instance plan bound to instance b's slices. */
+  /* Per-instance tasks [B] (B = 1 for a single-instance plan), or NULL: every instance then plans the
+   * task of the plan's own constants.  Non-NULL: every launch of dial_mpc_step (the env-step row and all
+   * rollout rows) reads instance b's reward inputs from tasks[b], and the plan's task fields, including
+   * what dial_plan_set_command / _set_stages put there, are ignored.  Instance b's results are bitwise
+   * those of a plan whose constants hold tasks[b].  The captured graph holds the pointer, not the
+   * contents: the caller may rewrite tasks between dial_mpc_step calls with a copy on the same stream
+   * (stream-ordered, like dial_plan_set_command).  Each task must satisfy the ranges of dial_task. */
+  const dial_task* tasks;
 } dial_mpc_buffers;
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u

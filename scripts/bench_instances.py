@@ -7,7 +7,9 @@ plan of B instances of a BASELINE config: the synthetic state of bench.py (reset
 env steps) for every instance, instance b's planner rng PRNGKey(seed + b), a 256 MiB L2 flush between
 steps outside the timed CUDA events.  Prints one JSON line: value = B * Ndiffuse * Nsample * Hsample
 / step time, ms per control step, and the card, power limit and SM clocks read in the same run.
-``--instances 1`` is the single-instance plan (bench.py's timed step)."""
+``--instances 1`` is the single-instance plan (bench.py's timed step).  ``--distinct-tasks``: instance b
+plans its own velocity command (vx spread over [-1, 1], a per-instance task bound through
+``DeviceLoop(..., envs=...)``) instead of the config's shared one."""
 import argparse
 import json
 import os
@@ -33,6 +35,8 @@ def main():
     ap.add_argument("--instances", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--distinct-tasks", action="store_true",
+                    help="bind one task per instance: B distinct forward-velocity commands")
     args = ap.parse_args()
     if args.instances < 1 or args.steps < 1:
         ap.error("--instances and --steps must be at least 1")
@@ -49,10 +53,18 @@ def main():
     state = env.reset(drandom.PRNGKey(0))
     for _ in range(10):
         state = env.step(state, torch.zeros(mb.nu, device=mb.device))
+    envs = None
+    if args.distinct_tasks:
+        from dataclasses import replace
+        import dial_mpc_b200.envs as E
+        if not hasattr(env._config, "default_vx"):
+            ap.error(f"--distinct-tasks sweeps default_vx, which {type(env).__name__} has not")
+        envs = [E.get_environment(b["env"], config=replace(env._config, default_vx=float(v)))
+                for v in np.linspace(-1.0, 1.0, B)]
     if B == 1:
-        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed))
+        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs)
     else:
-        loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]))
+        loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=mb.device)
     for _ in range(max(args.warmup, 3)):
         loop.step(cfg.Ndiffuse, env_step=2)
@@ -68,7 +80,7 @@ def main():
     torch.cuda.synchronize()
     t = sum(a.elapsed_time(e) for a, e in evs) / 1e3 / args.steps
     rows = B * (cfg.Nsample + 1)
-    print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, rows_per_rollout=rows,
+    print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=bool(envs), rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
                           value=B * cfg.Ndiffuse * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
