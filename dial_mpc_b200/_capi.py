@@ -211,6 +211,7 @@ def _bind(path: str) -> C.CDLL:
     lib.dial_reverse_rollout.argtypes = [V, C.POINTER(dial_state), P, U2, P, P, P, V]
     lib.dial_reverse_update.argtypes = [V, P, U2, P, P, P, P, P, V]
     lib.dial_reverse_update_x.argtypes = [V, P, U2, P, P, P, P, P, P, V]
+    lib.dial_reverse_update_fused.argtypes = [V, P, P, P, P, P, P, V]
     lib.dial_reverse_trajbar.argtypes = [V, P, I, P, P, P, V]
     lib.dial_exchange_create.argtypes = [V, I, I, P]
     lib.dial_exchange_connect.argtypes = [V, P]
@@ -236,8 +237,8 @@ def _bind(path: str) -> C.CDLL:
     lib.dial_plan_get_task.argtypes = [V, C.POINTER(dial_task)]
     lib.dial_plan_get_task.restype = C.c_int
     for fn in ("dial_rollout", "dial_env_step", "dial_env_step_kin", "dial_plan_set_command", "dial_plan_set_stages", "dial_pipeline_init", "dial_reverse_rollout",
-               "dial_reverse_update", "dial_reverse_update_x", "dial_reverse_trajbar", "dial_reverse_trajectories",
-               "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status"):
+               "dial_reverse_update", "dial_reverse_update_x", "dial_reverse_update_fused", "dial_reverse_trajbar",
+               "dial_reverse_trajectories", "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status"):
         getattr(lib, fn).restype = C.c_int
     if lib.dial_abi_version() != DEFINES["DIAL_ABI_VERSION"]:
         raise RuntimeError(f"{os.path.basename(path)} ABI version does not match include/dial_b200.h")
@@ -266,6 +267,6 @@ def check(rc: int) -> None:
 
 EXPORTS = ["dial_abi_version", "dial_last_error", "dial_sizeof", "dial_plan_create", "dial_plan_destroy", "dial_rollout",
            "dial_env_step", "dial_env_step_kin", "dial_plan_set_command", "dial_plan_set_stages", "dial_pipeline_init", "dial_reverse_rollout", "dial_reverse_update", "dial_reverse_update_x",
-           "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status",
+           "dial_reverse_update_fused", "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status",
            "dial_reverse_trajbar", "dial_reverse_trajectories", "dial_key_split", "dial_fp32_peak", "dial_launch_count", "dial_rollout_wpc", "dial_debug_counters",
            "dial_solver_variant", "dial_custom_reward_id", "dial_mpc_bind", "dial_mpc_step", "dial_plan_get_task"]

@@ -54,15 +54,15 @@ DIAL_DECL_LAUNCH(4)
 // softmax weights over all rewards (core/dial_core.py:125-128), single CTA
 // ---------------------------------------------------------------------------------
 // block-wide sum of K values per thread (+ optionally the max of one): shuffle tree, one smem
-// stage, result identical in every thread
-template <int K>
-__device__ __forceinline__ void block_reduce(float (&v)[K], float* mx, float* red) {
+// stage, result identical in every thread.  T = double: 64-bit shuffles (the reward statistics).
+template <typename T, int K>
+__device__ __forceinline__ void block_reduce(T (&v)[K], T* mx, T* red) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
     for (int k = 0; k < K; ++k) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-    if (mx) *mx = fmaxf(*mx, __shfl_xor_sync(0xffffffffu, *mx, o));
+    if (mx) *mx = fmax(*mx, __shfl_xor_sync(0xffffffffu, *mx, o));
   }
   __syncthreads();   // previous use of `red` is over
   if (lane == 0) {
@@ -72,25 +72,89 @@ __device__ __forceinline__ void block_reduce(float (&v)[K], float* mx, float* re
   }
   __syncthreads();
 #pragma unroll
-  for (int k = 0; k < K; ++k) v[k] = lane < nw ? red[k * 32 + lane] : 0.f;
-  if (mx) *mx = lane < nw ? red[K * 32 + lane] : -INFINITY;
+  for (int k = 0; k < K; ++k) v[k] = lane < nw ? red[k * 32 + lane] : T(0);
+  if (mx) *mx = lane < nw ? red[K * 32 + lane] : T(-INFINITY);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
     for (int k = 0; k < K; ++k) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-    if (mx) *mx = fmaxf(*mx, __shfl_xor_sync(0xffffffffu, *mx, o));
+    if (mx) *mx = fmax(*mx, __shfl_xor_sync(0xffffffffu, *mx, o));
   }
 }
 
 // rews [n] (mean sample last) -> weights [n] = softmax((rews - rews[n-1]) / std(rews) / temp)
-// (core/dial_core.py:125-128).  Three passes: statistics of d = r - rbar (count, sum, sum of
-// squares, max: the shift keeps the one-pass variance accurate), exp + normaliser, scale.
-// Deviations from the reference, which has no guards (SURVEY Appendix F):
+// (core/dial_core.py:125-128).  Deviations from the reference, which has no guards (SURVEY Appendix F):
 //   * non-finite rewards (diverged samples) get weight 0 and are left out of the statistics;
 //   * std == 0 (all finite rewards equal, e.g. zero noise): uniform weights over the finite
 //     samples instead of 0/0 = NaN;
 //   * no finite reward at all: the whole weight goes to the mean sample (Ybar is kept);
 //   * a non-finite rbar only changes the reference point of the shift (softmax is shift-invariant).
+// One function computes the statistics for both kernels that use them (weights_kernel and the fused
+// update_kernel), so the eager update and the control-step graph cannot drift apart.  The kernels
+// compute the logit of sample i as (r_i - shift) * inv - mx.
+struct SoftmaxParams {
+  float shift, inv, mx;   // inv = 1 / std / temp, 0 when the finite rewards are flat (uniform weights)
+  bool none;              // no finite reward
+};
+// Pass 2 of reward_softmax_params (ill-conditioned rewards): the deviations from the pass-1 mean
+// (rbar + mean), summed and block-reduced in fp64.  Not inlined: the fp64 registers of this rare path
+// stay out of the register allocation of the kernels' common path.
+__device__ __noinline__ SoftmaxParams reward_softmax_params_fp64(const float* __restrict__ rews, int n, float temp,
+                                                                 float rbar, float mean, float cnt, float* red_f) {
+  double* red = reinterpret_cast<double*>(red_f);
+  SoftmaxParams s;
+  s.none = false;
+  const double c = isfinite(mean) ? (double)rbar + (double)mean : 0.0;
+  double s1[1] = {0.0}, s2[1] = {0.0}, rmax = -INFINITY;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float r = __ldcg(rews + i);
+    if (isfinite(r)) { const double d = (double)r - c; s1[0] += d; s2[0] += d * d; rmax = fmax(rmax, (double)r); }
+  }
+  block_reduce<double, 1>(s1, &rmax, red);      // two reductions: `red` holds 2 x 32 doubles
+  block_reduce<double, 1>(s2, nullptr, red);
+  const double m = s1[0] / (double)cnt, var64 = s2[0] / (double)cnt - m * m;
+  s.shift = (float)rmax;   // the logit of the largest reward is 0; (r - rmax) is exact near the top
+  s.mx = 0.f;
+  // (clamped: a std of a few denormal ulp would give inf, and 0 * inf = NaN for the max sample)
+  s.inv = var64 > 0.0 ? (float)fmin(1.0 / (sqrt(var64) * (double)temp), 3.4028234663852886e38) : 0.f;
+  return s;
+}
+// Pass 1: count, sum and sum of squares of d = r - rbar and the max of d over the finite rewards, in
+// fp32 (rbar = 0 when it is not finite).  The one-pass variance is accurate while the shift lies near
+// the bulk of the rewards: it is used when rbar is finite, nothing overflowed and the shift is within
+// 8 standard deviations of the mean (|mean(d)| <= 8 std), where it loses at most 6 bits.  Otherwise it
+// cancels: with a NaN mean row, rewards -8 +- 0.003 gave a std of exactly 0, -30 +- 0.01 one 21 % off;
+// a mean sample 1e4 spreads below the others put it 1 % off at 2^17 rewards; a finite reward beyond
+// 1.8e19 overflowed d^2 (std = inf, every sample the same weight).  Those rewards take pass 2: the
+// deviations from the pass-1 mean, summed and block-reduced in fp64 (no cancellation, no overflow for
+// fp32 rewards), and logits relative to the largest finite reward.  The branch is uniform across the
+// block (every thread holds the same sums).  `red`: shared memory for 4 x 32 floats.
+__device__ __forceinline__ SoftmaxParams reward_softmax_params(const float* __restrict__ rews, int n, float temp,
+                                                               float* red) {
+  float rbar = __ldcg(rews + n - 1);
+  const bool rbar_finite = isfinite(rbar);
+  if (!rbar_finite) rbar = 0.f;
+  float st[3] = {0.f, 0.f, 0.f}, dmax = -INFINITY;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float r = __ldcg(rews + i);
+    if (isfinite(r)) { const float d = r - rbar; st[0] += 1.f; st[1] += d; st[2] += d * d; dmax = fmaxf(dmax, d); }
+  }
+  block_reduce<float, 3>(st, &dmax, red);
+  SoftmaxParams s;
+  const float cnt = st[0];
+  s.none = cnt == 0.f;
+  const float mean = st[1] / fmaxf(cnt, 1.f);
+  const float var = st[2] / fmaxf(cnt, 1.f) - mean * mean;
+  const float sd = sqrtf(fmaxf(var, 0.f));
+  if (s.none || (rbar_finite && isfinite(st[2]) && fabsf(mean) <= 8.f * sd)) {
+    s.shift = rbar;
+    s.inv = (sd > 0.f) ? 1.f / sd / temp : 0.f;
+    s.mx = dmax * s.inv;
+    return s;
+  }
+  return reward_softmax_params_fp64(rews, n, temp, rbar, mean, cnt, red);
+}
+
 // Multi-GPU consumer side of the reward exchange (dial_exchange_*): wait until every rank's flag
 // in the local mailbox carries the current sequence number.  Bounded spin (~4 s of %globaltimer):
 // a peer that never arrives sets *err instead of hanging the GPU.
@@ -130,7 +194,7 @@ __device__ __forceinline__ void xch_wait_flags(const uint32_t* flags, uint32_t w
 
 __global__ void __launch_bounds__(1024) weights_kernel(const float* __restrict__ rews, int n, float temp,
                                                         float* __restrict__ weights, const XchWait X) {
-  __shared__ float red[4 * 32];
+  __shared__ __align__(8) float red[4 * 32];
   const int tid = threadIdx.x;
   if (X.mbox) {
     const uint32_t seq = *X.seq, buf = seq & 1u;
@@ -139,33 +203,20 @@ __global__ void __launch_bounds__(1024) weights_kernel(const float* __restrict__
     if (X.rews_copy)
       for (int i = tid; i < n; i += blockDim.x) X.rews_copy[i] = __ldcg(rews + i);
   }
-  float rbar = __ldcg(rews + n - 1);
-  if (!isfinite(rbar)) rbar = 0.f;
-  float st[3] = {0.f, 0.f, 0.f}, dmax = -INFINITY;
-  for (int i = tid; i < n; i += blockDim.x) {
-    const float r = __ldcg(rews + i);
-    if (isfinite(r)) { const float d = r - rbar; st[0] += 1.f; st[1] += d; st[2] += d * d; dmax = fmaxf(dmax, d); }
-  }
-  block_reduce<3>(st, &dmax, red);
-  const float cnt = st[0];
-  if (cnt == 0.f) {
+  const SoftmaxParams s = reward_softmax_params(rews, n, temp, red);
+  if (s.none) {
     for (int i = tid; i < n; i += blockDim.x) weights[i] = (i == n - 1) ? 1.f : 0.f;
     if (X.mbox && tid == 0) *X.seq = *X.seq + 1u;
     return;
   }
-  const float mean = st[1] / cnt;
-  const float sd = sqrtf(fmaxf(st[2] / cnt - mean * mean, 0.f));
-  const bool flat = !(sd > 0.f);
-  const float inv = flat ? 0.f : 1.f / sd / temp;   // flat: every logit 0 -> uniform weights
-  const float mx = dmax * inv;
   float z[1] = {0.f};
   for (int i = tid; i < n; i += blockDim.x) {
     const float r = __ldcg(rews + i);
-    const float e = isfinite(r) ? expf((r - rbar) * inv - mx) : 0.f;
+    const float e = isfinite(r) ? expf((r - s.shift) * s.inv - s.mx) : 0.f;   // flat: inv = 0, every logit 0
     weights[i] = e;
     z[0] += e;
   }
-  block_reduce<1>(z, nullptr, red);
+  block_reduce<float, 1>(z, nullptr, red);
   const float iz = 1.f / z[0];
   for (int i = tid; i < n; i += blockDim.x) weights[i] *= iz;
   if (X.mbox && tid == 0) *X.seq = *X.seq + 1u;   // the next reverse_once uses the other mailbox half
@@ -282,7 +333,7 @@ __global__ void __launch_bounds__(YBAR_THREADS) ybar_kernel(const float* __restr
 // Fused update of the control step graph: weights + Ybar + rng advance in ONE multi-CTA kernel
 // (dial_core.py:106,125-132).  Every CTA recomputes the reward statistics (n <= 131072: up to 512
 // L2-resident loads per thread at the 65536-sample config, a few at 2048), accumulates sum_n e_n Y0s_n and sum_n e_n over its share of the samples with
-// e_n = exp((r_n - rbar) / std / temp - max); the last CTA adds the partials in fixed order,
+// e_n = exp((r_n - rbar) / std / temp - max) (reward_softmax_params); the last CTA adds the partials in fixed order,
 // divides, normalises the stored weights, and advances the planner rng.  Two graph nodes fewer per
 // reverse_once (a launch boundary inside a graph costs about a microsecond, so this is about graph
 // size and the host-visible weights dependency more than time).
@@ -295,7 +346,7 @@ __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __res
                                                                const float* __restrict__ noise, int Ntotal, int Hn1, int nu,
                                                                float* __restrict__ partial, unsigned int* __restrict__ counter,
                                                                float* __restrict__ Ybar_out) {
-  __shared__ float red[4 * 32];
+  __shared__ __align__(8) float red[4 * 32];
   __shared__ float acc[YBAR_THREADS];
   __shared__ bool is_last;
   const int tid = threadIdx.x;
@@ -312,20 +363,8 @@ __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __res
   uint32_t key0, key1;
   const uint32_t r0 = rng[0], r1 = rng[1];
   split_key(r0, r1, key0, key1);
-  // ---- statistics of d = r - rbar over the finite rewards (see weights_kernel) --------------------
-  float rbar = __ldcg(rews + n - 1);
-  if (!isfinite(rbar)) rbar = 0.f;
-  float st[3] = {0.f, 0.f, 0.f}, dmax = -INFINITY;
-  for (int i = tid; i < n; i += blockDim.x) {
-    const float r = __ldcg(rews + i);
-    if (isfinite(r)) { const float d = r - rbar; st[0] += 1.f; st[1] += d; st[2] += d * d; dmax = fmaxf(dmax, d); }
-  }
-  block_reduce<3>(st, &dmax, red);
-  const float cnt = st[0];
-  const float mean = st[1] / fmaxf(cnt, 1.f);
-  const float sd = sqrtf(fmaxf(st[2] / fmaxf(cnt, 1.f) - mean * mean, 0.f));
-  const float inv = (sd > 0.f) ? 1.f / sd / temp : 0.f;
-  const float mx = dmax * inv;
+  // ---- softmax parameters over the finite rewards (the same function as weights_kernel) -----------
+  const SoftmaxParams sp = reward_softmax_params(rews, n, temp, red);
   // ---- this CTA's share of sum e_n Y0s_n (thread -> (sample slot, knot element)) and sum e_n ------------
   const int ne = Hn1 * nu;
   const int slots = YBAR_THREADS / ne;
@@ -337,8 +376,8 @@ __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __res
     const uint32_t ntot = (uint32_t)Ntotal * (uint32_t)ne;
     for (int s_ = blockIdx.x * slots + slot; s_ <= Ntotal; s_ += gridDim.x * slots) {
       const float r = __ldcg(rews + s_);
-      float e = isfinite(r) ? expf((r - rbar) * inv - mx) : 0.f;
-      if (cnt == 0.f) e = (s_ == Ntotal) ? 1.f : 0.f;       // no finite reward: keep the mean sample
+      float e = isfinite(r) ? expf((r - sp.shift) * sp.inv - sp.mx) : 0.f;
+      if (sp.none) e = (s_ == Ntotal) ? 1.f : 0.f;          // no finite reward: keep the mean sample
       float y = yb;
       if (s_ < Ntotal && k > 0) {
         const uint32_t idx = (uint32_t)s_ * (uint32_t)ne + (uint32_t)el;
@@ -351,7 +390,7 @@ __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __res
   }
   acc[tid] = a;
   float zz[1] = {z};
-  block_reduce<1>(zz, nullptr, red);
+  block_reduce<float, 1>(zz, nullptr, red);
   __syncthreads();
   if (tid < ne) {
     float s_ = 0.f;
@@ -896,6 +935,30 @@ extern "C" int dial_reverse_update_x(dial_plan* p, const float* eps, const uint3
   return 0;
 }
 
+// The fused update of every instance of the plan: the one launch of update_kernel, used by the
+// control-step graph (mpc_enqueue) and by dial_reverse_update_fused.  Grid upd_grid x n_inst over the
+// plan's partials and per-instance counters.
+static int launch_update(dial_plan* p, const float* rews, float* weights, const XchWait& X, uint32_t* rng,
+                         const float* Ybar, const float* noise, float* Ybar_out, cudaStream_t st) {
+  const dial_plan_desc& c = p->hP.c;
+  update_kernel<<<dim3(p->upd_grid, p->n_inst), YBAR_THREADS, 0, st>>>(rews, c.Ntotal + 1, c.temp_sample, weights, X, rng, Ybar,
+                                                                     noise, c.Ntotal, c.Hnode + 1, p->hM.m.nu, p->partial,
+                                                                     p->counter, Ybar_out);
+  p->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dial_reverse_update_fused(dial_plan* p, const float* rews, uint32_t* rng, const float* Ybar,
+                                         const float* noise_scale, float* Ybar_out, float* weights, void* stream) {
+  if (!p || !rews || !rng || !Ybar || !noise_scale || !Ybar_out || !weights) return fail("dial_reverse_update_fused: null argument");
+  const dial_plan_desc& c = p->hP.c;
+  if (c.Ntotal != c.Nsample) return fail("dial_reverse_update_fused: sharded plans (Ntotal != Nsample) are not supported");
+  if (c.Ntotal + 1 > (1 << 17)) return fail("dial_reverse_update_fused: needs Ntotal + 1 <= 131072 (the fused update)");
+  XchWait X; memset(&X, 0, sizeof(X));
+  return launch_update(p, rews, weights, X, rng, Ybar, noise_scale, Ybar_out, (cudaStream_t)stream);
+}
+
 // the bars of every instance of the plan (the control-step graph; the public call below is single-instance)
 static int enqueue_trajbar(dial_plan* p, const float* weights, int rank, float* qbar, float* qdbar, float* xbar,
                            cudaStream_t st) {
@@ -1097,10 +1160,8 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     float* w = wts[i & 1];
     XchWait X = xch_wait_args(p, B.rews_all);
     if (fused) {
-      update_kernel<<<dim3(p->upd_grid, ni), YBAR_THREADS, 0, st>>>(B.rews, c.Ntotal + 1, c.temp_sample, w, X, B.rng, Y[cur], noise, c.Ntotal,
-                                                          n1, nu, p->partial, p->counter, Y[cur ^ 1]);
-      p->launches++;
-      CUDA_OK(cudaGetLastError());
+      int rc = launch_update(p, B.rews, w, X, B.rng, Y[cur], noise, Y[cur ^ 1], st);
+      if (rc) return rc;
     } else {
       weights_kernel<<<1, 1024, 0, st>>>(B.rews, c.Ntotal + 1, c.temp_sample, w, X);
       p->launches++;

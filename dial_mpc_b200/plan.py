@@ -171,6 +171,15 @@ class Plan:
                                                    _ptr(rews_all), _ptr(Ybar_out), _ptr(weights), _ptr(rews_gathered),
                                                    _stream()))
 
+    def reverse_update_fused(self, rews, rng, Ybar, noise_scale, Ybar_out, weights):
+        """The control-step graph's update (one fused kernel launch for every instance of the plan) on
+        caller buffers: rews [B,Ntotal+1], rng [B,2] int32 (the uint32 key bits; advanced in place to
+        ``split(rng)[0]``), Ybar / Ybar_out [B,Hn+1,nu], noise_scale [Hn+1], weights [B,Ntotal+1] out.
+        A single-instance plan takes the same tensors without the leading B."""
+        assert rng.is_cuda and rng.dtype == torch.int32 and rng.is_contiguous(), "rng: contiguous int32 CUDA tensor"
+        self._check(self.lib.dial_reverse_update_fused(self.handle, _ptr(rews), C.c_void_p(rng.data_ptr()), _ptr(Ybar),
+                                                       _ptr(noise_scale), _ptr(Ybar_out), _ptr(weights), _stream()))
+
     # -- multi-GPU exchange over NVLink peer memory (include/dial_b200.h: dial_exchange_*) -------------
     def exchange_setup(self, rank: int, world: int, group=None) -> None:
         """Create this rank's mailbox, all-gather the CUDA IPC handles over ``torch.distributed`` and

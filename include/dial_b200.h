@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define DIAL_ABI_VERSION 10
+#define DIAL_ABI_VERSION 11
 
 /* capacities of the fixed-size device model */
 #define DIAL_MAXB 24   /* bodies incl. world            */
@@ -260,6 +260,17 @@ int dial_reverse_update(dial_plan* plan, const float* eps, const uint32_t key[2]
 int dial_reverse_update_x(dial_plan* plan, const float* eps, const uint32_t key[2],
                           const float* Ybar, const float* noise_scale, const float* rews_all,
                           float* Ybar_out, float* weights, float* rews_gathered, void* stream);
+
+/* Stage 2 as the control-step graph runs it (dial_mpc_step): ONE launch of the fused update kernel
+ * (statistics, softmax, Ybar = sum_n w_n Y0s_n with Y0s regenerated from the Threefry stream keyed
+ * by split(rng)[1], rng advance) on caller buffers, for every instance of the plan (B = n_inst,
+ * 1 for a single-instance plan).  All [dev]: rews [B][Ntotal+1] (mean sample last); rng [B][2],
+ * read and advanced in place to split(rng)[0]; Ybar and Ybar_out [B][Hn+1][nu]; noise_scale [Hn+1];
+ * weights [B][Ntotal+1] out.  Uses the plan's partials and counters like the graph does, so it must
+ * not run concurrently with dial_mpc_step on the same plan.  Fails for sharded plans
+ * (Ntotal != Nsample) and for Ntotal + 1 > 131072. */
+int dial_reverse_update_fused(dial_plan* plan, const float* rews, uint32_t* rng, const float* Ybar,
+                              const float* noise_scale, float* Ybar_out, float* weights, void* stream);
 
 /* qbar/qdbar/xbar (core/dial_core.py:133-135): weighted sums of this rank's stored
  * trajectories with `weights` [dev][Ntotal+1]; sharded runs sum the outputs across

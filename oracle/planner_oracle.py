@@ -34,6 +34,44 @@ def spline_matrix(x_from: np.ndarray, x_to: np.ndarray) -> np.ndarray:
     return M
 
 
+def make_Y0s(eps, Ybar, noise_scale):
+    """Y0s = eps * noise + Ybar with node 0 pinned, the mean row Ybar appended, clipped to [-1, 1]
+    (dial_core.py:107-116)."""
+    Y0s = eps * noise_scale[None, :, None] + Ybar
+    Y0s[:, 0] = Ybar[0]
+    Y0s = np.concatenate([Y0s, Ybar[None]], 0)
+    return np.clip(Y0s, -1.0, 1.0)
+
+
+def softmax_weights_fp64(rews, temp):
+    """The update's weights softmax((rews - rews[-1]) / std(rews) / temp) (dial_core.py:125-128) in
+    fp64, with the guards of the CUDA kernels (the reference has none):
+    * non-finite rewards get weight 0 and are left out of the statistics;
+    * softmax is shift-invariant, so a non-finite mean-row reward rews[-1] changes nothing (the
+      logits are taken relative to the largest finite reward);
+    * flat finite rewards (std 0) give uniform weights over the finite samples;
+    * no finite reward at all puts the whole weight on the mean row."""
+    r = np.asarray(rews, dtype=np.float64)
+    fin = np.isfinite(r)
+    w = np.zeros_like(r)
+    if not fin.any():
+        w[-1] = 1.0
+        return w
+    rf = r[fin]
+    sd = rf.std()                      # two-pass (mean first): no cancellation
+    e = np.exp((rf - rf.max()) / sd / temp) if sd > 0 else np.ones_like(rf)
+    w[fin] = e / e.sum()
+    return w
+
+
+def reverse_update_fp64(rews, temp, eps, Ybar, noise_scale):
+    """Weights and Ybar_new = sum_n w_n Y0s_n of one reverse_once update in fp64: the reference for
+    the CUDA update kernels on given rewards.  eps [N, Hn+1, nu], rews [N+1] (mean row last)."""
+    w = softmax_weights_fp64(rews, temp)
+    Y0s = make_Y0s(np.asarray(eps, np.float64), np.asarray(Ybar, np.float64), np.asarray(noise_scale, np.float64))
+    return w, np.einsum("n,nij->ij", w, Y0s)
+
+
 class PlannerOracle:
     def __init__(self, env: OracleEnv, Nsample, Hsample, Hnode, temp_sample,
                  horizon_diffuse_factor, traj_diffuse_factor, sigma_scale=1.0):
@@ -62,10 +100,7 @@ class PlannerOracle:
         return self.u2node(u)
 
     def make_Y0s(self, eps, Ybar, noise_scale):
-        Y0s = eps * noise_scale[None, :, None] + Ybar
-        Y0s[:, 0] = Ybar[0]
-        Y0s = np.concatenate([Y0s, Ybar[None]], 0)
-        return np.clip(Y0s, -1.0, 1.0)
+        return make_Y0s(eps, Ybar, noise_scale)
 
     def reverse_once(self, state: OState, eps, Ybar, noise_scale) -> Tuple[np.ndarray, Dict]:
         Y0s = self.make_Y0s(eps, Ybar, noise_scale)
@@ -161,11 +196,53 @@ def sample_jump_sequence_oracle(rng, n_steps=10):
     return np.array(pos), np.array(yaw)
 
 
-def jax_normal_legacy(key, shape):
-    """jax.random.normal(key, shape, float32): sqrt(2)*erfinv(uniform(-1+ulp, 1))."""
-    n = int(np.prod(shape))
+def _normal_uniform_legacy(key, n):
+    """The fp32 uniform in (-1, 1) that jax.random.normal feeds to erfinv (legacy layout)."""
     bits = jax_random_bits_legacy(key, n)
     f = ((bits >> np.uint32(9)) | np.uint32(0x3F800000)).view(np.float32) - np.float32(1.0)
     lo = np.nextafter(np.float32(-1.0), np.float32(0.0))
-    u = np.maximum(lo, f * (np.float32(1.0) - lo) + lo).astype(np.float32)
+    return np.maximum(lo, f * (np.float32(1.0) - lo) + lo).astype(np.float32)
+
+
+def jax_normal_legacy(key, shape):
+    """jax.random.normal(key, shape, float32): sqrt(2)*erfinv(uniform(-1+ulp, 1))."""
+    u = _normal_uniform_legacy(key, int(np.prod(shape)))
     return (np.sqrt(2.0) * erfinv(u.astype(np.float64))).reshape(shape)
+
+
+ERFINV_TAIL_W = 5.0
+
+
+def erfinv_xla(u):
+    """XLA's single-precision erfinv (Giles' polynomials: the algorithm jax.random.normal runs in
+    float32, and the kernels' erfinv_f32) in fp64, except for u * u, which is rounded to fp32 before
+    log1p as in float32.  Near |u| = 1 that one rounding is amplified by 1 / (1 - u^2): at |u| = 0.9999
+    it moves eps by about 50 fp32 ulp away from the exact sqrt(2) erfinv(u).  Elsewhere the polynomials
+    are within about 2 ulp of the exact function."""
+    x = np.asarray(u, dtype=np.float32)
+    w = -np.log1p(-(x * x).astype(np.float64))
+    x = x.astype(np.float64)
+    lo = w < ERFINV_TAIL_W
+    t = np.where(lo, w - 2.5, np.sqrt(w) - 3.0)
+    p = np.where(lo, 2.81022636e-08, -0.000200214257)
+    for a, b in zip((3.43273939e-07, -3.5233877e-06, -4.39150654e-06, 0.00021858087, -0.00125372503, -0.00417768164,
+                     0.246640727, 1.50140941),
+                    (0.000100950558, 0.00134934322, -0.00367342844, 0.00573950773, -0.0076224613, 0.00943887047,
+                     1.00167406, 2.83297682)):
+        p = np.where(lo, a, b) + p * t
+    return p * x
+
+
+def jax_normal_legacy_xla(key, shape):
+    """jax_normal_legacy with XLA's float32 erfinv algorithm (:func:`erfinv_xla`) instead of the exact
+    erfinv: what the kernels' sampler computes, up to the fp32 rounding of the remaining steps."""
+    u = _normal_uniform_legacy(key, int(np.prod(shape)))
+    return (np.sqrt(2.0) * erfinv_xla(u)).reshape(shape)
+
+
+def erfinv_tail_indices(key, n):
+    """Flat indices i < n of jax.random.normal(key, (n,)) (legacy layout) whose uniform u takes the
+    tail branch of XLA's single-precision erfinv, w = -log(1 - u^2) >= 5: |u| > 0.9966, |eps| > 2.93
+    (about 0.37 % of the elements).  The kernels' sampler evaluates that branch only there."""
+    u = _normal_uniform_legacy(key, n).astype(np.float64)
+    return np.flatnonzero(-np.log1p(-u * u) >= ERFINV_TAIL_W)
