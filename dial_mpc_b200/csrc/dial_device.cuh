@@ -182,6 +182,84 @@ struct RolloutArgs {
 };
 
 // ---------------------------------------------------------------------------------
+// Integer structure of the env step as a template policy.  The warp-uniform bounds and selectors the
+// env step reads (body / dof / contact counts, tree depth, star chains, pair kind, solver iteration
+// counts, physics steps per env step, the reward's environment) come from `SH`:
+//   ShapeRT     reads them from the staged model and plan (every model);
+//   ShapeFixed  returns the model's structure as compile-time constants (-DDIAL_SHAPE_*: a specialised
+//               kernel, built for one model and selected only for plans whose values all match, see
+//               shape_matches).  Loops then get constant trip counts and dead branches drop out.
+// Lane-varying tables (body depth, joint type, chains, star positions) and every float constant stay
+// run-time data: the arithmetic of each row is the same in both kernels, bit for bit.
+// ---------------------------------------------------------------------------------
+struct ShapeRT {
+  static HD int nbody(const DevModel& M) { return M.m.nbody; }
+  static HD int nq(const DevModel& M) { return M.m.nq; }
+  static HD int nv(const DevModel& M) { return M.m.nv; }
+  static HD int nu(const DevModel& M) { return M.m.nu; }
+  static HD int maxdepth(const DevModel& M) { return M.maxdepth; }
+  static HD int nroot(const DevModel& M) { return M.nroot; }
+  static HD int ncon(const DevModel& M) { return M.m.ncon; }
+  static HD int nedge(const DevModel& M) { return M.nedge; }
+  static HD int nchain(const DevModel& M) { return M.star_nchain; }
+  static HD int sb_on(const DevModel& M) { return M.sb_on; }
+  static HD int sb_nroot(const DevModel& M) { return M.sb_nroot; }
+  static HD int sb_len(const DevModel& M, int l) { return M.sb_len[l]; }
+  static HD int pair_kind(const DevModel& M, int k) { return M.m.pair_kind[k]; }
+  static HD int iterations(const DevModel& M) { return M.m.iterations; }
+  static HD int ls_iterations(const DevModel& M) { return M.m.ls_iterations; }
+  static HD int n_frames(const dial_plan_desc& c) { return c.n_frames; }
+  static HD int env_id(const dial_plan_desc& c) { return c.env_id; }
+  static HD int nfeet(const dial_plan_desc& c) { return c.nfeet; }
+};
+
+#ifdef DIAL_SHAPE_NBODY
+// Internal linkage: a specialised unit's rollout_kernel<3, 6, ShapeFixed> and shape_matches<ShapeFixed>
+// hold its own values and must not be merged with another unit's at link time.  The contact count and the
+// plan's selectors (env_id, nfeet, n_frames) stay run-time values (inherited from ShapeRT): fixing them
+// lets the compiler merge code across branches that are taken at run time and fuse a different set of
+// multiply-adds, which changes the fp32 rounding of the rows (measured on H100: rewards differ in the
+// last bits); the fields below leave every row bit for bit as the generic kernel computes it.
+namespace {
+struct ShapeFixed : ShapeRT {
+  static HD constexpr int nbody(const DevModel&) { return DIAL_SHAPE_NBODY; }
+  static HD constexpr int nq(const DevModel&) { return DIAL_SHAPE_NQ; }
+  static HD constexpr int nv(const DevModel&) { return DIAL_SHAPE_NV; }
+  static HD constexpr int nu(const DevModel&) { return DIAL_SHAPE_NU; }
+  static HD constexpr int maxdepth(const DevModel&) { return DIAL_SHAPE_MAXDEPTH; }
+  static HD constexpr int nroot(const DevModel&) { return DIAL_SHAPE_NROOT; }
+  static HD constexpr int nchain(const DevModel&) { return DIAL_SHAPE_NCHAIN; }
+  static HD constexpr int sb_on(const DevModel&) { return 1; }
+  static HD constexpr int sb_nroot(const DevModel&) { return DIAL_SHAPE_SB_NROOT; }
+  static HD constexpr int sb_len(const DevModel&, int) { return DIAL_SHAPE_CHAINLEN; }   // every chain
+  static HD constexpr int pair_kind(const DevModel&, int) { return DIAL_SHAPE_PAIR_KIND; }  // every pair
+  static HD constexpr int iterations(const DevModel&) { return DIAL_SHAPE_ITERATIONS; }
+  static HD constexpr int ls_iterations(const DevModel&) { return DIAL_SHAPE_LS_ITERATIONS; }
+};
+}  // namespace
+#endif
+
+// Whether a kernel compiled for policy SH computes what the run-time kernel computes for this model and
+// plan: every value SH fixes equals the model's / plan's own.
+template <class SH>
+static inline bool shape_matches(const DevModel& M, const dial_plan_desc& c) {
+  using R = ShapeRT;
+  if (!M.s_on || !R::sb_on(M) || SH::sb_on(M) != R::sb_on(M)) return false;
+  if (SH::nbody(M) != R::nbody(M) || SH::nq(M) != R::nq(M) || SH::nv(M) != R::nv(M) || SH::nu(M) != R::nu(M) ||
+      SH::maxdepth(M) != R::maxdepth(M) || SH::nroot(M) != R::nroot(M) || SH::ncon(M) != R::ncon(M) ||
+      SH::nedge(M) != R::nedge(M) || SH::nchain(M) != R::nchain(M) || SH::sb_nroot(M) != R::sb_nroot(M) ||
+      SH::iterations(M) != R::iterations(M) || SH::ls_iterations(M) != R::ls_iterations(M) ||
+      SH::n_frames(c) != R::n_frames(c) || SH::env_id(c) != R::env_id(c) || SH::nfeet(c) != R::nfeet(c))
+    return false;
+  for (int l = 0; l < R::nchain(M); ++l) if (SH::sb_len(M, l) != R::sb_len(M, l)) return false;
+  for (int k = 0; k < R::ncon(M); ++k) {
+    const int p = M.con_pair[k];
+    if (SH::pair_kind(M, p) != R::pair_kind(M, p)) return false;
+  }
+  return true;
+}
+
+// ---------------------------------------------------------------------------------
 // small vector / quaternion helpers
 // ---------------------------------------------------------------------------------
 struct V3 { float x, y, z; };
@@ -860,7 +938,7 @@ DEV void star_store_row(float* p, const float* Rr, const float* Rc) {
 }
 
 // y = M x and (edge lanes) J x with one publication of x.  Mr/Mc: this lane's row of M.
-template <int NL, int NR, bool WITH_M, bool WITH_J>
+template <int NL, int NR, bool WITH_M, bool WITH_J, class SH = ShapeRT>
 DEV void star_mul_MJ(WarpCtx& w, const float* Mr, const float* Mc, float x, float& Mx, float& Jx) {
   using SD = StarDims<NL, NR>;
   const DevModel& M = *w.M;
@@ -885,7 +963,7 @@ DEV void star_mul_MJ(WarpCtx& w, const float* Mr, const float* Mc, float x, floa
   } else if (w.s_chain == -1) {
     // root dof: the coupling column, sum over every chain slot of M[slot dof][root a] x[slot dof]
     const float* col = Ms + SD::NRP * SD::RS + w.s_col;
-    const int nslot = M.star_nchain * SD::CS;
+    const int nslot = SH::nchain(M) * SD::CS;
     for (int s0 = 0; s0 < nslot; s0 += 4) {
       F4 xv = ld4(xs + SD::NRP + s0);
       y0 += col[(s0 + 0) * SD::RS] * xv.x; y1 += col[(s0 + 1) * SD::RS] * xv.y;
@@ -897,7 +975,7 @@ DEV void star_mul_MJ(WarpCtx& w, const float* Mr, const float* Mc, float x, floa
   Mx = y;
   if (WITH_J) {
     float j = 0.f;
-    if (w.lane < M.nedge) {
+    if (w.lane < SH::nedge(M)) {
       const float* row = SM(Js) + w.lane * SD::RS;
       float jr[SD::NRP], jc[SD::CS], xe[SD::CS];
       ldv<NR>(row, jr);
@@ -915,7 +993,7 @@ DEV void star_mul_MJ(WarpCtx& w, const float* Mr, const float* Mc, float x, floa
 }
 
 // J^T f: edge lane e holds f_e; dof lane returns sum_e J[e][my column] f_e
-template <int NL, int NR>
+template <int NL, int NR, class SH = ShapeRT>
 DEV float star_mul_JT(WarpCtx& w, float f) {
   using SD = StarDims<NL, NR>;
   const DevModel& M = *w.M;
@@ -926,7 +1004,7 @@ DEV float star_mul_JT(WarpCtx& w, float f) {
   syncwarp();
   float y0 = 0.f, y1 = 0.f, y2 = 0.f, y3 = 0.f;   // independent partial sums (dependent-issue latency)
   const float* col = Js + w.s_col;
-  for (int c = 0; c < M.m.ncon; ++c) {
+  for (int c = 0; c < SH::ncon(M); ++c) {
     const F4 fv = ld4(frow + 4 * c);
     if ((w.s_conmask >> c) & 1u) {
       const float* jc = col + 4 * c * SD::RS;
@@ -937,7 +1015,7 @@ DEV float star_mul_JT(WarpCtx& w, float f) {
 }
 
 // H row of this lane: M + active limit + sum over active edges d_e j_e^T j_e
-template <int NL, int NR>
+template <int NL, int NR, class SH = ShapeRT>
 DEV void star_build_H(WarpCtx& w, const Solver& S, const float* Mr, const float* Mc, float* Rr, float* Rc) {
   using SD = StarDims<NL, NR>;
   const DevModel& M = *w.M;
@@ -958,7 +1036,7 @@ DEV void star_build_H(WarpCtx& w, const Solver& S, const float* Mr, const float*
 #pragma unroll
     for (int a = 0; a < NR; ++a) Rr[a] += (a == w.s_depth) ? ld : 0.f;
   }
-  for (int e = 0; e < M.nedge; ++e) {
+  for (int e = 0; e < SH::nedge(M); ++e) {
     const float de = frow[e];
     if (de == 0.f) continue;                           // warp-uniform
     const float* row = Js + e * SD::RS;
@@ -976,7 +1054,7 @@ DEV void star_build_H(WarpCtx& w, const Solver& S, const float* Mr, const float*
 
 // Solve H x = g for the star structure (block elimination, see star_solve above); rows in the
 // star layout are published once and gathered with compile-time offsets.
-template <int NL, int NR>
+template <int NL, int NR, class SH = ShapeRT>
 DEV float star_solve2(WarpCtx& w, const float* Rr, const float* Rc, float g) {
   using SD = StarDims<NL, NR>;
   static_assert(NR + 1 <= 8, "root block + rhs must fit the 8 lanes of a group");
@@ -991,7 +1069,7 @@ DEV float star_solve2(WarpCtx& w, const float* Rr, const float* Rc, float g) {
   }
   syncwarp();
   const int grp = lane >> 3, j = lane & 7, gbase = lane & ~7;
-  const bool ischain = grp < M.star_nchain;
+  const bool ischain = grp < SH::nchain(M);
   const int len = ischain ? M.star_len[grp] : 0;
   const int cb = SD::NRP + grp * SD::CS;
   // ---- gather: chain block A (whole group) and this lane's column of [C | g] -------------------
@@ -1122,11 +1200,11 @@ DEV float star_solve2(WarpCtx& w, const float* Rr, const float* Rc, float g) {
 }
 
 // efc_force, qfrc_constraint, costs and the gradient in the star layout
-template <int NL, int NR>
+template <int NL, int NR, class SH = ShapeRT>
 DEV void star_update_constraint(WarpCtx& w, Solver& S) {
   float fl = (S.l_Jaref < 0.f) ? -S.l_D * S.l_Jaref : 0.f;
   float fe = (S.e_Jaref < 0.f) ? -S.e_D * S.e_Jaref : 0.f;
-  float qfc = star_mul_JT<NL, NR>(w, fe) + S.l_sign * fl;
+  float qfc = star_mul_JT<NL, NR, SH>(w, fe) + S.l_sign * fl;
   S.grad = S.Ma - S.qfs - qfc;
   float g = (S.Ma - S.qfs) * (S.qacc - S.qas);
   float c = ((S.l_Jaref < 0.f) ? S.l_D * S.l_Jaref * S.l_Jaref : 0.f)
@@ -1223,9 +1301,10 @@ DEV void ls_points(int lane, const Solver& S, const LSRow& K, float l_jv, float 
 }
 
 // MJX solver._linesearch given M.search (mv) and J.search (e_jv) of this lane's rows
+template <class SH = ShapeRT>
 DEV void linesearch_core(WarpCtx& w, Solver& S, float mv, float e_jv) {
   const DevModel& M = *w.M;
-  const int nv = M.m.nv;
+  const int nv = SH::nv(M);
   const float scale = M.m.meaninertia * (float)(nv > 1 ? nv : 1);
   float l_jv = S.l_sign * S.search;
   float ss = S.search * S.search, sMa = S.search * (S.Ma - S.qfs), sMv = S.search * mv;
@@ -1242,7 +1321,8 @@ DEV void linesearch_core(WarpCtx& w, Solver& S, float mv, float e_jv) {
   ls_points<1, false>(w.lane, S, K, l_jv, e_jv, qg, a1, &lo);
   if (lo.d0 < p0.d0) { hi = p0; } else { hi = lo; lo = p0; }
   bool swap = true;
-  for (int it = 0; it < M.m.ls_iterations; ++it) {
+#pragma unroll 1
+  for (int it = 0; it < SH::ls_iterations(M); ++it) {
     bool done = !swap;
     done |= (lo.d0 < 0.f) && (lo.d0 > -gtol);
     done |= (hi.d0 > 0.f) && (hi.d0 < gtol);
@@ -1976,11 +2056,12 @@ DEV V3 frame_tangent(V3 n) {   // second row of mjx math.make_frame(n)
   return vnormalize(alt - n * dot(n, alt), bn);
 }
 
+template <class SH = ShapeRT>
 DEV void collide(WarpCtx& w) {
   const DevModel& M = *w.M;
   const dial_model_desc& m = M.m;
   const int lane = w.lane;
-  if (lane >= m.ncon) return;
+  if (lane >= SH::ncon(M)) return;
   const float* xpos = SM(xpos);
   const float* xmat = SM(xmat);
   const int k = M.con_pair[lane];
@@ -1990,7 +2071,7 @@ DEV void collide(WarpCtx& w) {
   const float* X2 = xmat + 9 * b2;
   const V3 gp1 = mat_apply(X1, m.geom_pos[g1]) + ld3(xpos + 3 * b1);
   const V3 gp2 = mat_apply(X2, m.geom_pos[g2]) + ld3(xpos + 3 * b2);
-  const int kind = m.pair_kind[k];
+  const int kind = SH::pair_kind(M, k);
   V3 n, t1, p;
   float dist;
   if (kind == PAIR_PLANE_SPHERE || kind == PAIR_PLANE_CAPSULE) {
@@ -2040,12 +2121,12 @@ DEV void collide(WarpCtx& w) {
 // one physics step (mjx.step) for the warp's sample.  State (qpos,qvel,warm,ctrl) in
 // the slab; kinematic arrays of the forward pass are left in the slab for the reward.
 // ---------------------------------------------------------------------------------
-template <int NL, int NR>
+template <int NL, int NR, class SH = ShapeRT>
 DEV void physics_step(WarpCtx& w, bool integrate) {
   constexpr int MCU = (NL == 3 && NR == 6) ? 9 : DIAL_MAXCHAIN;  // longest dof chain of the variant
   const DevModel& M = *w.M;
   const dial_model_desc& m = M.m;
-  const int lane = w.lane, nb = m.nbody, nv = m.nv;
+  const int lane = w.lane, nb = SH::nbody(M), nv = SH::nv(M);
   float* xpos = SM(xpos); float* xquat = SM(xquat); float* xmat = SM(xmat); float* xipos = SM(xipos);
   float* cinert = SM(cinert); float* cdof = SM(cdof); float* cdofdot = SM(cdofdot);
   float* cvel = SM(cvel); float* cacc = SM(cacc); float* cfrc = SM(cfrc);
@@ -2089,7 +2170,7 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
   }
   V3 pos = v3(0, 0, 0);
   Q4 quat; quat.w = 1.f; quat.x = quat.y = quat.z = 0.f;
-  for (int lv = 1; lv <= M.maxdepth; ++lv) {
+  for (int lv = 1; lv <= SH::maxdepth(M); ++lv) {
     if (depth == lv) {
       if (jtype == JNT_FREE) {
         const int qa = m.jnt_qposadr[jid];
@@ -2126,7 +2207,7 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
   // ---- 2. subtree COM of each tree root --------------------------------------------
   const int myroot = isbody ? M.body_rootidx[b] : -1;
   V3 com = v3(0, 0, 0);
-  for (int r = 0; r < M.nroot; ++r) {
+  for (int r = 0; r < SH::nroot(M); ++r) {
     float mass = (myroot == r) ? m.body_mass[b] : 0.f;
     float sx = mass * xip.x, sy = mass * xip.y, sz = mass * xip.z;
     warp_sum3(sx, sy, sz);
@@ -2181,7 +2262,7 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
 
   // ---- 4. velocities / accelerations down the tree, local RNE force ---------------------
   float mycv[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, myca[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  for (int lv = 1; lv <= M.maxdepth; ++lv) {
+  for (int lv = 1; lv <= SH::maxdepth(M); ++lv) {
     if (depth == lv) {
       int p = m.body_parentid[b];
       float cv[6], ca[6];
@@ -2256,20 +2337,20 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
     const float* src = comp < 10 ? cinert + comp : cfrc + (comp - 10);
     const int stride = comp < 10 ? CIS : 6;
     float* dst = comp < 10 ? crb + comp : cfs + (comp - 10);
-    if (NL > 0 && M.sb_on) {
+    if (NL > 0 && SH::sb_on(M)) {
       // star models: suffix sums along each hanging chain (half-warp h takes chains h and h + 2),
       // then the root bodies, deepest first, collect their child root and the chains hanging off them
-      for (int l = half; l < M.star_nchain; l += 2) {
+      for (int l = half; l < SH::nchain(M); l += 2) {
         const int top = M.sb_top[l];
         float acc = 0.f;
-        for (int k = M.sb_len[l] - 1; k >= 0; --k) { acc += src[(top + k) * stride]; dst[(top + k) * stride] = acc; }
+        for (int k = SH::sb_len(M, l) - 1; k >= 0; --k) { acc += src[(top + k) * stride]; dst[(top + k) * stride] = acc; }
       }
       syncwarp();
       if (half == 0) {
         float below = 0.f;
-        for (int r = 0; r < M.sb_nroot; ++r) {
+        for (int r = 0; r < SH::sb_nroot(M); ++r) {
           float acc = src[M.sb_root[r] * stride] + below;
-          for (int l = 0; l < M.star_nchain; ++l)
+          for (int l = 0; l < SH::nchain(M); ++l)
             if (M.sb_att[l] == r) acc += dst[M.sb_top[l] * stride];
           dst[M.sb_root[r] * stride] = acc;
           below = acc;
@@ -2290,7 +2371,7 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
   syncwarp();
 
   // ---- 7. collision (lane = contact) ---------------------------------------------------
-  collide(w);
+  collide<SH>(w);
   syncwarp();
 
   // ---- 6. compact mass-matrix row, bias, smooth force (lane = dof) ----------------------
@@ -2405,7 +2486,7 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
   if (isdof) {
     V3 ca_ = v3(mycdof[0], mycdof[1], mycdof[2]), cl_ = v3(mycdof[3], mycdof[4], mycdof[5]);
     V3 rc = ld3(rcom + 3 * M.body_rootidx[m.dof_bodyid[d]]);
-    for (int c = 0; c < m.ncon; ++c) {
+    for (int c = 0; c < SH::ncon(M); ++c) {
       if (!((w.s_conmask >> c) & 1u)) continue;   // my column is structurally zero in this contact's rows
       const int k = M.con_pair[c];
       float e0 = 0.f, e1 = 0.f, e2 = 0.f, e3 = 0.f;
@@ -2437,8 +2518,8 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
     }
   }
   float ejv, dummy;
-  star_mul_MJ<NL, NR, false, true>(w, Mr, Mc, myqvel, dummy, ejv);
-  if (lane < M.nedge) {
+  star_mul_MJ<NL, NR, false, true, SH>(w, Mr, Mc, myqvel, dummy, ejv);
+  if (lane < SH::nedge(M)) {
     int c = lane >> 2;
     int k = M.con_pair[c];
     float pos = cdist[c] - (m.pair_margin[k] - m.pair_gap[k]);
@@ -2471,13 +2552,13 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
   int it = 0;
   bool done;
   {
-    float x = star_solve2<NL, NR>(w, Rr, Rc, g);
+    float x = star_solve2<NL, NR, SH>(w, Rr, Rc, g);
     S.qas = x;
-    if (M.nedge == 0 && M.nlimited == 0) { S.qacc = x; done = true; }
+    if (SH::nedge(M) == 0 && M.nlimited == 0) { S.qacc = x; done = true; }
     else {
       float Maw, eJw, eJs;
-      star_mul_MJ<NL, NR, true, true>(w, Mr, Mc, mywarm, Maw, eJw);
-      star_mul_MJ<NL, NR, false, true>(w, Mr, Mc, S.qas, dummy, eJs);
+      star_mul_MJ<NL, NR, true, true, SH>(w, Mr, Mc, mywarm, Maw, eJw);
+      star_mul_MJ<NL, NR, false, true, SH>(w, Mr, Mc, S.qas, dummy, eJs);
       eJw -= S.e_aref; eJs -= S.e_aref;
       float lJw = S.l_sign * mywarm - S.l_aref;
       float gw = (Maw - S.qfs) * (mywarm - S.qas);
@@ -2493,9 +2574,9 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
       S.l_Jaref = usewarm ? lJw : lJs;
       S.cost = INFINITY;
       S.prev_cost = 0.f;
-      star_update_constraint<NL, NR>(w, S);
+      star_update_constraint<NL, NR, SH>(w, S);
       done = false;
-      if (m.iterations != 1) {
+      if (SH::iterations(M) != 1) {
         float improvement = (S.prev_cost - S.cost) / scale;
         float gradient = sqrtf(S.gradnorm2) / scale;
         done = (improvement < m.tolerance) || (gradient < m.tolerance);
@@ -2503,18 +2584,18 @@ DEV void physics_step(WarpCtx& w, bool integrate) {
     }
   }
   while (!done) {
-    star_build_H<NL, NR>(w, S, Mr, Mc, Rr, Rc);
-    float x = star_solve2<NL, NR>(w, Rr, Rc, S.grad);
+    star_build_H<NL, NR, SH>(w, S, Mr, Mc, Rr, Rc);
+    float x = star_solve2<NL, NR, SH>(w, Rr, Rc, S.grad);
     S.search = -x;
     float mv, e_jv;
-    star_mul_MJ<NL, NR, true, true>(w, Mr, Mc, S.search, mv, e_jv);
-    linesearch_core(w, S, mv, e_jv);
+    star_mul_MJ<NL, NR, true, true, SH>(w, Mr, Mc, S.search, mv, e_jv);
+    linesearch_core<SH>(w, S, mv, e_jv);
     ++it;
-    star_update_constraint<NL, NR>(w, S);
-    done = it >= m.iterations;
+    star_update_constraint<NL, NR, SH>(w, S);
+    done = it >= SH::iterations(M);
     float improvement = (S.prev_cost - S.cost) / scale;
     float gradient = sqrtf(S.gradnorm2) / scale;
-    if (m.iterations != 1) done = done || (improvement < m.tolerance) || (gradient < m.tolerance);
+    if (SH::iterations(M) != 1) done = done || (improvement < m.tolerance) || (gradient < m.tolerance);
   }
   qacc = S.qacc;
   qacc_int = qacc;
@@ -2702,24 +2783,26 @@ DEV BaseKin base_kin(WarpCtx& w, int bid) {
 // Per-foot / per-contact terms of the built-in rewards, one lane each (lanes 0..3), summed into
 // lane 0 by two xor-shuffles: [0] gait term (walk envs) or contact bonus (seq-jump), [1] penalty.
 // The task fields (commands, gait, stage tables, user constants) come from `T`, the rest from the plan.
+template <class SH = ShapeRT>
 DEV void reward_partials(WarpCtx& w, const dial_task& T, int step, int stage, float& p0, float& p1) {
   const DevModel& M = *w.M;
   const dial_plan_desc& c = w.P->c;
   const dial_model_desc& m = M.m;
   const float stepf = (float)step;
   const int f = w.lane;
+  const int env = SH::env_id(c);
   p0 = 0.f; p1 = 0.f;
-  if (c.env_id == DIAL_ENV_GO2_WALK || c.env_id == DIAL_ENV_H1_WALK || c.env_id == DIAL_ENV_H1_LOCO) {
-    if (f < c.nfeet) {
+  if (env == DIAL_ENV_GO2_WALK || env == DIAL_ENV_H1_WALK || env == DIAL_ENV_H1_LOCO) {
+    if (f < SH::nfeet(c)) {
       float zt = foot_step(T.gait_duty, T.gait_cadence, T.gait_amplitude, T.gait_phase[f], stepf * c.dt);
       float z;
-      if (c.env_id == DIAL_ENV_GO2_WALK) {
+      if (env == DIAL_ENV_GO2_WALK) {
         int sid = c.feet_site[f], sb = m.site_bodyid[sid];
         const float* X = SM(xmat) + 9 * sb;
         z = SM(xpos)[3 * sb + 2] + X[6] * m.site_pos[sid][0] + X[7] * m.site_pos[sid][1] + X[8] * m.site_pos[sid][2];
         float e = (zt - z) / 0.05f;
         p0 = -e * e;
-      } else if (c.env_id == DIAL_ENV_H1_WALK) {
+      } else if (env == DIAL_ENV_H1_WALK) {
         z = fminf(SM(cdist)[2 * f], SM(cdist)[2 * f + 1]);
         p0 = -(zt - z) * (zt - z);
       } else {   // H1 loco: two capsules (4 contacts) per foot
@@ -2727,7 +2810,7 @@ DEV void reward_partials(WarpCtx& w, const dial_task& T, int step, int stage, fl
         p0 = -(zt - z) * (zt - z);
       }
     }
-  } else if (c.env_id == DIAL_ENV_GO2_SEQJUMP) {
+  } else if (env == DIAL_ENV_GO2_SEQJUMP) {
     if (f < 4) {
       const int i = f;
       float dist = SM(cdist)[i];
@@ -2749,14 +2832,16 @@ DEV void reward_partials(WarpCtx& w, const dial_task& T, int step, int stage, fl
   p0 += shfl_xor(p0, 2); p1 += shfl_xor(p1, 2);
 }
 
+template <class SH = ShapeRT>
 DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, float part0, float part1) {
   const DevModel& M = *w.M;
   const dial_plan_desc& c = w.P->c;
   const dial_model_desc& m = M.m;
   const float stepf = (float)step;
+  const int env = SH::env_id(c);
   float rew = 0.f;
 #ifdef DIAL_CUSTOM_REWARD_FILE
-  if (c.env_id == DIAL_ENV_CUSTOM) {
+  if (env == DIAL_ENV_CUSTOM) {
     dial_reward_ctx x;
     x.step = step; x.dt = c.dt;
     x.nq = m.nq; x.nv = m.nv; x.nu = m.nu; x.nbody = m.nbody; x.ncon = m.ncon; x.nsite = m.nsite; x.n_user = T.n_user;
@@ -2773,17 +2858,17 @@ DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, flo
   V3 up = qrot(rot0, v3(0, 0, 1));
   float r_upright = -(up.x * up.x + up.y * up.y + (up.z - 1.f) * (up.z - 1.f));
   BaseKin bk = base_kin(w, c.torso_body);
-  if (c.env_id == DIAL_ENV_ALLEGRO) {
+  if (env == DIAL_ENV_ALLEGRO) {
     // manipulation.py:75-84: ball angular velocity / position tracking + joint deviation
     const int ob = c.torso_body;
     V3 wv = ld3(SM(cvel) + 6 * ob) * (3.14159265358979f / 180.f);
     V3 dw = wv - ld3(T.ang_cmd);
     V3 dp = ld3(SM(xpos) + 3 * ob) - ld3(T.pos_tar);
     float rj = 0.f;
-    for (int a = 0; a < m.nu; ++a) { float e = SM(qpos)[7 + a] - c.joint_offset[a]; rj -= e * e; }
+    for (int a = 0; a < SH::nu(M); ++a) { float e = SM(qpos)[7 + a] - c.joint_offset[a]; rj -= e * e; }
     return -dot(dw, dw) - 5.f * dot(dp, dp) + 0.1f * rj;
   }
-  if (c.env_id == DIAL_ENV_GO2_WALK || c.env_id == DIAL_ENV_H1_WALK || c.env_id == DIAL_ENV_H1_LOCO) {
+  if (env == DIAL_ENV_GO2_WALK || env == DIAL_ENV_H1_WALK || env == DIAL_ENV_H1_LOCO) {
     float ramp = stepf * c.dt / c.ramp_up_time;
     // randomize_tasks: a one-step command override (dial_plan_set_command / the task's cmd_step)
     const float* vel_cmd = step == T.cmd_step ? T.cmd_vel : T.vel_cmd;
@@ -2799,23 +2884,23 @@ DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, flo
     float r_vel = -((bk.vb.x - vtx) * (bk.vb.x - vtx) + (bk.vb.y - vty) * (bk.vb.y - vty));
     float r_ang = -(bk.ab.z - atz) * (bk.ab.z - atz);
     float r_h = -(bk.pos.z - T.pos_tar[2]) * (bk.pos.z - T.pos_tar[2]);
-    if (c.env_id == DIAL_ENV_GO2_WALK) {
+    if (env == DIAL_ENV_GO2_WALK) {
       rew = 0.1f * r_gaits + 0.5f * r_upright + 0.3f * r_yaw + r_vel + r_ang + r_h;
-    } else if (c.env_id == DIAL_ENV_H1_LOCO) {
+    } else if (env == DIAL_ENV_H1_LOCO) {
       // unitree_h1_env.py:774-800: all three body-rate components, foot-level and energy terms
       float atx = fminf(ang_cmd[0] * ramp, ang_cmd[0]), aty = fminf(ang_cmd[1] * ramp, ang_cmd[1]);
       float r_ang3 = -((bk.ab.x - atx) * (bk.ab.x - atx) + (bk.ab.y - aty) * (bk.ab.y - aty) + (bk.ab.z - atz) * (bk.ab.z - atz));
       float r_level = 0.f;
-      for (int f = 0; f < c.nfeet; ++f) {
+      for (int f = 0; f < SH::nfeet(c); ++f) {
         const float* X = SM(xmat) + 9 * m.site_bodyid[c.feet_site[f]];
         r_level -= X[2] * X[2] + X[5] * X[5] + (X[8] - 1.f) * (X[8] - 1.f);
       }
       float r_energy = 0.f;
-      for (int a = 0; a < m.nu; ++a) { float e = SM(ctrl)[a] / c.joint_torque_range[a][1] * SM(qvel)[6 + a] / 160.f; r_energy -= e * e; }
+      for (int a = 0; a < SH::nu(M); ++a) { float e = SM(ctrl)[a] / c.joint_torque_range[a][1] * SM(qvel)[6 + a] / 160.f; r_energy -= e * e; }
       rew = 10.f * r_gaits + 0.5f * r_upright + 0.5f * r_yaw + r_vel + r_ang3 + 0.5f * r_h + 0.02f * r_level + 0.01f * r_energy;
     } else {
       float r_energy = 0.f;
-      for (int a = 0; a < m.nu; ++a) { float e = SM(ctrl)[a] / c.joint_torque_range[a][1]; r_energy -= e * e; }
+      for (int a = 0; a < SH::nu(M); ++a) { float e = SM(ctrl)[a] / c.joint_torque_range[a][1]; r_energy -= e * e; }
       rew = 5.f * r_gaits + 0.5f * r_upright + 0.1f * r_yaw + r_vel + r_ang + 0.5f * r_h + 0.01f * r_energy;
     }
   } else {  // DIAL_ENV_GO2_SEQJUMP
@@ -2834,7 +2919,7 @@ DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, flo
 // ---------------------------------------------------------------------------------
 // the per-warp rollout: one sample row, H env steps
 // ---------------------------------------------------------------------------------
-template <int NL, int NR>
+template <int NL, int NR, class SH = ShapeRT>
 DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const RolloutArgs& A,
                       int row, int lane) {
   WarpCtx w;
@@ -2845,7 +2930,7 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
   const DevModel& M = *Mp;
   const dial_model_desc& m = M.m;
   const dial_plan_desc& c = Pp->c;
-  const int nq = m.nq, nv = m.nv, nu = m.nu, nb = m.nbody;
+  const int nq = SH::nq(M), nv = SH::nv(M), nu = SH::nu(M), nb = SH::nbody(M);
   // instance of a batched launch and the row inside it (the sample index)
   const int inst = A.rows_per_inst > 0 ? row / A.rows_per_inst : 0;
   const int lrow = row - inst * A.rows_per_inst;
@@ -2871,11 +2956,11 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
       w.s_pos = M.s_pos[lane]; w.s_chain = M.s_chain[lane]; w.s_depth = M.s_depth[lane];
       if (w.s_chain >= 0) { w.s_cb = SD::NRP + w.s_chain * SD::CS; w.s_col = SD::NRP + w.s_depth; w.s_top = M.s_top[w.s_chain]; }
       else w.s_col = w.s_depth;
-      for (int c = 0; c < m.ncon; ++c)
+      for (int c = 0; c < SH::ncon(M); ++c)
         if (w.s_chain < 0 || M.s_con_chain[c] == w.s_chain) w.s_conmask |= 1u << c;
     }
-    if (lane < M.nedge) { const int cc = M.s_con_chain[lane >> 2]; if (cc >= 0) w.e_cb = SD::NRP + cc * SD::CS; }
-    const int nz = 2 * M.s_npos * SD::RS + M.nedge * SD::RS + M.s_npos + 8;   // Ms, Hs, Js, xs are contiguous
+    if (lane < SH::nedge(M)) { const int cc = M.s_con_chain[lane >> 2]; if (cc >= 0) w.e_cb = SD::NRP + cc * SD::CS; }
+    const int nz = 2 * M.s_npos * SD::RS + SH::nedge(M) * SD::RS + M.s_npos + 8;   // Ms, Hs, Js, xs are contiguous
     for (int i = lane; i < nz; i += 32) SM(Ms)[i] = 0.f;
     for (int i = lane; i < 32; i += 32) SM(frow)[i] = 0.f;
   }
@@ -2924,7 +3009,7 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
   float rsum = 0.f;
   const bool fwd_only = A.mode == 2;  // pipeline_init: mjx.forward only, zero ctrl
   const int H = fwd_only ? 1 : A.H;
-  const int nfr = fwd_only ? 1 : c.n_frames;
+  const int nfr = fwd_only ? 1 : SH::n_frames(c);
   for (int t = 0; t < H; ++t) {
     if (A.lockstep && (A.sync_every <= 1 || t % A.sync_every == 0)) cta_sync();
     // action -> joint target -> torque (base_env.py:37-66)
@@ -2950,14 +3035,14 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
       SM(ctrl)[lane] = ctrl;
     }
     syncwarp();
-    for (int f = 0; f < nfr; ++f) physics_step<NL, NR>(w, !fwd_only);
+    for (int f = 0; f < nfr; ++f) physics_step<NL, NR, SH>(w, !fwd_only);
     if (fwd_only) break;
     float rew = 0.f, part0, part1;
     // the task of this row, derived here from `row` (live anyway) and the launch arguments so that no
     // register holds it over the physics step
     const dial_task& T = A.tasks ? A.tasks[A.task_rows > 0 ? row / A.task_rows : 0] : plan_task(c);
-    reward_partials(w, T, step, stage, part0, part1);
-    if (lane == 0) rew = reward_lane0(w, T, step, stage, part0, part1);
+    reward_partials<SH>(w, T, step, stage, part0, part1);
+    if (lane == 0) rew = reward_lane0<SH>(w, T, step, stage, part0, part1);
     stage = shfl_i(stage, 0);
     step += 1;
     rsum += rew;

@@ -49,6 +49,21 @@ DIAL_DECL_LAUNCH(3)
 #if DIAL_HAS_VARIANT(4)
 DIAL_DECL_LAUNCH(4)
 #endif
+// Shape-specialised star<3,6> kernels (dial_rollout_variant.cu with -DDIAL_SHAPE_NAME=s): the stock Go2
+// scene, with the structure values that dial_mpc_b200.modelc.shape derives from its model.  A plan launches one only when dial_shape_matches_<s> finds every fixed
+// value equal to its own model and plan.  Custom-reward builds hold none.
+#ifndef DIAL_ONLY_VARIANT
+typedef cudaError_t (*dial_launch_fn)(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t);
+#define DIAL_DECL_SHAPE(s) \
+  cudaError_t dial_launch_rollout_##s(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t); \
+  bool dial_shape_matches_##s(const DevModel&, const dial_plan_desc&);
+DIAL_DECL_SHAPE(go2)
+static const struct {
+  const char* name;
+  dial_launch_fn launch;
+  bool (*matches)(const DevModel&, const dial_plan_desc&);
+} kShapes[] = {{"go2", dial_launch_rollout_go2, dial_shape_matches_go2}};
+#endif
 
 // ---------------------------------------------------------------------------------
 // softmax weights over all rewards (core/dial_core.py:125-128), single CTA
@@ -544,6 +559,7 @@ struct dial_plan {
   DevModel* dM = nullptr;
   DevPlan* dP = nullptr;
   int variant = 0;
+  int shape = 0;                // 1 + index into kShapes: the shape-specialised kernel of the variant; 0: generic
   int n_inst = 1;               // independent planner instances (dial_plan_desc.n_inst)
   int num_sms = 132;
   size_t smem_bytes = 0;
@@ -626,6 +642,9 @@ static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, c
     if (e != cudaSuccess) return e;
   }
   p->launches++;
+#ifndef DIAL_ONLY_VARIANT
+  if (p->shape > 0) return kShapes[p->shape - 1].launch(p->dM, p->dP, A, grid, wpc, smem, st);
+#endif
   switch (p->variant) {
 #if DIAL_HAS_VARIANT(1)
     case 1: return dial_launch_rollout_v1(p->dM, p->dP, A, grid, wpc, smem, st);
@@ -737,6 +756,13 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     }
   }
   p->n_inst = c.n_inst > 1 ? c.n_inst : 1;
+#ifndef DIAL_ONLY_VARIANT
+  // the specialised kernel computes bit for bit what the generic one does; DIAL_FORCE_GENERIC_SHAPE=1
+  // keeps the generic kernel (tests compare the two)
+  if (p->variant == 1 && !getenv("DIAL_FORCE_GENERIC_SHAPE"))
+    for (int s = 0; s < (int)(sizeof(kShapes) / sizeof(kShapes[0])); ++s)
+      if (kShapes[s].matches(p->hM, p->hP.c)) { p->shape = s + 1; break; }
+#endif
   auto bad = [&](cudaError_t e, const char* what) {
     g_err = std::string(what) + ": " + cudaGetErrorString(e);
     dial_plan_destroy(p);
@@ -1248,6 +1274,15 @@ extern "C" int dial_solver_variant(const dial_model_desc* model) {
   else if ((v = star_variant(*D)) < 0) g_err = "this build instantiates the dense (elliptic) solver path for nv = " DIAL_STR(DIAL_DENSE_NV) " only (custom builds: dial_mpc_b200.custom compiles it for the model's nv)";
   delete D;
   return v;
+}
+
+extern "C" const char* dial_plan_rollout_kernel(const dial_plan* p) {
+  static const char* const generic[] = {"v0", "v1", "v2", "v3", "v4"};
+  if (!p) return "";
+#ifndef DIAL_ONLY_VARIANT
+  if (p->shape > 0) return kShapes[p->shape - 1].name;
+#endif
+  return p->variant >= 0 && p->variant <= 4 ? generic[p->variant] : "";
 }
 
 extern "C" const char* dial_custom_reward_id(void) {

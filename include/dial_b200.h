@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define DIAL_ABI_VERSION 11
+#define DIAL_ABI_VERSION 12
 
 /* capacities of the fixed-size device model */
 #define DIAL_MAXB 24   /* bodies incl. world            */
@@ -374,6 +374,13 @@ int dial_debug_counters(dial_plan* plan, float out[8]);
  * 4 star<5,6>, 0 generic tree, <0 unsupported): custom-reward builds compile only this one
  * (-DDIAL_ONLY_VARIANT=v). */
 int dial_solver_variant(const dial_model_desc* model);
+
+/* The rollout kernel `plan` launches: "v<variant>" (the generic instantiation of its solver variant,
+ * see dial_solver_variant) or the name of a kernel specialised on the integer structure of one model
+ * ("go2": the stock Go2 scene), chosen at plan creation when every value it fixes equals the plan's
+ * own; DIAL_FORCE_GENERIC_SHAPE=1 at plan creation keeps the generic one.
+ * "" for a null plan. */
+const char* dial_plan_rollout_kernel(const dial_plan* plan);
 
 /* "" for the stock library; the identifier (-DDIAL_CUSTOM_REWARD_ID) of the reward source a
  * custom build was compiled with.  Only such a build accepts env_id == DIAL_ENV_CUSTOM. */

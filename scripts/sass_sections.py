@@ -1,8 +1,9 @@
 """Static size of the env-step path of one rollout-kernel variant, from its SASS and -lineinfo line tables.
 
-    python scripts/sass_sections.py [--variant 1] [--cubin FILE]
+    python scripts/sass_sections.py [--variant 1 | --shape go2] [--cubin FILE]
 
-Compiles `dial_rollout_variant.cu` for the variant with the library's nvcc flags (or reads a cubin),
+Compiles `dial_rollout_variant.cu` for the variant (or for the shape-specialised star<3,6> kernel of that
+name, with the structure defines the library build uses) with the library's nvcc flags (or reads a cubin),
 prints ptxas' register / stack / spill report, and attributes the SASS bytes of the kernel to source:
   * the cold tail (the divergent fall-backs of the warp shuffles that ptxas places after the last
     EXIT: taken only when a shuffle runs under a partial mask) is counted apart;
@@ -28,10 +29,15 @@ HDR = "dial_device.cuh"
 VAR = "dial_rollout_variant.cu"
 
 
-def compile_cubin(variant, out):
+def compile_cubin(variant, out, shape=None):
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + g.NVCC_FLAGS + [f"-DDIAL_VARIANT={variant}", "-Xptxas", "-v", "-cubin", "-o", out,
-                                   os.path.join(g.CSRC, VAR)]
+    flags = [f"-DDIAL_VARIANT={variant}"]
+    if shape:
+        defs = dict(g._shape_defines())
+        if shape not in defs:
+            raise SystemExit(f"unknown shape {shape!r} (known: {', '.join(defs)})")
+        flags = ["-DDIAL_VARIANT=1", f"-DDIAL_SHAPE_NAME={shape}"] + [f"-D{d}" for d in defs[shape]]
+    cmd = [nvcc] + g.NVCC_FLAGS + flags + ["-Xptxas", "-v", "-cubin", "-o", out, os.path.join(g.CSRC, VAR)]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise SystemExit(r.stderr)
@@ -92,13 +98,14 @@ def parse_sass(dis):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--variant", type=int, default=1)
+    ap.add_argument("--shape", help="the shape-specialised star<3,6> kernel of this name (e.g. go2)")
     ap.add_argument("--cubin", help="read this cubin instead of compiling the variant (it must be built with -lineinfo)")
     args = ap.parse_args()
     with tempfile.TemporaryDirectory() as tmp:
         cubin = args.cubin
         if not cubin:
-            cubin = os.path.join(tmp, f"rollout_v{args.variant}.cubin")
-            compile_cubin(args.variant, cubin)
+            cubin = os.path.join(tmp, f"rollout_{args.shape or 'v%d' % args.variant}.cubin")
+            compile_cubin(args.variant, cubin, args.shape)
         dis = subprocess.run([os.environ.get("NVDISASM", "/usr/local/cuda/bin/nvdisasm"), "-gi", "-c", cubin],
                              capture_output=True, text=True, check=True).stdout
     insts = parse_sass(dis)
