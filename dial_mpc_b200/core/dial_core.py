@@ -307,7 +307,10 @@ class DeviceLoop:
         ``envs``: B env objects of ``mbdpi.env``'s class, one task per instance (commands, gait, jump
         sequence, custom-reward user constants; ``BaseEnv.task``).  Every other field of their plan
         descriptors must equal ``mbdpi.env``'s: the plan shares it.  Instance b then computes bitwise
-        what a single-instance loop on ``envs[b]`` computes.  A batched loop whose states all carry
+        what a single-instance loop on ``envs[b]`` computes.  An env whose ``sys.model`` differs from
+        ``mbdpi.env``'s also gives its instance that physical model (``dial_plan_set_instance_model``:
+        the same structure, timestep, joint and control ranges; masses, friction, damping, gravity, ...
+        may differ).  A batched loop whose states all carry
         ``randomize_target`` binds per-instance tasks as well: each instance draws its own commands
         (and seq-jump its own jump sequence, from its state's info)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
@@ -379,6 +382,11 @@ class DeviceLoop:
             # seq-jump: the jump sequence drawn at reset is constant afterwards; one upload at bind time
             pl.set_stages(mbdpi.env.stage_tables(states[0].info))
         pl.mpc_bind(self.buf, mbdpi.M_shift.cpu().numpy())
+        if envs is not None:
+            base = bytes(_capi.fill_model_desc(mbdpi.env.sys.model))
+            for b, env_b in enumerate(envs):
+                if bytes(_capi.fill_model_desc(env_b.sys.model)) != base:
+                    pl.set_instance_model(b, env_b.sys)
 
     @staticmethod
     def _check_shared(ref_env, env) -> None:
@@ -416,6 +424,16 @@ class DeviceLoop:
         self._tasks_host[b] = t
         self._task_cmd[b] = ()
         self._upload_task(b)
+
+    def set_model(self, b: int, env_or_sys) -> None:
+        """Replace instance b's physical model before the next ``step``: an env (its ``sys``), a
+        ``System`` or a ``CompiledModel`` with the structure, timestep, joint and control ranges of
+        ``mbdpi.env``'s model.  A stream-ordered copy on the current stream.  The first per-instance
+        model of a loop makes the next steps capture their graphs again."""
+        b = int(b)
+        if not 0 <= b < self.n_instances:
+            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        self.plan.set_instance_model(b, getattr(env_or_sys, "sys", env_or_sys))
 
     def step(self, n_diffuse: Optional[int] = None, env_step=True) -> None:
         """One control step (asynchronous on the current stream).  env_step: True = env step + shift
@@ -601,18 +619,25 @@ def main():
         if not isinstance(overrides, list) or len(overrides) != args.instances:
             parser.error(f"--instance-overrides must hold a list of {args.instances} mappings (one per instance), "
                          f"got {len(overrides) if isinstance(overrides, list) else type(overrides).__name__}")
-        known = {f.name for f in dataclasses.fields(env_config_type)}
+        known = {f.name for f in dataclasses.fields(env_config_type)} | {"sys"}
         envs = []
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, got "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields or sys, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
+            ov = dict(ov)
+            sys_ov = ov.pop("sys", None)
             cfg_b = load_dataclass_from_dict(env_config_type, dict(config_dict, **ov), convert_list_to_array=True)
             envs.append(dial_envs.get_environment(dial_config.env_name, config=cfg_b))
             try:
+                if sys_ov is not None:
+                    # sys: {field: value}: the instance's own physical model (System.tree_replace)
+                    if not isinstance(sys_ov, dict):
+                        raise ValueError(f"sys must map model fields, got {sys_ov!r}")
+                    envs[-1].sys = envs[-1].sys.tree_replace(sys_ov)
                 DeviceLoop._check_shared(env, envs[-1])
-            except ValueError as e:
+            except (ValueError, KeyError) as e:
                 parser.error(f"--instance-overrides entry {b}: {e}")
     if args.instances > 1:
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs)

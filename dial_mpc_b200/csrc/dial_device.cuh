@@ -179,6 +179,10 @@ struct RolloutArgs {
   uint32_t* xch_flags[DIAL_MAXRANK];     // flags of rank p:   [2][DIAL_MAXRANK], slot [buf][source rank] = sequence + 1
   const uint32_t* xch_seq;               // local: sequence number of the current reverse_once
   unsigned int* xch_done;                // local: CTAs of this launch that have finished
+  // per-instance models (dial_plan_set_instance_model), [instances] or null: row r runs the model of
+  // instance r / rows_per_inst (models[0] when rows_per_inst == 0).  The grid then has
+  // ceil(rows_per_inst / blockDim-warps) CTAs per instance, each staging its instance's model.
+  const DevModel* models;
 };
 
 // ---------------------------------------------------------------------------------

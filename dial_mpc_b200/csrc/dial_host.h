@@ -296,6 +296,33 @@ static inline bool derive_model(const dial_model_desc& m, DevModel& D, std::stri
   return true;
 }
 
+// The first field in which `inst` (derived from an instance's model) may not differ from the plan's
+// model `plan`, or null.  An instance runs the plan's kernel, launch shape and descriptor, so the integer
+// structure must be equal, and so must the floats the plan descriptor copies from the model: timestep
+// (n_frames), jnt_range (physical_joint_range) and actuator_ctrlrange (joint_torque_range).
+static inline const char* instance_model_difference(const DevModel& plan, const DevModel& inst) {
+  const dial_model_desc &a = plan.m, &b = inst.m;
+#define DIAL_SAME(f) if (memcmp(&a.f, &b.f, sizeof(a.f)) != 0) return #f;
+  DIAL_SAME(nq) DIAL_SAME(nv) DIAL_SAME(nu) DIAL_SAME(nbody) DIAL_SAME(njnt) DIAL_SAME(ngeom) DIAL_SAME(nsite)
+  DIAL_SAME(ncon) DIAL_SAME(npair) DIAL_SAME(iterations) DIAL_SAME(ls_iterations) DIAL_SAME(eulerdamp) DIAL_SAME(cone)
+  DIAL_SAME(timestep)
+  DIAL_SAME(body_parentid) DIAL_SAME(body_rootid) DIAL_SAME(body_depth) DIAL_SAME(body_jntadr) DIAL_SAME(body_dofadr)
+  DIAL_SAME(body_dofnum) DIAL_SAME(jnt_type) DIAL_SAME(jnt_qposadr) DIAL_SAME(jnt_dofadr) DIAL_SAME(jnt_limited)
+  DIAL_SAME(jnt_range) DIAL_SAME(dof_bodyid) DIAL_SAME(dof_jntid) DIAL_SAME(dof_parentid) DIAL_SAME(geom_type)
+  DIAL_SAME(geom_bodyid) DIAL_SAME(pair_kind) DIAL_SAME(pair_geom1) DIAL_SAME(pair_geom2) DIAL_SAME(pair_ncon)
+  DIAL_SAME(pair_condim) DIAL_SAME(site_bodyid) DIAL_SAME(actuator_dofadr) DIAL_SAME(actuator_qposadr)
+  DIAL_SAME(actuator_ctrllimited) DIAL_SAME(actuator_forcelimited) DIAL_SAME(actuator_ctrlrange)
+#undef DIAL_SAME
+  // derive_model's tables follow from the fields above, except root_invmass (a float, from body_mass)
+  const size_t off = offsetof(DevModel, maxdepth), inv = offsetof(DevModel, root_invmass);
+  const char *pa = reinterpret_cast<const char*>(&plan), *pb = reinterpret_cast<const char*>(&inst);
+  if (memcmp(pa + off, pb + off, inv - off) != 0 ||
+      memcmp(pa + inv + sizeof(plan.root_invmass), pb + inv + sizeof(plan.root_invmass),
+             sizeof(DevModel) - inv - sizeof(plan.root_invmass)) != 0)
+    return "derived structure";
+  return nullptr;
+}
+
 // The counts the reward loops over, in range (the kernel indexes the tables with them unchecked).
 static inline bool task_valid(const dial_task& t) {
   return t.n_stage >= 1 && t.n_stage <= DIAL_MAXSTAGE && t.n_user >= 0 && t.n_user <= DIAL_MAXUSER;

@@ -589,6 +589,11 @@ struct dial_plan {
   uint32_t* mpc_key = nullptr;  // sampling key of the current reverse_once
   struct MpcGraph { int n_diffuse, env_step, seen; cudaGraphExec_t exec; int64_t launches; };
   std::vector<MpcGraph> mpc_graphs;
+  // per-instance models (dial_plan_set_instance_model): device array [n_inst] read by dial_mpc_step,
+  // its pinned host staging [n_inst] and, per slot, the event of the last copy out of the staging slot
+  DevModel* dModels = nullptr;
+  DevModel* hModels = nullptr;
+  std::vector<cudaEvent_t> model_ev;
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -635,6 +640,8 @@ extern "C" size_t dial_sizeof(int which) {
 static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, cudaStream_t st) {
   const size_t smem = sizeof(DevModel) + sizeof(DevPlan) + (size_t)wpc * p->hM.warp_floats * sizeof(float);
   int grid = (A.nrows + wpc - 1) / wpc;
+  // per-instance models: ceil(rows_per_inst / wpc) CTAs per instance (rollout_kernel's row mapping)
+  if (A.models && A.rows_per_inst > 0) grid = (A.nrows / A.rows_per_inst) * ((A.rows_per_inst + wpc - 1) / wpc);
   if (A.row_counter) {
     const int resident = p->num_sms * (wpc > 8 ? 1 : 16 / wpc);
     grid = grid < resident ? grid : resident;
@@ -688,7 +695,15 @@ static cudaError_t launch_rollout_any(dial_plan* p, const RolloutArgs& A0, cudaS
   RolloutArgs A = A0;
   const char* f = getenv("DIAL_WPC");
   int wpc = f ? atoi(f) : 0;
-  if (wpc == 0) wpc = default_wpc(p, A.nrows);
+  if (wpc == 0) {
+    wpc = default_wpc(p, A.nrows);
+    // per-instance models: a CTA holds rows of one instance; spread each instance's rows evenly over
+    // the CTAs it needs at that width
+    if (A.models && A.rows_per_inst > 0) {
+      const int cpi = (A.rows_per_inst + wpc - 1) / wpc;
+      wpc = (A.rows_per_inst + cpi - 1) / cpi;
+    }
+  }
   if (wpc < 1 || wpc > DIAL_MAXTHREADS / 32) return cudaErrorInvalidValue;
   // lock-step pays off on both solver paths.  The dense (elliptic) path used to run free with
   // dynamic row assignment because MJX's 50-iteration line searches made its rows heavy-tailed;
@@ -697,7 +712,8 @@ static cudaError_t launch_rollout_any(dial_plan* p, const RolloutArgs& A0, cudaS
   // env step, per physics substep, per Newton iteration = level 3, the dense default).  DIAL_NO_LOCKSTEP=1 restores the free-running
   // warps, DIAL_NO_MIDSYNC=1 / DIAL_DENSE_LOCKSTEP=2 select the coarser levels.
   A.lockstep = (wpc >= 2 && !getenv("DIAL_NO_LOCKSTEP")) ? 1 : 0;
-  if (p->hM.dense && !A.lockstep && A.nrows > wpc * p->num_sms && !getenv("DIAL_NO_DYNAMIC_ROWS")) A.row_counter = p->row_counter;
+  // (not with per-instance models: a persistent warp takes rows of any instance)
+  if (p->hM.dense && !A.lockstep && !A.models && A.nrows > wpc * p->num_sms && !getenv("DIAL_NO_DYNAMIC_ROWS")) A.row_counter = p->row_counter;
   // second barrier before the constraint solve: the dense path needs it (and a third per Newton
   // iteration); on the star paths it stopped paying once the solver shrank — DIAL_MIDSYNC=1 /
   // DIAL_NO_MIDSYNC=1 override
@@ -819,6 +835,8 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   }
   cudaFree(p->xch.bars_partial);
   cudaFree(p->mpc_Msh); cudaFree(p->mpc_Y1); cudaFree(p->mpc_key);
+  for (cudaEvent_t e : p->model_ev) if (e) cudaEventDestroy(e);
+  cudaFree(p->dModels); cudaFreeHost(p->hModels);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   cudaFree(p->weights2);
@@ -872,6 +890,55 @@ extern "C" int dial_plan_set_stages(dial_plan* p, int n_stage, const float* pose
   const size_t off = offsetof(dial_plan_desc, n_stage), end = offsetof(dial_plan_desc, n_user);
   CUDA_OK(cudaMemcpyAsync((char*)p->dP + off, (const char*)&p->hP.c + off, end - off, cudaMemcpyHostToDevice,
                           (cudaStream_t)stream));
+  return 0;
+}
+
+extern "C" int dial_plan_set_instance_model(dial_plan* p, int b, const dial_model_desc* m, void* stream) {
+  if (!p || !m) return fail("dial_plan_set_instance_model: null argument");
+  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_instance_model: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
+  if (p->hP.c.Ntotal != p->hP.c.Nsample) return fail("dial_plan_set_instance_model: sharded plans (Ntotal != Nsample) share one model");
+  DevModel* D = new (std::nothrow) DevModel();
+  if (!D) return fail("out of memory");
+  std::string err;
+  if (!derive_model(*m, *D, err)) { delete D; return fail("dial_plan_set_instance_model: " + err); }
+  const char* diff = instance_model_difference(p->hM, *D);
+  if (diff) {
+    delete D;
+    return fail(std::string("dial_plan_set_instance_model: field '") + diff + "' differs from the plan's model "
+                "(an instance's model may differ in floats other than timestep, jnt_range and actuator_ctrlrange only)");
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (!p->dModels) {
+    // first call: every slot starts as the plan's own model; the graphs captured so far launch without
+    // per-instance models and are recaptured on their next use
+    const size_t n = (size_t)p->n_inst;
+    if ((e = cudaMallocHost(&p->hModels, n * sizeof(DevModel))) == cudaSuccess &&
+        (e = cudaMalloc(&p->dModels, n * sizeof(DevModel))) == cudaSuccess) {
+      for (size_t i = 0; i < n; ++i) p->hModels[i] = p->hM;
+      e = cudaMemcpy(p->dModels, p->hModels, n * sizeof(DevModel), cudaMemcpyHostToDevice);
+    }
+    if (e != cudaSuccess) {
+      cudaFree(p->dModels); cudaFreeHost(p->hModels); p->dModels = nullptr; p->hModels = nullptr;
+      delete D;
+      return fail(std::string("dial_plan_set_instance_model: ") + cudaGetErrorString(e));
+    }
+    p->model_ev.assign(n, nullptr);
+    for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+    p->mpc_graphs.clear();
+  }
+  // stream-ordered copy out of the slot's pinned staging; the staging slot is rewritten only after the
+  // previous copy out of it has run
+  cudaEvent_t& ev = p->model_ev[b];
+  if (ev) e = cudaEventSynchronize(ev);
+  else e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) {
+    p->hModels[b] = *D;
+    e = cudaMemcpyAsync(p->dModels + b, p->hModels + b, sizeof(DevModel), cudaMemcpyHostToDevice, st);
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
+  delete D;
+  CUDA_OK(e);
   return 0;
 }
 
@@ -1143,6 +1210,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     A.nrows = ni; A.H = 1; A.mode = 0; A.us = Y[cur]; A.rewss = B.reward;
     if (batched) { A.rows_per_inst = 1; A.us_row = n1 * nu; }
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
+    A.models = p->dModels;
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
     CUDA_OK(launch_rollout(p, A, 1, st));
   }
@@ -1176,6 +1244,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     A.nrows = ni * (c.Nsample + 1); A.H = c.Hsample + 1; A.mode = 1;
     if (batched) A.rows_per_inst = c.Nsample + 1;
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? c.Nsample + 1 : 0; }
+    A.models = p->dModels;
     A.Ybar = Y[cur]; A.noise = noise;
     if (fused) A.rng_dev = B.rng; else A.key_dev = p->mpc_key;
     p->cur ^= 1;

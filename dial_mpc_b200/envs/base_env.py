@@ -36,13 +36,11 @@ class System:
         return self.model.timestep
 
     def tree_replace(self, params: Dict[str, Any]) -> "System":
-        """Subset of ``sys.tree_replace`` used by the reference: {"opt.timestep": dt}."""
-        m = self.model
-        for k, v in params.items():
-            if k != "opt.timestep":
-                raise NotImplementedError(k)
-            m = m.replace_timestep(float(v))
-        return System(m)
+        """``sys.tree_replace`` of the float model fields (``CompiledModel.replace``): ``opt.timestep``,
+        ``opt.gravity``, ``body_mass``, ``pair_friction``, ... as full arrays or ``{name: value}``
+        mappings.  Derived constants are left as they are, as in MJX; ``sys.model.set_const()``
+        recomputes them.  Structural fields raise ``KeyError``."""
+        return System(self.model.replace(params))
 
     def keyframe(self, name: str) -> np.ndarray:
         return self.model.keyframe_qpos(name)
@@ -112,6 +110,17 @@ class BaseEnv:
         self._plan = None  # lazily created 1-sample plan for reset()/step()
 
     # -- Brax PipelineEnv surface ---------------------------------------------------------
+    @property
+    def sys(self) -> System:
+        return self._sys
+
+    @sys.setter
+    def sys(self, value: System) -> None:
+        """Assigning a new system (e.g. ``env.sys = env.sys.tree_replace({...})``) drops the cached plan:
+        the next ``reset`` / ``step`` runs the new model."""
+        self._sys = value
+        self._plan = None
+
     @property
     def dt(self) -> float:
         return self._config.timestep * self._n_frames

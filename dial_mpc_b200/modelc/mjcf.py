@@ -320,6 +320,72 @@ class CompiledModel:
         m.timestep = float(timestep)
         return m
 
+    # float fields ``replace`` accepts, with the name table their entries are named by
+    FLOAT_FIELDS = {"body_mass": "body", "body_inertia": "body", "body_ipos": "body", "dof_damping": "joint",
+                    "dof_armature": "joint", "actuator_gear": "actuator", "actuator_gain": "actuator",
+                    "actuator_bias": "actuator", "pair_friction": "pair", "pair_solref": "pair",
+                    "pair_solimp": "pair", "geom_size": "geom"}
+
+    def replace(self, params: Dict[str, Any]) -> "CompiledModel":
+        """A copy with float fields replaced, like ``mjx.Model.tree_replace``: ``"opt.timestep"``,
+        ``"opt.gravity"`` or a name of ``FLOAT_FIELDS``, each mapped to a full array or to
+        ``{name: value}``.  Bodies are named by body name, dofs by joint name (a value per dof of the
+        joint, or one for all of them), actuators by actuator name, geoms by geom name and contact pairs
+        by the name of the pair's moving geom (geom2).  Derived constants (``body_invweight0``,
+        ``dof_invweight0``, ``meaninertia``) are left as they are; ``set_const`` recomputes them."""
+        import copy
+        m = copy.copy(self)
+        m.arrays = dict(self.arrays)
+        m.gravity = np.array(self.gravity, dtype=np.float64)
+        for key, val in params.items():
+            if key == "opt.timestep":
+                m.timestep = float(val)
+                continue
+            if key == "opt.gravity":
+                g = np.array(val, dtype=np.float64)
+                if g.shape != (3,):
+                    raise ValueError(f"opt.gravity needs 3 values, got shape {g.shape}")
+                m.gravity = g
+                continue
+            if key not in self.FLOAT_FIELDS:
+                raise KeyError(f"tree_replace: {key!r} is not a replaceable float field (accepted: opt.timestep, "
+                               f"opt.gravity, {', '.join(self.FLOAT_FIELDS)}); structure cannot be replaced")
+            old = self.arrays[key]
+            if not isinstance(val, dict):
+                new = np.array(val, dtype=old.dtype)
+                if new.shape != old.shape:
+                    raise ValueError(f"tree_replace: {key} has shape {old.shape}, got {new.shape}")
+                m.arrays[key] = new
+                continue
+            new = old.copy()
+            for name, v in val.items():
+                rows = self._entries(self.FLOAT_FIELDS[key], name, key)
+                new[rows] = np.broadcast_to(np.asarray(v, dtype=old.dtype), new[rows].shape)
+            m.arrays[key] = new
+        return m
+
+    def _entries(self, table: str, name: str, key: str):
+        """Index (or dof slice) of entry ``name`` of ``table`` in the arrays of field ``key``."""
+        if table == "pair":
+            geoms = [self.names["geom"][g] for g in self.arrays["pair_geom2"]]
+            if name not in geoms:
+                raise KeyError(f"tree_replace: {key}: no contact pair whose moving geom is {name!r} (pairs: {geoms})")
+            return geoms.index(name)
+        if name not in self.names.get(table, []):
+            raise KeyError(f"tree_replace: {key}: unknown {table} {name!r} (known: {self.names.get(table, [])})")
+        i = self.names[table].index(name)
+        if table != "joint":
+            return i
+        a = self.arrays["jnt_dofadr"][i]
+        nd = {0: 6, 1: 3}.get(int(self.arrays["jnt_type"][i]), 1)
+        return slice(a, a + nd)
+
+    def set_const(self) -> "CompiledModel":
+        """Recompute the constants MuJoCo's ``mj_setConst`` derives at qpos0 (``body_invweight0``,
+        ``dof_invweight0``, ``meaninertia``) from the current masses and inertias, in place."""
+        _set_const(self)
+        return self
+
 
 # --------------------------------------------------------------------------
 # compiler

@@ -82,6 +82,14 @@ class Plan:
                                                   tgt.ctypes.data_as(F), rad.ctypes.data_as(F), _stream()))
         self._stages = key
 
+    def set_instance_model(self, b: int, model) -> None:
+        """Instance b's own physical model (a ``CompiledModel`` or ``System`` with the plan model's
+        structure, timestep, joint ranges and control ranges) for every later ``mpc_step``; a
+        stream-ordered copy on the current stream (``dial_plan_set_instance_model``)."""
+        model = getattr(model, "model", model)
+        md = _capi.fill_model_desc(model)
+        self._check(self.lib.dial_plan_set_instance_model(self.handle, int(b), C.byref(md), _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

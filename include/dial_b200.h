@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define DIAL_ABI_VERSION 12
+#define DIAL_ABI_VERSION 13
 
 /* capacities of the fixed-size device model */
 #define DIAL_MAXB 24   /* bodies incl. world            */
@@ -343,7 +343,27 @@ typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound 
    * contents: the caller may rewrite tasks between dial_mpc_step calls with a copy on the same stream
    * (stream-ordered, like dial_plan_set_command).  Each task must satisfy the ranges of dial_task. */
   const dial_task* tasks;
+  /* Per-instance models are not a buffer: dial_plan_set_instance_model (below) writes them into a
+   * plan-owned array that every launch of dial_mpc_step reads. */
 } dial_mpc_buffers;
+
+/* Give instance b (0 <= b < n_inst; b = 0 for a single-instance plan) of the plan its own physical model
+ * `m` [host], e.g. a payload on the base (body_mass, body_inertia, body_ipos), another floor friction
+ * (pair_friction), joint damping, motor strength (actuator_gear) or gravity.  m must have the integer
+ * structure of the plan's model (bodies, dofs, contact pairs, solver iteration counts, ...) and the same
+ * timestep, jnt_range and actuator_ctrlrange (the plan descriptor holds copies of them); any other float
+ * may differ.  Otherwise the call fails and dial_last_error names the first field that differs.  The
+ * plan's gains, torque limits, joint ranges and dt stay shared by every instance.
+ * Only dial_mpc_step reads per-instance models (the env-step row and every rollout row of instance b):
+ * instance b's results are then bitwise those of a plan created from m.  dial_env_step(_kin),
+ * dial_pipeline_init, dial_rollout and the eager dial_reverse_* keep using the plan's own model.
+ * The copy is stream-ordered on `stream`, out of plan-owned pinned staging, so it may be issued between
+ * dial_mpc_step calls like dial_plan_set_command.  The first call on a plan allocates the per-instance
+ * array (every slot starts as the plan's own model) and drops the captured graphs, which are captured
+ * again on their next use; later calls do not.  Sharded plans (Ntotal != Nsample) reject the call.
+ * Launches with per-instance models give each instance's rows CTAs of their own (each CTA stages one
+ * model), with at most the warps per CTA of the default policy (dial_rollout_wpc). */
+int dial_plan_set_instance_model(dial_plan* plan, int b, const dial_model_desc* m, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops

@@ -9,8 +9,12 @@ steps outside the timed CUDA events.  Prints one JSON line: value = B * Ndiffuse
 / step time, ms per control step, and the card, power limit and SM clocks read in the same run.
 ``--instances 1`` is the single-instance plan (bench.py's timed step).  ``--distinct-tasks``: instance b
 plans its own velocity command (vx spread over [-1, 1], a per-instance task bound through
-``DeviceLoop(..., envs=...)``) instead of the config's shared one."""
+``DeviceLoop(..., envs=...)``) instead of the config's shared one.  ``--distinct-models``: instance b
+runs its own physical model (base mass +3 kg * b / B, foot friction 1 - 0.5 b / B where the model has
+feet ``FR FL RR RL``, else every pair's friction scaled so; a per-instance model bound through
+``dial_plan_set_instance_model``)."""
 import argparse
+import copy
 import json
 import os
 import subprocess
@@ -37,6 +41,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--distinct-tasks", action="store_true",
                     help="bind one task per instance: B distinct forward-velocity commands")
+    ap.add_argument("--distinct-models", action="store_true",
+                    help="bind one physical model per instance: B distinct base masses and foot frictions")
     args = ap.parse_args()
     if args.instances < 1 or args.steps < 1:
         ap.error("--instances and --steps must be at least 1")
@@ -61,6 +67,16 @@ def main():
             ap.error(f"--distinct-tasks sweeps default_vx, which {type(env).__name__} has not")
         envs = [E.get_environment(b["env"], config=replace(env._config, default_vx=float(v)))
                 for v in np.linspace(-1.0, 1.0, B)]
+    if args.distinct_models:
+        m = env.sys.model
+        torso = int(env.plan_desc().torso_body)
+        base = [env if envs is None else envs[i] for i in range(B)]
+        envs = []
+        for i, e in enumerate(base):
+            e = copy.copy(e)
+            e.sys = e.sys.tree_replace({"body_mass": {m.names["body"][torso]: m.arrays["body_mass"][torso] + 3.0 * i / B},
+                                        "pair_friction": m.arrays["pair_friction"] * (1.0 - 0.5 * i / B)})
+            envs.append(e)
     if B == 1:
         loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs)
     else:
@@ -80,7 +96,8 @@ def main():
     torch.cuda.synchronize()
     t = sum(a.elapsed_time(e) for a, e in evs) / 1e3 / args.steps
     rows = B * (cfg.Nsample + 1)
-    print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=bool(envs), rows_per_rollout=rows,
+    print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
+                          distinct_models=args.distinct_models, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
                           value=B * cfg.Ndiffuse * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
