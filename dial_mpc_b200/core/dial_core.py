@@ -48,9 +48,12 @@ def softmax_update(weights, Y0s, sigma, mu_0t):
 
 class MBDPI:
     def __init__(self, args: DialConfig, env, rank: int = 0, world_size: int = 1, process_group=None,
-                 compute_bars: bool = True, plan_factory=None, n_instances: int = 1):
+                 compute_bars: bool = True, plan_factory=None, n_instances: int = 1, n_ensemble: int = 0):
         """``n_instances`` > 1: one plan holds that many independent planner instances (same model,
-        config and annealing schedule; own state, rng and knots), advanced together by ``DeviceLoop``."""
+        config and annealing schedule; own state, rng and knots), advanced together by ``DeviceLoop``.
+        ``n_ensemble`` = K >= 1: every instance plans against K member models (``DeviceLoop(...,
+        ensemble=...)``) and scores each sample by its reward averaged over them, while its env step runs
+        its own model (the plant).  K = 1 with the nominal member is the plain mismatch experiment."""
         self.args = args
         self.env = env
         self.nu = env.action_size
@@ -65,6 +68,9 @@ class MBDPI:
         self.n_instances = int(n_instances)
         if self.n_instances < 1:
             raise ValueError("n_instances must be >= 1")
+        self.n_ensemble = int(n_ensemble)
+        if not 0 <= self.n_ensemble <= _capi.DEFINES["DIAL_MAXENS"]:
+            raise ValueError(f"n_ensemble must be in 0..{_capi.DEFINES['DIAL_MAXENS']}, got {self.n_ensemble}")
 
         sigma_control = args.horizon_diffuse_factor ** np.arange(args.Hnode + 1)[::-1]
         self.sigma_control_np = (sigma_control * args.sigma_scale).astype(np.float64)
@@ -79,7 +85,7 @@ class MBDPI:
 
         desc = env.plan_desc(Nsample=self.Nlocal, Ntotal=args.Nsample, shard_offset=rank * self.Nlocal,
                              Hsample=args.Hsample, Hnode=args.Hnode, temp_sample=args.temp_sample,
-                             M_n2u=self.M_n2u_np, n_inst=self.n_instances)
+                             M_n2u=self.M_n2u_np, n_inst=self.n_instances, n_ens=self.n_ensemble)
         # plan_factory exists for the CPU test harness (tests/emul); the product path is Plan
         self.plan = (plan_factory or Plan)(env, desc)
         dev = self.plan.device
@@ -212,6 +218,9 @@ class MBDPI:
         if self.n_instances > 1:
             raise RuntimeError(f"MBDPI.{what} plans one instance; a plan of {self.n_instances} instances runs "
                                "through DeviceLoop (one CUDA graph per control step for all instances)")
+        if self.n_ensemble > 0:
+            raise RuntimeError(f"MBDPI.{what} plans on the plan's own model; an ensemble plan (n_ensemble = "
+                               f"{self.n_ensemble}) runs through DeviceLoop, which rolls every member")
 
     @property
     def exchange_name(self) -> str:
@@ -294,7 +303,7 @@ class DeviceLoop:
     the GPUs inside the kernels (peer-memory exchange), so no host collective sits in the step."""
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
-                 compute_bars: bool = True, noise=None, envs=None):
+                 compute_bars: bool = True, noise=None, envs=None, ensemble=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -312,7 +321,14 @@ class DeviceLoop:
         the same structure, timestep, joint and control ranges; masses, friction, damping, gravity, ...
         may differ).  A batched loop whose states all carry
         ``randomize_target`` binds per-instance tasks as well: each instance draws its own commands
-        (and seq-jump its own jump sequence, from its state's info)."""
+        (and seq-jump its own jump sequence, from its state's info).
+
+        ``ensemble`` (an ``mbdpi`` with ``n_ensemble`` = K >= 1): the planning models, either one list of K
+        envs, ``System``s or ``CompiledModel``s shared by every instance, or B such lists (one per
+        instance).  ``envs[b]``'s model stays instance b's plant (the env step); the rollouts of member k
+        run ``ensemble[k]`` (or ``ensemble[b][k]``), and ``rews`` receives each sample's reward averaged
+        over the members.  A member whose model equals ``mbdpi.env``'s needs no upload; None: every
+        member is ``mbdpi.env``'s model."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -381,12 +397,38 @@ class DeviceLoop:
         elif self._rand and hasattr(mbdpi.env, "stage_tables"):
             # seq-jump: the jump sequence drawn at reset is constant afterwards; one upload at bind time
             pl.set_stages(mbdpi.env.stage_tables(states[0].info))
+        members = self._ensemble_lists(mbdpi, ensemble)
         pl.mpc_bind(self.buf, mbdpi.M_shift.cpu().numpy())
+        base = bytes(_capi.fill_model_desc(mbdpi.env.sys.model))
         if envs is not None:
-            base = bytes(_capi.fill_model_desc(mbdpi.env.sys.model))
             for b, env_b in enumerate(envs):
                 if bytes(_capi.fill_model_desc(env_b.sys.model)) != base:
                     pl.set_instance_model(b, env_b.sys)
+        for b, row in enumerate(members):
+            for k, m in enumerate(row):
+                if bytes(_capi.fill_model_desc(m)) != base:
+                    pl.set_ensemble_model(b, k, m)
+
+    @staticmethod
+    def _model(env_or_sys):
+        """The ``CompiledModel`` of an env, a ``System`` or a ``CompiledModel``."""
+        m = getattr(env_or_sys, "sys", env_or_sys)
+        return getattr(m, "model", m)
+
+    def _ensemble_lists(self, mbdpi, ensemble) -> list:
+        """``ensemble`` as B lists of K models ([] when None)."""
+        if ensemble is None:
+            return []
+        K, B = mbdpi.n_ensemble, mbdpi.n_instances
+        if K < 1:
+            raise ValueError("ensemble= needs an MBDPI built with n_ensemble >= 1")
+        ens = list(ensemble)
+        per_instance = len(ens) > 0 and all(isinstance(e, (list, tuple)) for e in ens)
+        rows = [list(e) for e in ens] if per_instance else [ens] * B
+        if len(rows) != B or any(len(r) != K for r in rows):
+            raise ValueError(f"ensemble must be a list of {K} models or {B} such lists, got "
+                             f"{[len(r) for r in rows] if per_instance else len(ens)}")
+        return [[self._model(m) for m in r] for r in rows]
 
     @staticmethod
     def _check_shared(ref_env, env) -> None:
@@ -434,6 +476,19 @@ class DeviceLoop:
         if not 0 <= b < self.n_instances:
             raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
         self.plan.set_instance_model(b, getattr(env_or_sys, "sys", env_or_sys))
+
+    def set_ensemble_model(self, b: int, k: int, env_or_sys) -> None:
+        """Replace member k of instance b's planning ensemble before the next ``step``: an env, a ``System``
+        or a ``CompiledModel`` (``Plan.set_ensemble_model``).  The first member set on a loop makes the next
+        steps capture their graphs again."""
+        b, k = int(b), int(k)
+        if self.mbdpi.n_ensemble < 1:
+            raise RuntimeError("set_ensemble_model needs an MBDPI built with n_ensemble >= 1")
+        if not 0 <= b < self.n_instances:
+            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        if not 0 <= k < self.mbdpi.n_ensemble:
+            raise IndexError(f"member {k} out of range (0..{self.mbdpi.n_ensemble - 1})")
+        self.plan.set_ensemble_model(b, k, self._model(env_or_sys))
 
     def step(self, n_diffuse: Optional[int] = None, env_step=True) -> None:
         """One control step (asynchronous on the current stream).  env_step: True = env step + shift
@@ -539,17 +594,50 @@ def save_run(output_dir, rollout, infos, timestamp=None):
     return states, preds
 
 
-def run_instances(dial_config, env, B, Nstep, envs=None):
+def load_ensemble(spec, env):
+    """The ``--ensemble`` file's mapping -> (K member ``System``s, the plant's ``sys`` mapping or None).
+    ``members``: a list of K ``System.tree_replace`` mappings of ``env``'s model (``{}``: the nominal
+    model); ``plant`` (optional): one such mapping for every instance's plant.  Raises ValueError naming
+    the entry that is malformed."""
+    if not isinstance(spec, dict) or set(spec) - {"members", "plant"} or "members" not in spec:
+        raise ValueError("must map 'members' (a list of sys mappings) and optionally 'plant' (one sys mapping), got "
+                         f"{sorted(spec) if isinstance(spec, dict) else spec!r}")
+    members, plant = spec["members"], spec.get("plant")
+    kmax = _capi.DEFINES["DIAL_MAXENS"]
+    if not isinstance(members, list) or not 1 <= len(members) <= kmax:
+        raise ValueError(f"members must be a list of 1..{kmax} sys mappings, got "
+                         f"{len(members) if isinstance(members, list) else type(members).__name__}")
+    out = []
+    for k, ov in enumerate(members):
+        ov = {} if ov is None else ov
+        if not isinstance(ov, dict):
+            raise ValueError(f"members[{k}] must map model fields, got {ov!r}")
+        try:
+            out.append(env.sys.tree_replace(ov))
+        except (KeyError, ValueError) as e:
+            raise ValueError(f"members[{k}]: {e}") from None
+    if plant is not None:
+        if not isinstance(plant, dict):
+            raise ValueError(f"plant must map model fields, got {plant!r}")
+        try:
+            env.sys.tree_replace(plant)
+        except (KeyError, ValueError) as e:
+            raise ValueError(f"plant: {e}") from None
+    return out, plant
+
+
+def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
-    plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task, when given).  With
-    ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key."""
-    mbdpi = MBDPI(dial_config, env, n_instances=B)
+    plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
+    ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
+    ``ensemble``: K planning models shared by every instance (``DeviceLoop(..., ensemble=...)``)."""
+    mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
         rng, rng_reset = drandom.split(drandom.PRNGKey(seed=dial_config.seed + b))
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
-    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs)
+    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -588,6 +676,10 @@ def main():
     parser.add_argument("--instance-overrides", type=str, default=None, metavar="FILE.yaml",
                         help="a YAML list of one mapping of env-config fields per instance (--instances of them): "
                              "instance b runs the config updated by mapping b (its own commands, gait, targets, ...)")
+    parser.add_argument("--ensemble", type=str, default=None, metavar="FILE.yaml",
+                        help="plan against an ensemble of models: a YAML mapping with 'members', a list of K sys "
+                             "mappings ({} = the nominal model), and optionally 'plant', one sys mapping applied to "
+                             "every instance's simulated robot before its own --instance-overrides sys")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -612,6 +704,14 @@ def main():
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
     env = dial_envs.get_environment(dial_config.env_name, config=env_config)
     envs = None
+    members, plant = None, None
+    if args.ensemble is not None:
+        if args.eager:
+            parser.error("--ensemble runs on the CUDA-graph loop; it excludes --eager")
+        try:
+            members, plant = load_ensemble(yaml.safe_load(open(args.ensemble)), env)
+        except (ValueError, yaml.YAMLError) as e:
+            parser.error(f"--ensemble {args.ensemble}: {e}")
     if args.instance_overrides is not None:
         if args.instances < 2:
             parser.error("--instance-overrides needs --instances B with B >= 2")
@@ -631,6 +731,8 @@ def main():
             cfg_b = load_dataclass_from_dict(env_config_type, dict(config_dict, **ov), convert_list_to_array=True)
             envs.append(dial_envs.get_environment(dial_config.env_name, config=cfg_b))
             try:
+                if plant is not None:
+                    envs[-1].sys = envs[-1].sys.tree_replace(plant)
                 if sys_ov is not None:
                     # sys: {field: value}: the instance's own physical model (System.tree_replace)
                     if not isinstance(sys_ov, dict):
@@ -639,19 +741,27 @@ def main():
                 DeviceLoop._check_shared(env, envs[-1])
             except (ValueError, KeyError) as e:
                 parser.error(f"--instance-overrides entry {b}: {e}")
+    plant_env = env
+    if plant is not None and envs is None:
+        # one plant for every instance: the env the loop steps (and resets) with the plant's model
+        plant_env = dial_envs.get_environment(dial_config.env_name, config=env_config)
+        plant_env.sys = env.sys.tree_replace(plant)
+        if args.instances > 1:
+            envs = [plant_env] * args.instances
     if args.instances > 1:
-        run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs)
+        run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
+                      ensemble=members)
         return
-    mbdpi = MBDPI(dial_config, env)
+    mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
-    state = env.reset(rng_reset)
+    state = plant_env.reset(rng_reset)
     Y0 = torch.zeros(dial_config.Hnode + 1, mbdpi.nu, device=mbdpi.device)
     rng_exp, rng = drandom.split(rng)
     Nstep = args.n_steps or dial_config.n_steps
     rews, rollout, infos = [], [], []
     if mbdpi.world_size == 1 and not args.eager:
         # one CUDA graph per control step; the host launches it and logs
-        loop = DeviceLoop(mbdpi, state, rng, Y0)
+        loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members)
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):

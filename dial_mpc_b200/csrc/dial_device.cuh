@@ -183,7 +183,14 @@ struct RolloutArgs {
   // instance r / rows_per_inst (models[0] when rows_per_inst == 0).  The grid then has
   // ceil(rows_per_inst / blockDim-warps) CTAs per instance, each staging its instance's model.
   const DevModel* models;
+  // ensemble plans (dial_plan_desc.n_ens >= 1): the rows of instance b are K member blocks of
+  // rows_per_model = Nsample+1 rows each (rows_per_inst = K * rows_per_model); a member's row i takes
+  // sample i's perturbation, and `models` holds one model per member block.  0: one block per instance.
+  int32_t rows_per_model;
 };
+
+// rows of one model slot of `models`: a member block of an ensemble plan, else an instance
+HD int model_rows(const RolloutArgs& A) { return A.rows_per_model > 0 ? A.rows_per_model : A.rows_per_inst; }
 
 // ---------------------------------------------------------------------------------
 // Integer structure of the env step as a template policy.  The warp-uniform bounds and selectors the
@@ -2989,8 +2996,10 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
 #pragma unroll
   for (int k = 0; k < DIAL_MAXNODE; ++k) Y[k] = 0.f;
   if (A.mode == 1 && lane < nu) {
-    const bool is_mean = lrow == c.Nsample;
-    const uint32_t gidx = (uint32_t)(c.shard_offset + lrow);
+    // the sample index: every member of an ensemble rolls the same samples
+    const int smp = A.rows_per_model > 0 ? lrow % A.rows_per_model : lrow;
+    const bool is_mean = smp == c.Nsample;
+    const uint32_t gidx = (uint32_t)(c.shard_offset + smp);
     const uint32_t ntot = (uint32_t)c.Ntotal * (uint32_t)Hn1 * (uint32_t)nu;
     uint32_t key0 = A.key_dev ? A.key_dev[2 * inst] : A.key0, key1 = A.key_dev ? A.key_dev[2 * inst + 1] : A.key1;
     if (A.rng_dev) split_key(A.rng_dev[2 * inst], A.rng_dev[2 * inst + 1], key0, key1);

@@ -479,7 +479,8 @@ __global__ void mpc_shift_kernel(const float* __restrict__ Msh, const float* __r
 //            order, 8 independent loads in flight per thread
 //   stage 2: grid H: partials summed in fixed chunk order (bitwise deterministic)
 // Batched plans add an instance dimension (stage 1: z = 3 * instance + array, stage 2: y = instance)
-// over instance-major trajectories, weights, partials and outputs.
+// over instance-major trajectories, weights, partials and outputs.  Instance b's trajectories start at
+// row b * inst_rows: nrows on a plain plan, K * nrows on an ensemble plan, whose bars read member 0.
 // The only bandwidth-shaped kernel of the path: rows * H * (nq + nv + 3 (nbody-1)) * 4 bytes read
 // once from L2 / HBM (cfg1: 16 MB, cfg4 shard: 65 MB).
 // ---------------------------------------------------------------------------------
@@ -489,6 +490,7 @@ struct TrajArgs {
   float* out[3];
   int ncol[3], coloff[3];
   int coltot, nrows, H;
+  int inst_rows;   // trajectory rows between two instances (BATCH only)
   const float* weights;
   int w_offset, mean_row, mean_weight_index, include_mean;
   float* partial;  // [TB_CHUNKS][H][coltot]
@@ -504,7 +506,7 @@ __global__ void __launch_bounds__(256, 8) trajbar_partial_kernel(const TrajArgs 
   const int coloff = arr == 0 ? T.coloff[0] : (arr == 1 ? T.coloff[1] : T.coloff[2]);
   const int j = blockIdx.x * 256 + threadIdx.x;
   if (blockIdx.x * 256 >= len) return;
-  const float* __restrict__ traj = (arr == 0 ? T.traj[0] : (arr == 1 ? T.traj[1] : T.traj[2])) + (size_t)inst * T.nrows * len;
+  const float* __restrict__ traj = (arr == 0 ? T.traj[0] : (arr == 1 ? T.traj[1] : T.traj[2])) + (size_t)inst * T.inst_rows * len;
   const float* wts = BATCH ? T.weights + (size_t)inst * (T.mean_weight_index + 1) : T.weights;
   const int per = (T.nrows + TB_CHUNKS - 1) / TB_CHUNKS;
   const int r0 = chunk * per, r1 = min(T.nrows, r0 + per);
@@ -550,6 +552,20 @@ __global__ void __launch_bounds__(128, 8) trajbar_final_kernel(const TrajArgs T)
   }
 }
 
+// Ensemble plans (n_ens = K >= 2): rews[b][i] = (((r[b][0][i] + r[b][1][i]) + ...) + r[b][K-1][i]) / K
+// over the member rewards r [B][K][n1], in member order, fp32 with round-to-nearest (the library is
+// built with -use_fast_math, whose `/` is approximate).  One thread per (instance, sample).
+__global__ void __launch_bounds__(256) ensemble_mean_kernel(const float* __restrict__ r, int K, int n1, int total,
+                                                            float* __restrict__ rews) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= total) return;
+  const int b = j / n1, i = j - b * n1;
+  const float* rb = r + (size_t)b * K * n1 + i;
+  float s = rb[0];
+  for (int k = 1; k < K; ++k) s = __fadd_rn(s, rb[(size_t)k * n1]);
+  rews[j] = __fdiv_rn(s, (float)K);
+}
+
 // ---------------------------------------------------------------------------------
 // plan object
 // ---------------------------------------------------------------------------------
@@ -561,11 +577,12 @@ struct dial_plan {
   int variant = 0;
   int shape = 0;                // 1 + index into kShapes: the shape-specialised kernel of the variant; 0: generic
   int n_inst = 1;               // independent planner instances (dial_plan_desc.n_inst)
+  int n_ens = 0;                // planning models per instance (dial_plan_desc.n_ens)
   int num_sms = 132;
   size_t smem_bytes = 0;
   // workspaces
-  // trajectory workspaces [Nsample+1, Hs+1, *], double-buffered so that the bars of iteration i
-  // (side stream) can overlap the rollout of iteration i+1
+  // trajectory workspaces [n_inst, max(n_ens, 1), Nsample+1, Hs+1, *], double-buffered so that the bars
+  // of iteration i (side stream) can overlap the rollout of iteration i+1
   float *traj_q[2] = {nullptr, nullptr}, *traj_qd[2] = {nullptr, nullptr}, *traj_x[2] = {nullptr, nullptr};
   int cur = 0;
   float* weights = nullptr;                                        // [Ntotal+1]
@@ -594,6 +611,12 @@ struct dial_plan {
   DevModel* dModels = nullptr;
   DevModel* hModels = nullptr;
   std::vector<cudaEvent_t> model_ev;
+  // ensemble members (dial_plan_set_ensemble_model): the same for [n_inst * n_ens] member slots, and the
+  // members' rewards [n_inst, n_ens, Nsample+1] of one reverse_once (n_ens >= 2)
+  DevModel* dMembers = nullptr;
+  DevModel* hMembers = nullptr;
+  std::vector<cudaEvent_t> member_ev;
+  float* ens_rews = nullptr;
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -640,8 +663,8 @@ extern "C" size_t dial_sizeof(int which) {
 static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, cudaStream_t st) {
   const size_t smem = sizeof(DevModel) + sizeof(DevPlan) + (size_t)wpc * p->hM.warp_floats * sizeof(float);
   int grid = (A.nrows + wpc - 1) / wpc;
-  // per-instance models: ceil(rows_per_inst / wpc) CTAs per instance (rollout_kernel's row mapping)
-  if (A.models && A.rows_per_inst > 0) grid = (A.nrows / A.rows_per_inst) * ((A.rows_per_inst + wpc - 1) / wpc);
+  // per-instance or member models: ceil(model_rows / wpc) CTAs per model slot (rollout_kernel's row mapping)
+  if (A.models && model_rows(A) > 0) grid = (A.nrows / model_rows(A)) * ((model_rows(A) + wpc - 1) / wpc);
   if (A.row_counter) {
     const int resident = p->num_sms * (wpc > 8 ? 1 : 16 / wpc);
     grid = grid < resident ? grid : resident;
@@ -697,11 +720,11 @@ static cudaError_t launch_rollout_any(dial_plan* p, const RolloutArgs& A0, cudaS
   int wpc = f ? atoi(f) : 0;
   if (wpc == 0) {
     wpc = default_wpc(p, A.nrows);
-    // per-instance models: a CTA holds rows of one instance; spread each instance's rows evenly over
-    // the CTAs it needs at that width
-    if (A.models && A.rows_per_inst > 0) {
-      const int cpi = (A.rows_per_inst + wpc - 1) / wpc;
-      wpc = (A.rows_per_inst + cpi - 1) / cpi;
+    // per-instance or member models: a CTA holds rows of one model slot; spread each slot's rows evenly
+    // over the CTAs it needs at that width
+    if (A.models && model_rows(A) > 0) {
+      const int cpi = (model_rows(A) + wpc - 1) / wpc;
+      wpc = (model_rows(A) + cpi - 1) / cpi;
     }
   }
   if (wpc < 1 || wpc > DIAL_MAXTHREADS / 32) return cudaErrorInvalidValue;
@@ -772,6 +795,12 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     }
   }
   p->n_inst = c.n_inst > 1 ? c.n_inst : 1;
+  if (c.n_ens < 0 || c.n_ens > DIAL_MAXENS) { g_err = "n_ens out of range (0..DIAL_MAXENS = " DIAL_STR(DIAL_MAXENS) ")"; delete p; return nullptr; }
+  if (c.n_ens >= 1) {
+    if (c.Ntotal != c.Nsample) { g_err = "an ensemble plan (n_ens >= 1) cannot be sharded (Ntotal must equal Nsample)"; delete p; return nullptr; }
+    if ((int64_t)p->n_inst * c.n_ens * (c.Nsample + 1) > 0x7fffffff) { g_err = "n_inst * n_ens * (Nsample + 1) exceeds 2^31 - 1 rows per rollout launch"; delete p; return nullptr; }
+  }
+  p->n_ens = c.n_ens;
 #ifndef DIAL_ONLY_VARIANT
   // the specialised kernel computes bit for bit what the generic one does; DIAL_FORCE_GENERIC_SHAPE=1
   // keeps the generic kernel (tests compare the two)
@@ -789,13 +818,15 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
   if ((e = cudaMalloc(&p->dP, sizeof(DevPlan))) != cudaSuccess) return bad(e, "cudaMalloc(plan)");
   if ((e = cudaMemcpy(p->dM, &p->hM, sizeof(DevModel), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(model)");
   if ((e = cudaMemcpy(p->dP, &p->hP, sizeof(DevPlan), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(plan)");
-  const size_t B = (size_t)p->n_inst, rows = B * ((size_t)c.Nsample + 1), H = (size_t)c.Hsample + 1;
+  const size_t B = (size_t)p->n_inst, H = (size_t)c.Hsample + 1;
+  const size_t rows = B * (p->n_ens > 1 ? (size_t)p->n_ens : 1) * ((size_t)c.Nsample + 1);   // every member's trajectories
   const dial_model_desc& m = *model;
   for (int b = 0; b < 2; ++b) {
     if ((e = cudaMalloc(&p->traj_q[b], rows * H * m.nq * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_q)");
     if ((e = cudaMalloc(&p->traj_qd[b], rows * H * m.nv * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_qd)");
     if ((e = cudaMalloc(&p->traj_x[b], rows * H * 3 * (m.nbody - 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_x)");
   }
+  if (p->n_ens > 1 && (e = cudaMalloc(&p->ens_rews, rows * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(ens_rews)");
   if ((e = cudaMalloc(&p->weights, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
   if ((e = cudaMalloc(&p->weights2, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
   if ((e = cudaStreamCreateWithFlags(&p->side, cudaStreamNonBlocking)) != cudaSuccess) return bad(e, "cudaStreamCreate(side)");
@@ -837,6 +868,8 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   cudaFree(p->mpc_Msh); cudaFree(p->mpc_Y1); cudaFree(p->mpc_key);
   for (cudaEvent_t e : p->model_ev) if (e) cudaEventDestroy(e);
   cudaFree(p->dModels); cudaFreeHost(p->hModels);
+  for (cudaEvent_t e : p->member_ev) if (e) cudaEventDestroy(e);
+  cudaFree(p->dMembers); cudaFreeHost(p->hMembers); cudaFree(p->ens_rews);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   cudaFree(p->weights2);
@@ -893,53 +926,69 @@ extern "C" int dial_plan_set_stages(dial_plan* p, int n_stage, const float* pose
   return 0;
 }
 
-extern "C" int dial_plan_set_instance_model(dial_plan* p, int b, const dial_model_desc* m, void* stream) {
-  if (!p || !m) return fail("dial_plan_set_instance_model: null argument");
-  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_instance_model: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
-  if (p->hP.c.Ntotal != p->hP.c.Nsample) return fail("dial_plan_set_instance_model: sharded plans (Ntotal != Nsample) share one model");
+// Derive `m`, check it against the plan's model and copy it into slot `slot` of the model array `d`
+// [n] (pinned staging `h`, copy events `ev`), allocating the array on first use with every slot holding
+// the plan's own model and dropping the captured graphs then.  `fn` names the public call in errors.
+static int set_model_slot(dial_plan* p, const char* fn, DevModel*& d, DevModel*& h, std::vector<cudaEvent_t>& evs,
+                          size_t n, size_t slot, const dial_model_desc* m, cudaStream_t st) {
   DevModel* D = new (std::nothrow) DevModel();
   if (!D) return fail("out of memory");
   std::string err;
-  if (!derive_model(*m, *D, err)) { delete D; return fail("dial_plan_set_instance_model: " + err); }
+  if (!derive_model(*m, *D, err)) { delete D; return fail(std::string(fn) + ": " + err); }
   const char* diff = instance_model_difference(p->hM, *D);
   if (diff) {
     delete D;
-    return fail(std::string("dial_plan_set_instance_model: field '") + diff + "' differs from the plan's model "
+    return fail(std::string(fn) + ": field '" + diff + "' differs from the plan's model "
                 "(an instance's model may differ in floats other than timestep, jnt_range and actuator_ctrlrange only)");
   }
-  cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaSuccess;
-  if (!p->dModels) {
+  if (!d) {
     // first call: every slot starts as the plan's own model; the graphs captured so far launch without
-    // per-instance models and are recaptured on their next use
-    const size_t n = (size_t)p->n_inst;
-    if ((e = cudaMallocHost(&p->hModels, n * sizeof(DevModel))) == cudaSuccess &&
-        (e = cudaMalloc(&p->dModels, n * sizeof(DevModel))) == cudaSuccess) {
-      for (size_t i = 0; i < n; ++i) p->hModels[i] = p->hM;
-      e = cudaMemcpy(p->dModels, p->hModels, n * sizeof(DevModel), cudaMemcpyHostToDevice);
+    // this array and are recaptured on their next use
+    if ((e = cudaMallocHost(&h, n * sizeof(DevModel))) == cudaSuccess &&
+        (e = cudaMalloc(&d, n * sizeof(DevModel))) == cudaSuccess) {
+      for (size_t i = 0; i < n; ++i) h[i] = p->hM;
+      e = cudaMemcpy(d, h, n * sizeof(DevModel), cudaMemcpyHostToDevice);
     }
     if (e != cudaSuccess) {
-      cudaFree(p->dModels); cudaFreeHost(p->hModels); p->dModels = nullptr; p->hModels = nullptr;
+      cudaFree(d); cudaFreeHost(h); d = nullptr; h = nullptr;
       delete D;
-      return fail(std::string("dial_plan_set_instance_model: ") + cudaGetErrorString(e));
+      return fail(std::string(fn) + ": " + cudaGetErrorString(e));
     }
-    p->model_ev.assign(n, nullptr);
+    evs.assign(n, nullptr);
     for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     p->mpc_graphs.clear();
   }
   // stream-ordered copy out of the slot's pinned staging; the staging slot is rewritten only after the
   // previous copy out of it has run
-  cudaEvent_t& ev = p->model_ev[b];
+  cudaEvent_t& ev = evs[slot];
   if (ev) e = cudaEventSynchronize(ev);
   else e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
   if (e == cudaSuccess) {
-    p->hModels[b] = *D;
-    e = cudaMemcpyAsync(p->dModels + b, p->hModels + b, sizeof(DevModel), cudaMemcpyHostToDevice, st);
+    h[slot] = *D;
+    e = cudaMemcpyAsync(d + slot, h + slot, sizeof(DevModel), cudaMemcpyHostToDevice, st);
   }
   if (e == cudaSuccess) e = cudaEventRecord(ev, st);
   delete D;
   CUDA_OK(e);
   return 0;
+}
+
+extern "C" int dial_plan_set_instance_model(dial_plan* p, int b, const dial_model_desc* m, void* stream) {
+  if (!p || !m) return fail("dial_plan_set_instance_model: null argument");
+  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_instance_model: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
+  if (p->hP.c.Ntotal != p->hP.c.Nsample) return fail("dial_plan_set_instance_model: sharded plans (Ntotal != Nsample) share one model");
+  return set_model_slot(p, "dial_plan_set_instance_model", p->dModels, p->hModels, p->model_ev, (size_t)p->n_inst,
+                        (size_t)b, m, (cudaStream_t)stream);
+}
+
+extern "C" int dial_plan_set_ensemble_model(dial_plan* p, int b, int k, const dial_model_desc* m, void* stream) {
+  if (!p || !m) return fail("dial_plan_set_ensemble_model: null argument");
+  if (p->n_ens < 1) return fail("dial_plan_set_ensemble_model: the plan has no ensemble (dial_plan_desc.n_ens = 0)");
+  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_ensemble_model: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
+  if (k < 0 || k >= p->n_ens) return fail("dial_plan_set_ensemble_model: member " + std::to_string(k) + " out of range (0.." + std::to_string(p->n_ens - 1) + ")");
+  return set_model_slot(p, "dial_plan_set_ensemble_model", p->dMembers, p->hMembers, p->member_ev,
+                        (size_t)p->n_inst * p->n_ens, (size_t)b * p->n_ens + k, m, (cudaStream_t)stream);
 }
 
 extern "C" int dial_plan_get_task(const dial_plan* p, dial_task* out) {
@@ -1069,7 +1118,7 @@ static int enqueue_trajbar(dial_plan* p, const float* weights, int rank, float* 
   T.ncol[0] = m.nq; T.ncol[1] = m.nv; T.ncol[2] = 3 * (m.nbody - 1);
   T.coloff[0] = 0; T.coloff[1] = m.nq; T.coloff[2] = m.nq + m.nv;
   T.coltot = m.nq + m.nv + 3 * (m.nbody - 1);
-  T.nrows = rows; T.H = H; T.weights = w; T.w_offset = c.shard_offset; T.mean_row = c.Nsample;
+  T.nrows = rows; T.inst_rows = (p->n_ens > 1 ? p->n_ens : 1) * rows; T.H = H; T.weights = w; T.w_offset = c.shard_offset; T.mean_row = c.Nsample;
   T.mean_weight_index = c.Ntotal; T.include_mean = rank == 0 ? 1 : 0; T.partial = p->tb_partial;
   const int maxlen = H * (T.ncol[2] > T.ncol[0] ? T.ncol[2] : T.ncol[0]);   // nq = nv + 1 > nv always
   const dim3 g1((maxlen + 255) / 256, TB_CHUNKS, 3 * p->n_inst), g2(H, p->n_inst);
@@ -1198,6 +1247,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
   const dial_plan_desc& c = p->hP.c;
   const dial_mpc_buffers& B = p->mpc;
   const int n1 = c.Hnode + 1, nu = p->hM.m.nu, ni = p->n_inst;
+  const int K = p->n_ens > 1 ? p->n_ens : 1;   // rollout rows per sample
   const bool batched = ni > 1;
   float* Y[2] = {B.Y, p->mpc_Y1};
   int cur = 0;
@@ -1241,17 +1291,25 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     if (bars && i >= 2) CUDA_OK(cudaStreamWaitEvent(st, p->ev_side[i & 1], 0));
     RolloutArgs A; memset(&A, 0, sizeof(A));
     A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart; A.counters_in = B.counters;
-    A.nrows = ni * (c.Nsample + 1); A.H = c.Hsample + 1; A.mode = 1;
-    if (batched) A.rows_per_inst = c.Nsample + 1;
-    if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? c.Nsample + 1 : 0; }
-    A.models = p->dModels;
+    A.nrows = ni * K * (c.Nsample + 1); A.H = c.Hsample + 1; A.mode = 1;
+    if (batched || p->n_ens > 0) A.rows_per_inst = K * (c.Nsample + 1);
+    if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? K * (c.Nsample + 1) : 0; }
+    // the planner's models: the members (n_ens >= 1; the plan's model until one is set), else the instances'
+    if (p->n_ens > 0) { A.rows_per_model = c.Nsample + 1; A.models = p->dMembers; }
+    else A.models = p->dModels;
     A.Ybar = Y[cur]; A.noise = noise;
     if (fused) A.rng_dev = B.rng; else A.key_dev = p->mpc_key;
     p->cur ^= 1;
-    A.rews = B.rews; A.q = p->traj_q[p->cur]; A.qd = p->traj_qd[p->cur]; A.xpos = p->traj_x[p->cur];
+    A.rews = K > 1 ? p->ens_rews : B.rews; A.q = p->traj_q[p->cur]; A.qd = p->traj_qd[p->cur]; A.xpos = p->traj_x[p->cur];
     A.dbg = p->dbg;
     fill_xch(p, A);
     CUDA_OK(launch_rollout_any(p, A, st));
+    if (K > 1) {   // the member mean of each sample's reward (K = 1: the reward itself, r / 1 == r)
+      const int total = ni * (c.Nsample + 1);
+      ensemble_mean_kernel<<<(total + 255) / 256, 256, 0, st>>>(p->ens_rews, K, c.Nsample + 1, total, B.rews);
+      p->launches++;
+      CUDA_OK(cudaGetLastError());
+    }
     float* w = wts[i & 1];
     XchWait X = xch_wait_args(p, B.rews_all);
     if (fused) {

@@ -158,9 +158,10 @@ class BaseEnv:
         raise NotImplementedError
 
     def plan_desc(self, Nsample=1, Hsample=1, Hnode=2, temp_sample=1.0, M_n2u=None,
-                  Ntotal=None, shard_offset=0, n_inst=1) -> "_capi.dial_plan_desc":
+                  Ntotal=None, shard_offset=0, n_inst=1, n_ens=0) -> "_capi.dial_plan_desc":
         """``n_inst``: independent planner instances sharing this descriptor (batched control-step
-        graph, ``DeviceLoop`` on an ``MBDPI(..., n_instances=n_inst)``)."""
+        graph, ``DeviceLoop`` on an ``MBDPI(..., n_instances=n_inst)``).  ``n_ens``: planning models per
+        instance (``MBDPI(..., n_ensemble=n_ens)``; 0: the instance's own model)."""
         d = _capi.dial_plan_desc()
         d.env_id = self.env_id
         d.Nsample, d.Ntotal, d.shard_offset = int(Nsample), int(Ntotal or Nsample), int(shard_offset)
@@ -184,6 +185,7 @@ class BaseEnv:
             _capi._set(d.M_n2u, M_n2u)
         d.cmd_step = -1
         d.n_inst = int(n_inst)
+        d.n_ens = int(n_ens)
         d.n_stage = 1         # one (unused) stage unless the env has a jump sequence
         self._fill_reward_desc(d)
         return d

@@ -90,6 +90,14 @@ class Plan:
         md = _capi.fill_model_desc(model)
         self._check(self.lib.dial_plan_set_instance_model(self.handle, int(b), C.byref(md), _stream()))
 
+    def set_ensemble_model(self, b: int, k: int, model) -> None:
+        """Member k of instance b's planning ensemble (a plan with ``n_ens`` >= 1): the model its rollout
+        rows run in every later ``mpc_step``; the same checks and stream-ordered copy as
+        ``set_instance_model`` (``dial_plan_set_ensemble_model``)."""
+        model = getattr(model, "model", model)
+        md = _capi.fill_model_desc(model)
+        self._check(self.lib.dial_plan_set_ensemble_model(self.handle, int(b), int(k), C.byref(md), _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

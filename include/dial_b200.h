@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define DIAL_ABI_VERSION 13
+#define DIAL_ABI_VERSION 14
 
 /* capacities of the fixed-size device model */
 #define DIAL_MAXB 24   /* bodies incl. world            */
@@ -42,6 +42,7 @@ extern "C" {
 #define DIAL_MAXSTAGE 12
 #define DIAL_MAXUSER 64 /* user constants of a custom reward */
 #define DIAL_MAXRANK 8  /* GPUs of one NVLink domain sharing the samples */
+#define DIAL_MAXENS 16  /* planning models (ensemble members) of one instance */
 #define DIAL_IPC_HANDLE_BYTES 64
 
 /* environments (reward functors fused into the rollout kernel) */
@@ -141,6 +142,13 @@ typedef struct dial_plan_desc {
    * only, with the fused update; they cannot be sharded (Ntotal == Nsample) and need
    * Nsample + 1 <= 2^17. */
   int32_t n_inst;
+  /* ensemble planning (0..DIAL_MAXENS).  0: every rollout row of instance b runs instance b's model (the
+   * default).  K >= 1: instance b plans against K member models (dial_plan_set_ensemble_model) while its
+   * env step runs its instance model (dial_plan_set_instance_model), the plant.  Each reverse_once of
+   * dial_mpc_step rolls all Nsample+1 rows of instance b once per member, with the same perturbations,
+   * and scores sample i by the fp32 mean of its K rewards, summed in member order, then divided by K.
+   * Sharded plans reject n_ens >= 1. */
+  int32_t n_ens;
 } dial_plan_desc;
 
 /* The task of one planner instance: exactly the reward inputs that differ between tasks of one model,
@@ -343,8 +351,11 @@ typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound 
    * contents: the caller may rewrite tasks between dial_mpc_step calls with a copy on the same stream
    * (stream-ordered, like dial_plan_set_command).  Each task must satisfy the ranges of dial_task. */
   const dial_task* tasks;
-  /* Per-instance models are not a buffer: dial_plan_set_instance_model (below) writes them into a
-   * plan-owned array that every launch of dial_mpc_step reads. */
+  /* Per-instance and ensemble models are not buffers: dial_plan_set_instance_model and
+   * dial_plan_set_ensemble_model (below) write them into plan-owned arrays that dial_mpc_step reads.
+   * With n_ens = K >= 1, rews [B,Nsample+1] receives the member mean of each sample's reward, and
+   * qbar / qdbar / xbar are the weighted means of member 0's trajectories: member 0 is the prediction
+   * the caller reads. */
 } dial_mpc_buffers;
 
 /* Give instance b (0 <= b < n_inst; b = 0 for a single-instance plan) of the plan its own physical model
@@ -354,8 +365,10 @@ typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound 
  * timestep, jnt_range and actuator_ctrlrange (the plan descriptor holds copies of them); any other float
  * may differ.  Otherwise the call fails and dial_last_error names the first field that differs.  The
  * plan's gains, torque limits, joint ranges and dt stay shared by every instance.
- * Only dial_mpc_step reads per-instance models (the env-step row and every rollout row of instance b):
- * instance b's results are then bitwise those of a plan created from m.  dial_env_step(_kin),
+ * Only dial_mpc_step reads per-instance models: the env-step row of instance b and, on a plan with
+ * n_ens = 0, every rollout row of instance b; instance b's results are then bitwise those of a plan
+ * created from m.  With n_ens >= 1 the instance model is the plant only (the env-step row); the rollout
+ * rows run the member models of dial_plan_set_ensemble_model.  dial_env_step(_kin),
  * dial_pipeline_init, dial_rollout and the eager dial_reverse_* keep using the plan's own model.
  * The copy is stream-ordered on `stream`, out of plan-owned pinned staging, so it may be issued between
  * dial_mpc_step calls like dial_plan_set_command.  The first call on a plan allocates the per-instance
@@ -364,6 +377,16 @@ typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound 
  * Launches with per-instance models give each instance's rows CTAs of their own (each CTA stages one
  * model), with at most the warps per CTA of the default policy (dial_rollout_wpc). */
 int dial_plan_set_instance_model(dial_plan* plan, int b, const dial_model_desc* m, void* stream);
+
+/* Member k (0 <= k < n_ens) of instance b's planning ensemble on a plan with n_ens >= 1: the rollout
+ * rows of member (b, k) run model `m` in every reverse_once of dial_mpc_step.  The same checks, errors
+ * and stream-ordered copy out of plan-owned pinned staging as dial_plan_set_instance_model.  The first
+ * call allocates the member array [n_inst * n_ens] (every slot starts as the plan's own model, not the
+ * instance's) and drops the captured graphs; fails on a plan with n_ens == 0 and for b or k out of range.
+ * n_ens = 1 with no member set plans on the plan's model, bitwise as n_ens = 0 without instance models:
+ * the mismatch experiment, with the plant set by dial_plan_set_instance_model.  Launches with members
+ * give each member's Nsample+1 rows CTAs of their own, as per-instance models do per instance. */
+int dial_plan_set_ensemble_model(dial_plan* plan, int b, int k, const dial_model_desc* m, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops
@@ -378,7 +401,8 @@ int dial_mpc_bind(dial_plan* plan, const dial_mpc_buffers* buffers, const float*
 int dial_mpc_step(dial_plan* plan, int n_diffuse, int env_step, void* stream);
 /* A batched plan advances all B loops in the same graph: the env step rolls B rows, the shift runs
  * one CTA per instance, every reverse_once is one rollout launch over B (Nsample+1) rows and one
- * fused update launch over B instances.  DIAL_NO_FUSED_UPDATE is an error on a batched plan.  The
+ * fused update launch over B instances.  With n_ens = K >= 2 the rollout covers B K (Nsample+1) rows,
+ * row ((b K) + k)(Nsample+1) + i, and one more small launch averages the members' rewards into rews.  DIAL_NO_FUSED_UPDATE is an error on a batched plan.  The
  * eager dial_reverse_rollout / _update(_x) / _trajbar / _trajectories reject batched plans;
  * dial_rollout, dial_env_step(_kin) and dial_pipeline_init keep their single-instance meaning. */
 

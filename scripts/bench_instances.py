@@ -12,7 +12,11 @@ plans its own velocity command (vx spread over [-1, 1], a per-instance task boun
 ``DeviceLoop(..., envs=...)``) instead of the config's shared one.  ``--distinct-models``: instance b
 runs its own physical model (base mass +3 kg * b / B, foot friction 1 - 0.5 b / B where the model has
 feet ``FR FL RR RL``, else every pair's friction scaled so; a per-instance model bound through
-``dial_plan_set_instance_model``)."""
+``dial_plan_set_instance_model``).  ``--ensemble K``: every instance plans against K member models
+(dial_plan_desc.n_ens) spread as ``--distinct-models`` spreads the instances (member k: base mass
++3 kg * k / K, friction 1 - 0.5 k / K), bound through ``dial_plan_set_ensemble_model``.
+``--profile-kernels``: instead of the timing, run the steps without graph capture under torch.profiler and
+print the mean device time per launch of the rollout, update and ensemble-mean kernels."""
 import argparse
 import copy
 import json
@@ -43,9 +47,15 @@ def main():
                     help="bind one task per instance: B distinct forward-velocity commands")
     ap.add_argument("--distinct-models", action="store_true",
                     help="bind one physical model per instance: B distinct base masses and foot frictions")
+    ap.add_argument("--ensemble", type=int, default=0, metavar="K",
+                    help="plan every instance against K member models: K distinct base masses and foot frictions")
+    ap.add_argument("--profile-kernels", action="store_true",
+                    help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
     if args.instances < 1 or args.steps < 1:
         ap.error("--instances and --steps must be at least 1")
+    if args.profile_kernels:
+        os.environ["DIAL_NO_GRAPH"] = "1"     # kernels of a replayed graph are not listed one by one
     import numpy as np
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
@@ -55,7 +65,7 @@ def main():
     B, b = args.instances, BASELINE[args.config]
     cfg = dial_config(args.config, world=1)
     env = product_env(b["env"])
-    mb = MBDPI(cfg, env, n_instances=B)
+    mb = MBDPI(cfg, env, n_instances=B, n_ensemble=args.ensemble)
     state = env.reset(drandom.PRNGKey(0))
     for _ in range(10):
         state = env.step(state, torch.zeros(mb.nu, device=mb.device))
@@ -67,24 +77,44 @@ def main():
             ap.error(f"--distinct-tasks sweeps default_vx, which {type(env).__name__} has not")
         envs = [E.get_environment(b["env"], config=replace(env._config, default_vx=float(v)))
                 for v in np.linspace(-1.0, 1.0, B)]
+    m = env.sys.model
+    torso = int(env.plan_desc().torso_body)
+
+    def spread(e, f):
+        """e with base mass + 3 kg * f and every contact pair's friction scaled by 1 - 0.5 f."""
+        e = copy.copy(e)
+        e.sys = e.sys.tree_replace({"body_mass": {m.names["body"][torso]: m.arrays["body_mass"][torso] + 3.0 * f},
+                                    "pair_friction": m.arrays["pair_friction"] * (1.0 - 0.5 * f)})
+        return e
     if args.distinct_models:
-        m = env.sys.model
-        torso = int(env.plan_desc().torso_body)
         base = [env if envs is None else envs[i] for i in range(B)]
-        envs = []
-        for i, e in enumerate(base):
-            e = copy.copy(e)
-            e.sys = e.sys.tree_replace({"body_mass": {m.names["body"][torso]: m.arrays["body_mass"][torso] + 3.0 * i / B},
-                                        "pair_friction": m.arrays["pair_friction"] * (1.0 - 0.5 * i / B)})
-            envs.append(e)
+        envs = [spread(e, i / B) for i, e in enumerate(base)]
+    members = [spread(env, k / args.ensemble).sys for k in range(args.ensemble)] if args.ensemble else None
     if B == 1:
-        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs)
+        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members)
     else:
-        loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs)
+        loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
+                          ensemble=members)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=mb.device)
     for _ in range(max(args.warmup, 3)):
         loop.step(cfg.Ndiffuse, env_step=2)
     torch.cuda.synchronize()
+    if args.profile_kernels:
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.steps):
+                loop.step(cfg.Ndiffuse, env_step=2)
+            torch.cuda.synchronize()
+        acc = {}
+        for ev in prof.events():
+            for key in ("rollout_kernel", "update_kernel", "ensemble_mean_kernel", "trajbar"):
+                if key in ev.name and ev.device_type.name == "CUDA":
+                    n, tot = acc.get(key, (0, 0.0))
+                    acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
+        print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
+                              kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
+        return
     evs = []
     for _ in range(args.steps):
         flush.zero_()
@@ -95,9 +125,9 @@ def main():
         evs.append((e0, e1))
     torch.cuda.synchronize()
     t = sum(a.elapsed_time(e) for a, e in evs) / 1e3 / args.steps
-    rows = B * (cfg.Nsample + 1)
+    rows = B * max(args.ensemble, 1) * (cfg.Nsample + 1)
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
-                          distinct_models=args.distinct_models, rows_per_rollout=rows,
+                          distinct_models=args.distinct_models, ensemble=args.ensemble, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
                           value=B * cfg.Ndiffuse * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))

@@ -1,0 +1,90 @@
+"""Closed-loop comparison of a nominal planner and an ensemble planner on robots that differ from the model.
+
+    python scripts/ensemble_eval.py --plants 8 --steps 200 --ensemble 4
+
+Go2 trot at BASELINE configs[0] size.  B plants span a payload on the base of +0 ... +6 kg and a foot friction
+of 1.0 ... 0.4 (plant b: payload 6 b / (B-1) kg, friction 1 - 0.6 b / (B-1)); every instance starts from the
+same reset state and its own planner rng.  Planner A plans on the nominal model (n_ens = 1, the plain mismatch
+experiment).  Planner B plans on a K-member ensemble spanning the same range (member k: payload 6 k / (K-1) kg,
+friction 1 - 0.6 k / (K-1)) and weights every sample by its reward averaged over the members.  Both run the
+reference's closed loop (env step, shift, Ndiffuse iterations) for --steps control steps in one control-step
+graph per step, B instances at a time.  Prints a table per plant: mean env-step reward, minimum base height
+and whether the robot fell (base height below --fall-height at any step), and one JSON line."""
+import argparse
+import copy
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from scripts.bench_instances import gpu_info  # noqa: E402
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--plants", type=int, default=8)
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--ensemble", type=int, default=4)
+    ap.add_argument("--fall-height", type=float, default=0.15)
+    args = ap.parse_args()
+    if args.plants < 2 or args.ensemble < 2 or args.steps < 1:
+        ap.error("--plants and --ensemble must be at least 2, --steps at least 1")
+    import numpy as np
+    import torch
+    from baseline_configs import BASELINE, dial_config, product_env
+    from dial_mpc_b200 import random as drandom
+    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop
+
+    cfg = dial_config(0, world=1)
+    env = product_env(BASELINE[0]["env"])
+    m = env.sys.model
+    base = m.body_id("base")
+
+    def model(f):
+        """env's model with payload 6 f kg on the base and the feet's sliding friction scaled by 1 - 0.6 f
+        (f in [0, 1]; the contact pairs of the Go2 scene are the four feet on the floor)."""
+        fr = m.arrays["pair_friction"].copy()
+        fr[:, :2] *= 1.0 - 0.6 * f
+        e = copy.copy(env)
+        e.sys = env.sys.tree_replace({"body_mass": {"base": m.arrays["body_mass"][base] + 6.0 * f},
+                                      "pair_friction": fr})
+        return e
+
+    B, K = args.plants, args.ensemble
+    plants = [model(b / (B - 1)) for b in range(B)]
+    members = [model(k / (K - 1)).sys for k in range(K)]
+    rng, rng_reset = drandom.split(drandom.PRNGKey(cfg.seed))
+    results = {}
+    for name, ens in (("nominal", [env.sys]), (f"ensemble{K}", members)):
+        mb = MBDPI(cfg, env, n_instances=B, n_ensemble=len(ens))
+        states = [p.reset(rng_reset) for p in plants]
+        rngs = np.stack([drandom.split(drandom.PRNGKey(cfg.seed + b))[1] for b in range(B)])
+        loop = DeviceLoop(mb, states, rngs, envs=plants, ensemble=ens)
+        rew, height = [], []
+        for t in range(args.steps):
+            loop.step(cfg.Ndiffuse_init if t == 0 else cfg.Ndiffuse)
+            rew.append(loop.buf["reward"].clone())
+            height.append(loop.buf["qpos"][:, 2].clone())
+        rew, height = torch.stack(rew).cpu().numpy(), torch.stack(height).cpu().numpy()
+        results[name] = dict(mean_reward=rew.mean(0).tolist(), min_height=height.min(0).tolist(),
+                             fell=(height < args.fall_height).any(0).tolist())
+    print(f"Go2 trot, configs[0] size (N={cfg.Nsample}, H={cfg.Hsample}, Ndiffuse={cfg.Ndiffuse}), {args.steps} steps")
+    names = list(results)
+    print("| payload kg | friction | " + " | ".join(f"{n} reward | {n} min height | {n} fell" for n in names) + " |")
+    print("|---|---|" + "---|---|---|" * len(names))
+    for b in range(B):
+        f = b / (B - 1)
+        cells = []
+        for n in names:
+            r = results[n]
+            cells += [f"{r['mean_reward'][b]:.3f}", f"{r['min_height'][b]:.3f}", "yes" if r["fell"][b] else "no"]
+        print(f"| {6 * f:.2f} | {1 - 0.6 * f:.2f} | " + " | ".join(cells) + " |")
+    for n in names:
+        r = results[n]
+        print(f"{n}: mean reward {np.mean(r['mean_reward']):.4f}, falls {sum(r['fell'])} of {B}")
+    print(json.dumps(dict(steps=args.steps, plants=B, ensemble=K, results=results, gpu=gpu_info())))
+
+
+if __name__ == "__main__":
+    main()
