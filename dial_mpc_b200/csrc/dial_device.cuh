@@ -25,6 +25,8 @@
 #include "warp_emul.h"
 #define DEV inline
 #define HD inline
+// the emulator does not model the GPU's fused multiply-adds: a pinned one rounds as the unpinned code does there
+inline float __fmaf_rn(float a, float b, float c) { return a * b + c; }
 #else
 #define HD __host__ __device__ __forceinline__
 #define DEV __device__ __forceinline__
@@ -226,11 +228,13 @@ struct ShapeRT {
 
 #ifdef DIAL_SHAPE_NBODY
 // Internal linkage: a specialised unit's rollout_kernel<3, 6, ShapeFixed> and shape_matches<ShapeFixed>
-// hold its own values and must not be merged with another unit's at link time.  The contact count and the
-// plan's selectors (env_id, nfeet, n_frames) stay run-time values (inherited from ShapeRT): fixing them
-// lets the compiler merge code across branches that are taken at run time and fuse a different set of
-// multiply-adds, which changes the fp32 rounding of the rows (measured on H100: rewards differ in the
-// last bits); the fields below leave every row bit for bit as the generic kernel computes it.
+// hold its own values and must not be merged with another unit's at link time.  With a fixed contact count
+// the compiler split the line search's final `qacc += alpha * search` and `Ma += alpha * mv` updates
+// (linesearch_core) into a multiply and an add where the generic kernel fuses them, so rewards differed in
+// the last bits on H100; those two updates are written with __fmaf_rn, as the generic kernel compiles them
+// (scripts/contraction_diff.py compares the fused/unfused mix of every line in the two kernels).  The fields
+// below leave every row bit for bit as the generic kernel computes it.  env_id stays a run-time value
+// (inherited from ShapeRT).
 namespace {
 struct ShapeFixed : ShapeRT {
   static HD constexpr int nbody(const DevModel&) { return DIAL_SHAPE_NBODY; }
@@ -246,6 +250,15 @@ struct ShapeFixed : ShapeRT {
   static HD constexpr int pair_kind(const DevModel&, int) { return DIAL_SHAPE_PAIR_KIND; }  // every pair
   static HD constexpr int iterations(const DevModel&) { return DIAL_SHAPE_ITERATIONS; }
   static HD constexpr int ls_iterations(const DevModel&) { return DIAL_SHAPE_LS_ITERATIONS; }
+  // the library build always defines these; without them (scripts/contraction_diff.py) they stay run-time
+#ifdef DIAL_SHAPE_NCON
+  static HD constexpr int ncon(const DevModel&) { return DIAL_SHAPE_NCON; }
+  static HD constexpr int nedge(const DevModel&) { return DIAL_SHAPE_NEDGE; }
+#endif
+#ifdef DIAL_SHAPE_NFEET
+  static HD constexpr int nfeet(const dial_plan_desc&) { return DIAL_SHAPE_NFEET; }
+  static HD constexpr int n_frames(const dial_plan_desc&) { return DIAL_SHAPE_N_FRAMES; }
+#endif
 };
 }  // namespace
 #endif
@@ -1362,8 +1375,10 @@ DEV void linesearch_core(WarpCtx& w, Solver& S, float mv, float e_jv) {
   bool improved = (lo.cost < p0.cost) || (hi.cost < p0.cost);
   float alpha = (lo.cost < hi.cost) ? lo.alpha : hi.alpha;
   if (!improved) alpha = 0.f;
-  S.qacc += alpha * S.search;
-  S.Ma += alpha * mv;
+  // fused, as the kernels with a run-time contact count compile them: with the count fixed (ShapeFixed)
+  // the compiler splits them into a multiply and an add, which round twice
+  S.qacc = __fmaf_rn(alpha, S.search, S.qacc);
+  S.Ma = __fmaf_rn(alpha, mv, S.Ma);
   S.l_Jaref += alpha * l_jv;
   S.e_Jaref += alpha * e_jv;
 }

@@ -3,10 +3,11 @@
 
 The stock library builds the star<3,6> kernel once more for each entry of ``SHAPES``, specialised on the
 values derived here from the model JSON the environment loads: body / dof / actuator counts, tree depth,
-kinematic trees, the star chains, the contact pair kind and the solver's iteration counts.  A plan uses
-such a kernel only when the host finds every one of these values equal to its own model
-(``shape_matches``); anything else runs the generic kernel.  Float data (masses, time steps, gains,
-ranges) is never part of the structure."""
+kinematic trees, the star chains, the contact pair kind, the contact and pyramid-edge counts and the
+solver's iteration counts; and from the environment's plan under its default configuration: the number of
+feet and the physics steps per env step.  A plan uses such a kernel only when the host finds every one of
+these values equal to its own model and plan (``shape_matches``); anything else runs the generic kernel.
+Float data (masses, time steps, gains, ranges) is never part of the structure."""
 from __future__ import annotations
 
 from typing import List, Optional
@@ -16,10 +17,11 @@ from typing import List, Optional
 SHAPES = (("go2", "unitree_go2_walk"),)
 
 
-def structure_defines(md) -> Optional[List[str]]:
-    """``NAME=value`` defines of the structure of model descriptor ``md``, or None when it has no single
-    value for a field the policy fixes (chains of different lengths, mixed contact pair kinds, no star of
-    hanging chains)."""
+def structure_defines(md, pd=None) -> Optional[List[str]]:
+    """``NAME=value`` defines of the structure of model descriptor ``md`` (and, given plan descriptor
+    ``pd``, of the plan's feet and physics steps per env step), or None when it has no single value for a
+    field the policy fixes (chains of different lengths, mixed contact pair kinds, no star of hanging
+    chains)."""
     nb, nv = md.nbody, md.nv
     depth = [md.body_depth[b] for b in range(1, nb)]
     roots = {md.body_rootid[b] for b in range(1, nb)}
@@ -50,16 +52,21 @@ def structure_defines(md) -> Optional[List[str]]:
         return None
     vals = dict(NBODY=nb, NQ=md.nq, NV=nv, NU=md.nu, MAXDEPTH=max(depth), NROOT=len(roots), NCHAIN=len(lens),
                 CHAINLEN=lens[0], SB_NROOT=len(root_bodies), PAIR_KIND=kinds.pop(), ITERATIONS=md.iterations,
-                LS_ITERATIONS=md.ls_iterations)
+                LS_ITERATIONS=md.ls_iterations,
+                # pyramidal cones: four edges per contact (dial_host.h, DevModel.nedge of the star paths)
+                NCON=md.ncon, NEDGE=4 * md.ncon)
+    if pd is not None:
+        vals.update(NFEET=pd.nfeet, N_FRAMES=pd.n_frames)
     return [f"DIAL_SHAPE_{k}={int(v)}" for k, v in vals.items()]
 
 
 def env_structure_defines(env_name: str) -> List[str]:
-    """The defines of the model a registered environment loads under its default configuration."""
+    """The defines of the model a registered environment loads, and of its plan, under its default
+    configuration."""
     import dial_mpc_b200.envs as E
     from dial_mpc_b200 import _capi
     env = E.get_environment(env_name, config=E.get_config(env_name)())
-    d = structure_defines(_capi.fill_model_desc(env.sys.model))
+    d = structure_defines(_capi.fill_model_desc(env.sys.model), env.plan_desc())
     if d is None:
         raise ValueError(f"{env_name}: the model has no fixed structure to specialise on")
     return d
