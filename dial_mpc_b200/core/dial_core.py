@@ -11,6 +11,7 @@ from __future__ import annotations
 import argparse
 import dataclasses
 import importlib
+import math
 import os
 import sys
 import time
@@ -303,7 +304,7 @@ class DeviceLoop:
     the GPUs inside the kernels (peer-memory exchange), so no host collective sits in the step."""
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
-                 compute_bars: bool = True, noise=None, envs=None, ensemble=None):
+                 compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -328,7 +329,11 @@ class DeviceLoop:
         instance).  ``envs[b]``'s model stays instance b's plant (the env step); the rollouts of member k
         run ``ensemble[k]`` (or ``ensemble[b][k]``), and ``rews`` receives each sample's reward averaged
         over the members.  A member whose model equals ``mbdpi.env``'s needs no upload; None: every
-        member is ``mbdpi.env``'s model."""
+        member is ``mbdpi.env``'s model.
+
+        ``risk`` (an ensemble ``mbdpi``): how each sample's member rewards become its score, one risk spec
+        for every instance or a list of B (``risk_setting``: ``{"aggregate": "mean"}``, the default,
+        ``{"aggregate": "worst"}`` or ``{"aggregate": "cvar", "alpha": a}``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -408,6 +413,15 @@ class DeviceLoop:
             for k, m in enumerate(row):
                 if bytes(_capi.fill_model_desc(m)) != base:
                     pl.set_ensemble_model(b, k, m)
+        if risk is not None:
+            if mbdpi.n_ensemble < 1:
+                raise ValueError("risk= needs an MBDPI built with n_ensemble >= 1")
+            specs = list(risk) if isinstance(risk, (list, tuple)) else [risk] * B
+            if len(specs) != B:
+                raise ValueError(f"risk must be one risk spec or a list of {B}, got a list of {len(specs)}")
+            settings = [risk_setting(s, mbdpi.n_ensemble) for s in specs]   # every spec checked before any upload
+            for b, (mode, alpha) in enumerate(settings):
+                pl.set_ensemble_risk(b, mode, alpha)
 
     @staticmethod
     def _model(env_or_sys):
@@ -489,6 +503,26 @@ class DeviceLoop:
         if not 0 <= k < self.mbdpi.n_ensemble:
             raise IndexError(f"member {k} out of range (0..{self.mbdpi.n_ensemble - 1})")
         self.plan.set_ensemble_model(b, k, self._model(env_or_sys))
+
+    def set_risk(self, b: int, spec) -> None:
+        """Instance b's risk measure over its members' rewards from the next ``step`` on (a risk spec,
+        ``risk_setting``).  A stream-ordered copy on the current stream; the captured graphs are kept."""
+        b = int(b)
+        if self.mbdpi.n_ensemble < 1:
+            raise RuntimeError("set_risk needs an MBDPI built with n_ensemble >= 1")
+        if not 0 <= b < self.n_instances:
+            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        self.plan.set_ensemble_risk(b, *risk_setting(spec, self.mbdpi.n_ensemble))
+
+    def member_rewards(self) -> torch.Tensor:
+        """The member rewards of the last diffusion iteration of the steps launched so far, a new tensor
+        [B, K, Nsample+1] ([K, Nsample+1] for one instance): the rewards each sample's score reduces
+        (``Plan.member_rewards``).  Asynchronous on the current stream."""
+        K = self.mbdpi.n_ensemble
+        if K < 1:
+            raise RuntimeError("member_rewards needs an MBDPI built with n_ensemble >= 1")
+        lead = (self.n_instances,) if self.n_instances > 1 else ()
+        return self.plan.member_rewards(self.plan.empty(*lead, K, self.mbdpi.Nlocal + 1))
 
     def step(self, n_diffuse: Optional[int] = None, env_step=True) -> None:
         """One control step (asynchronous on the current stream).  env_step: True = env step + shift
@@ -594,14 +628,59 @@ def save_run(output_dir, rollout, infos, timestamp=None):
     return states, preds
 
 
+RISK_AGGREGATES = ("mean", "worst", "cvar")
+
+
+def risk_setting(spec, K: int):
+    """A risk spec -> (mode, alpha) of ``dial_plan_set_ensemble_risk`` for K members.  ``{"aggregate":
+    "mean"}``: the member mean (the default); ``{"aggregate": "worst"}``: the minimum, CVaR with alpha = 1/K;
+    ``{"aggregate": "cvar", "alpha": a}``: the mean of the worst fraction a in (0, 1] of the members.
+    Raises ValueError naming the bad key or value."""
+    if not isinstance(spec, dict):
+        raise ValueError(f"a risk spec maps 'aggregate' ({', '.join(RISK_AGGREGATES)}) and, for cvar, 'alpha'; "
+                         f"got {spec!r}")
+    extra = sorted(set(spec) - {"aggregate", "alpha"}, key=str)
+    if extra:
+        raise ValueError(f"unknown key {extra[0]!r} (a risk spec takes 'aggregate' and, for cvar, 'alpha')")
+    agg = spec.get("aggregate")
+    if agg not in RISK_AGGREGATES:
+        raise ValueError(f"aggregate must be one of {', '.join(RISK_AGGREGATES)}, got {agg!r}")
+    mean, cvar = _capi.DEFINES["DIAL_ENS_MEAN"], _capi.DEFINES["DIAL_ENS_CVAR"]
+    if agg != "cvar":
+        if "alpha" in spec:
+            raise ValueError(f"alpha applies to aggregate cvar only, not {agg}")
+        return (mean, 1.0) if agg == "mean" else (cvar, 1.0 / max(int(K), 1))
+    if "alpha" not in spec:
+        raise ValueError("aggregate cvar needs alpha, the fraction of the members it averages, in (0, 1]")
+    a = spec["alpha"]
+    if isinstance(a, bool) or not isinstance(a, (int, float)) or not math.isfinite(a) or not 0 < a <= 1 \
+            or not np.float32(a) > 0:
+        raise ValueError(f"alpha must be a finite number in (0, 1], got {a!r}")
+    return cvar, float(a)
+
+
+def load_risk(spec, K: int):
+    """The ``risk`` entry of an ``--ensemble`` file or an ``--instance-overrides`` mapping: the checked
+    risk spec (``risk_setting``), or None when ``spec`` has no ``risk``.  Raises ValueError starting with
+    'risk: '."""
+    if not isinstance(spec, dict) or spec.get("risk") is None:
+        return None
+    try:
+        risk_setting(spec["risk"], K)
+    except ValueError as e:
+        raise ValueError(f"risk: {e}") from None
+    return dict(spec["risk"])
+
+
 def load_ensemble(spec, env):
     """The ``--ensemble`` file's mapping -> (K member ``System``s, the plant's ``sys`` mapping or None).
     ``members``: a list of K ``System.tree_replace`` mappings of ``env``'s model (``{}``: the nominal
-    model); ``plant`` (optional): one such mapping for every instance's plant.  Raises ValueError naming
-    the entry that is malformed."""
-    if not isinstance(spec, dict) or set(spec) - {"members", "plant"} or "members" not in spec:
-        raise ValueError("must map 'members' (a list of sys mappings) and optionally 'plant' (one sys mapping), got "
-                         f"{sorted(spec) if isinstance(spec, dict) else spec!r}")
+    model); ``plant`` (optional): one such mapping for every instance's plant; ``risk`` (optional): the
+    risk spec of every instance, read by ``load_risk``.  Raises ValueError naming the entry that is
+    malformed."""
+    if not isinstance(spec, dict) or set(spec) - {"members", "plant", "risk"} or "members" not in spec:
+        raise ValueError("must map 'members' (a list of sys mappings) and optionally 'plant' (one sys mapping) and "
+                         f"'risk' (a risk spec), got {sorted(spec) if isinstance(spec, dict) else spec!r}")
     members, plant = spec["members"], spec.get("plant")
     kmax = _capi.DEFINES["DIAL_MAXENS"]
     if not isinstance(members, list) or not 1 <= len(members) <= kmax:
@@ -626,18 +705,19 @@ def load_ensemble(spec, env):
     return out, plant
 
 
-def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None):
+def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
-    ``ensemble``: K planning models shared by every instance (``DeviceLoop(..., ensemble=...)``)."""
+    ``ensemble``: K planning models shared by every instance (``DeviceLoop(..., ensemble=...)``), scored
+    under ``risk`` (one risk spec or B of them, ``DeviceLoop(..., risk=...)``)."""
     mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
         rng, rng_reset = drandom.split(drandom.PRNGKey(seed=dial_config.seed + b))
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
-    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble)
+    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -678,8 +758,11 @@ def main():
                              "instance b runs the config updated by mapping b (its own commands, gait, targets, ...)")
     parser.add_argument("--ensemble", type=str, default=None, metavar="FILE.yaml",
                         help="plan against an ensemble of models: a YAML mapping with 'members', a list of K sys "
-                             "mappings ({} = the nominal model), and optionally 'plant', one sys mapping applied to "
-                             "every instance's simulated robot before its own --instance-overrides sys")
+                             "mappings ({} = the nominal model), optionally 'plant', one sys mapping applied to "
+                             "every instance's simulated robot before its own --instance-overrides sys, and "
+                             "optionally 'risk', how a sample's member rewards become its score: {aggregate: mean} "
+                             "(default), {aggregate: worst} or {aggregate: cvar, alpha: A}; an --instance-overrides "
+                             "mapping may carry its own 'risk'")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -704,12 +787,14 @@ def main():
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
     env = dial_envs.get_environment(dial_config.env_name, config=env_config)
     envs = None
-    members, plant = None, None
+    members, plant, risk = None, None, None
     if args.ensemble is not None:
         if args.eager:
             parser.error("--ensemble runs on the CUDA-graph loop; it excludes --eager")
         try:
-            members, plant = load_ensemble(yaml.safe_load(open(args.ensemble)), env)
+            ens_spec = yaml.safe_load(open(args.ensemble))
+            members, plant = load_ensemble(ens_spec, env)
+            risk = load_risk(ens_spec, len(members))
         except (ValueError, yaml.YAMLError) as e:
             parser.error(f"--ensemble {args.ensemble}: {e}")
     if args.instance_overrides is not None:
@@ -719,15 +804,24 @@ def main():
         if not isinstance(overrides, list) or len(overrides) != args.instances:
             parser.error(f"--instance-overrides must hold a list of {args.instances} mappings (one per instance), "
                          f"got {len(overrides) if isinstance(overrides, list) else type(overrides).__name__}")
-        known = {f.name for f in dataclasses.fields(env_config_type)} | {"sys"}
+        known = {f.name for f in dataclasses.fields(env_config_type)} | {"sys", "risk"}
         envs = []
+        risks = [risk] * args.instances
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields or sys, got "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys or risk, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
             sys_ov = ov.pop("sys", None)
+            if ov.get("risk") is not None:
+                if members is None:
+                    parser.error(f"--instance-overrides entry {b}: risk needs --ensemble (it scores the members' rewards)")
+                try:
+                    risks[b] = load_risk(ov, len(members))
+                except ValueError as e:
+                    parser.error(f"--instance-overrides entry {b}: {e}")
+            ov.pop("risk", None)
             cfg_b = load_dataclass_from_dict(env_config_type, dict(config_dict, **ov), convert_list_to_array=True)
             envs.append(dial_envs.get_environment(dial_config.env_name, config=cfg_b))
             try:
@@ -749,8 +843,10 @@ def main():
         if args.instances > 1:
             envs = [plant_env] * args.instances
     if args.instances > 1:
+        if args.instance_overrides is not None and any(r is not None for r in risks):
+            risk = [r or {"aggregate": "mean"} for r in risks]
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
-                      ensemble=members)
+                      ensemble=members, risk=risk)
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
@@ -761,7 +857,7 @@ def main():
     rews, rollout, infos = [], [], []
     if mbdpi.world_size == 1 and not args.eager:
         # one CUDA graph per control step; the host launches it and logs
-        loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members)
+        loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk)
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):

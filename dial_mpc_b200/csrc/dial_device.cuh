@@ -27,6 +27,10 @@
 #define HD inline
 // the emulator does not model the GPU's fused multiply-adds: a pinned one rounds as the unpinned code does there
 inline float __fmaf_rn(float a, float b, float c) { return a * b + c; }
+// IEEE single operations with round-to-nearest (build with -ffp-contract=off so none is fused)
+inline float __fadd_rn(float a, float b) { return a + b; }
+inline float __fmul_rn(float a, float b) { return a * b; }
+inline float __fdiv_rn(float a, float b) { return a / b; }
 #else
 #define HD __host__ __device__ __forceinline__
 #define DEV __device__ __forceinline__
@@ -193,6 +197,72 @@ struct RolloutArgs {
 
 // rows of one model slot of `models`: a member block of an ensemble plan, else an instance
 HD int model_rows(const RolloutArgs& A) { return A.rows_per_model > 0 ? A.rows_per_model : A.rows_per_inst; }
+
+// ---------------------------------------------------------------------------------
+// Risk measure of an ensemble plan (dial_plan_set_ensemble_risk): how the K >= 2 member rewards of one
+// sample become its score.  The host derives the setting once (ens_risk_derive); the reduction kernel
+// (dial_kernels.cu) applies it per (instance, sample) with ens_risk_reduce, which the emulator build
+// also runs on the CPU.
+// ---------------------------------------------------------------------------------
+struct alignas(16) EnsRisk {
+  int32_t mode;     // DIAL_ENS_MEAN or DIAL_ENS_CVAR
+  int32_t n_tail;   // CVaR: the n_tail lowest rewards count in full
+  float frac;       // CVaR: the weight of the next-lowest reward s_{n_tail} (0: none)
+  float denom;      // CVaR: the divisor (alpha K; n_tail when frac == 0)
+};
+
+// (K, mode, alpha) -> the setting, in fp64 (include/dial_b200.h: dial_plan_set_ensemble_risk)
+inline EnsRisk ens_risk_derive(int K, int mode, float alpha) {
+  EnsRisk R;
+  R.mode = mode; R.n_tail = K; R.frac = 0.f; R.denom = (float)K;
+  if (mode != DIAL_ENS_CVAR) return R;
+  const double t = (double)alpha * K;
+  if (t <= 1.0 + 1e-6) { R.n_tail = 1; R.denom = 1.f; }                       // the worst case: the minimum
+  else if (fabs(t - round(t)) <= 1e-6 * K) { R.n_tail = (int)round(t); R.denom = (float)R.n_tail; }
+  else { R.n_tail = (int)floor(t); R.frac = (float)(t - R.n_tail); R.denom = (float)t; }
+  return R;
+}
+
+// The score of one sample: member k's reward at r[k * stride], 2 <= K <= DIAL_MAXENS.  The mean sums in
+// member order.  CVaR sorts the K rewards in registers (compile-time indices, +inf padding past K) with
+// an odd-even transposition sort: K rounds of adjacent compare-exchanges that swap on a strict `>` only,
+// so equal values (ties, -0 / +0) keep member order and the padding never moves.  Then it sums the
+// n_tail lowest in ascending order, adds frac * s_{n_tail} as a separate multiply and add, and divides.
+// All control flow depends on K and the setting only (uniform across a CTA of the reduction kernel).
+// DEV, not HD: the _rn intrinsics are device functions; the emulator build compiles it for the host.
+DEV float ens_risk_reduce(const float* r, size_t stride, int K, const EnsRisk& R) {
+  if (R.mode == DIAL_ENS_MEAN) {
+    float s = r[0];
+    for (int k = 1; k < K; ++k) s = __fadd_rn(s, r[(size_t)k * stride]);
+    return __fdiv_rn(s, (float)K);
+  }
+  float s[DIAL_MAXENS];
+  bool nan = false;
+#pragma unroll
+  for (int k = 0; k < DIAL_MAXENS; ++k) {
+    s[k] = k < K ? r[(size_t)k * stride] : INFINITY;
+    nan = nan || isnan(s[k]);
+  }
+#pragma unroll
+  for (int pass = 0; pass < DIAL_MAXENS; ++pass) {
+    if (pass >= K) break;
+#pragma unroll
+    for (int j = pass & 1; j + 1 < DIAL_MAXENS; j += 2) {
+      const float a = s[j], b = s[j + 1];
+      const bool swap = a > b;
+      s[j] = swap ? b : a;
+      s[j + 1] = swap ? a : b;
+    }
+  }
+  float acc = s[0], next = s[1];
+#pragma unroll
+  for (int j = 1; j < DIAL_MAXENS; ++j) {
+    if (j < R.n_tail) acc = __fadd_rn(acc, s[j]);
+    if (j == R.n_tail) next = s[j];
+  }
+  if (R.frac > 0.f) acc = __fadd_rn(acc, __fmul_rn(R.frac, next));
+  return nan ? NAN : __fdiv_rn(acc, R.denom);
+}
 
 // ---------------------------------------------------------------------------------
 // Integer structure of the env step as a template policy.  The warp-uniform bounds and selectors the

@@ -552,18 +552,16 @@ __global__ void __launch_bounds__(128, 8) trajbar_final_kernel(const TrajArgs T)
   }
 }
 
-// Ensemble plans (n_ens = K >= 2): rews[b][i] = (((r[b][0][i] + r[b][1][i]) + ...) + r[b][K-1][i]) / K
-// over the member rewards r [B][K][n1], in member order, fp32 with round-to-nearest (the library is
-// built with -use_fast_math, whose `/` is approximate).  One thread per (instance, sample).
-__global__ void __launch_bounds__(256) ensemble_mean_kernel(const float* __restrict__ r, int K, int n1, int total,
-                                                            float* __restrict__ rews) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= total) return;
-  const int b = j / n1, i = j - b * n1;
-  const float* rb = r + (size_t)b * K * n1 + i;
-  float s = rb[0];
-  for (int k = 1; k < K; ++k) s = __fadd_rn(s, rb[(size_t)k * n1]);
-  rews[j] = __fdiv_rn(s, (float)K);
+// Ensemble plans (n_ens = K >= 2): rews[b][i] = instance b's risk measure risk[b] of the member rewards
+// r[b][0..K-1][i] (ens_risk_reduce; the mean: (((r0 + r1) + ...) + r_{K-1}) / K), fp32 with
+// round-to-nearest (the library is built with -use_fast_math, whose `/` is approximate).  One thread per
+// (instance, sample); grid.y is the instance, so a CTA reads one setting and takes one branch.
+__global__ void __launch_bounds__(256) ensemble_reduce_kernel(const float* __restrict__ r, const EnsRisk* __restrict__ risk,
+                                                              int K, int n1, float* __restrict__ rews) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+  if (i >= n1) return;
+  const EnsRisk R = risk[b];
+  rews[(size_t)b * n1 + i] = ens_risk_reduce(r + (size_t)b * K * n1 + i, (size_t)n1, K, R);
 }
 
 // ---------------------------------------------------------------------------------
@@ -617,6 +615,11 @@ struct dial_plan {
   DevModel* hMembers = nullptr;
   std::vector<cudaEvent_t> member_ev;
   float* ens_rews = nullptr;
+  // risk measure per instance (dial_plan_set_ensemble_risk, n_ens >= 2): device array [n_inst] read by
+  // the reduction, its pinned staging and the per-slot events of the last copy, as for the models
+  EnsRisk* dRisk = nullptr;
+  EnsRisk* hRisk = nullptr;
+  std::vector<cudaEvent_t> risk_ev;
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -826,7 +829,15 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     if ((e = cudaMalloc(&p->traj_qd[b], rows * H * m.nv * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_qd)");
     if ((e = cudaMalloc(&p->traj_x[b], rows * H * 3 * (m.nbody - 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_x)");
   }
-  if (p->n_ens > 1 && (e = cudaMalloc(&p->ens_rews, rows * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(ens_rews)");
+  if (p->n_ens > 1) {
+    if ((e = cudaMalloc(&p->ens_rews, rows * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(ens_rews)");
+    // every instance starts at the mean
+    if ((e = cudaMallocHost(&p->hRisk, B * sizeof(EnsRisk))) != cudaSuccess) return bad(e, "cudaMallocHost(risk)");
+    if ((e = cudaMalloc(&p->dRisk, B * sizeof(EnsRisk))) != cudaSuccess) return bad(e, "cudaMalloc(risk)");
+    for (size_t b = 0; b < B; ++b) p->hRisk[b] = ens_risk_derive(p->n_ens, DIAL_ENS_MEAN, 1.f);
+    if ((e = cudaMemcpy(p->dRisk, p->hRisk, B * sizeof(EnsRisk), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(risk)");
+    p->risk_ev.assign(B, nullptr);
+  }
   if ((e = cudaMalloc(&p->weights, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
   if ((e = cudaMalloc(&p->weights2, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
   if ((e = cudaStreamCreateWithFlags(&p->side, cudaStreamNonBlocking)) != cudaSuccess) return bad(e, "cudaStreamCreate(side)");
@@ -870,6 +881,8 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   cudaFree(p->dModels); cudaFreeHost(p->hModels);
   for (cudaEvent_t e : p->member_ev) if (e) cudaEventDestroy(e);
   cudaFree(p->dMembers); cudaFreeHost(p->hMembers); cudaFree(p->ens_rews);
+  for (cudaEvent_t e : p->risk_ev) if (e) cudaEventDestroy(e);
+  cudaFree(p->dRisk); cudaFreeHost(p->hRisk);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   cudaFree(p->weights2);
@@ -989,6 +1002,42 @@ extern "C" int dial_plan_set_ensemble_model(dial_plan* p, int b, int k, const di
   if (k < 0 || k >= p->n_ens) return fail("dial_plan_set_ensemble_model: member " + std::to_string(k) + " out of range (0.." + std::to_string(p->n_ens - 1) + ")");
   return set_model_slot(p, "dial_plan_set_ensemble_model", p->dMembers, p->hMembers, p->member_ev,
                         (size_t)p->n_inst * p->n_ens, (size_t)b * p->n_ens + k, m, (cudaStream_t)stream);
+}
+
+extern "C" int dial_plan_set_ensemble_risk(dial_plan* p, int b, int mode, float alpha, void* stream) {
+  if (!p) return fail("dial_plan_set_ensemble_risk: null plan");
+  if (p->n_ens < 1) return fail("dial_plan_set_ensemble_risk: the plan has no ensemble (dial_plan_desc.n_ens = 0)");
+  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_ensemble_risk: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
+  if (mode != DIAL_ENS_MEAN && mode != DIAL_ENS_CVAR)
+    return fail("dial_plan_set_ensemble_risk: mode " + std::to_string(mode) + " is neither DIAL_ENS_MEAN (0) nor DIAL_ENS_CVAR (1)");
+  if (mode == DIAL_ENS_CVAR && !(alpha > 0.f && alpha <= 1.f)) {   // also rejects NaN and infinities
+    char buf[64];
+    snprintf(buf, sizeof(buf), "%g", (double)alpha);
+    return fail(std::string("dial_plan_set_ensemble_risk: alpha must be finite and in (0, 1] for DIAL_ENS_CVAR, got ") + buf);
+  }
+  if (p->n_ens < 2) return 0;   // one member: every risk measure of one reward is that reward
+  // stream-ordered copy out of the slot's pinned staging, rewritten only after its previous copy has run;
+  // the captured graphs hold the array's pointer and read the new setting at their next replay
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaEvent_t& ev = p->risk_ev[b];
+  cudaError_t e = ev ? cudaEventSynchronize(ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) {
+    p->hRisk[b] = ens_risk_derive(p->n_ens, mode, alpha);
+    e = cudaMemcpyAsync(p->dRisk + b, p->hRisk + b, sizeof(EnsRisk), cudaMemcpyHostToDevice, st);
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
+  if (e != cudaSuccess) return fail(std::string("dial_plan_set_ensemble_risk: ") + cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int dial_plan_member_rewards(dial_plan* p, float* out, void* stream) {
+  if (!p || !out) return fail("dial_plan_member_rewards: null argument");
+  if (p->n_ens < 1) return fail("dial_plan_member_rewards: the plan has no ensemble (dial_plan_desc.n_ens = 0)");
+  if (!p->mpc_bound) return fail("dial_plan_member_rewards: call dial_mpc_bind first");
+  const size_t n = (size_t)p->n_inst * p->n_ens * ((size_t)p->hP.c.Nsample + 1);
+  const float* src = p->n_ens > 1 ? p->ens_rews : p->mpc.rews;   // n_ens = 1: the rollout writes rews itself
+  CUDA_OK(cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
 }
 
 extern "C" int dial_plan_get_task(const dial_plan* p, dial_task* out) {
@@ -1304,9 +1353,9 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     A.dbg = p->dbg;
     fill_xch(p, A);
     CUDA_OK(launch_rollout_any(p, A, st));
-    if (K > 1) {   // the member mean of each sample's reward (K = 1: the reward itself, r / 1 == r)
-      const int total = ni * (c.Nsample + 1);
-      ensemble_mean_kernel<<<(total + 255) / 256, 256, 0, st>>>(p->ens_rews, K, c.Nsample + 1, total, B.rews);
+    if (K > 1) {   // each sample's score under its instance's risk measure (K = 1: the reward itself)
+      const dim3 grid((c.Nsample + 1 + 255) / 256, ni);
+      ensemble_reduce_kernel<<<grid, 256, 0, st>>>(p->ens_rews, p->dRisk, K, c.Nsample + 1, B.rews);
       p->launches++;
       CUDA_OK(cudaGetLastError());
     }

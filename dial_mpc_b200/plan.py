@@ -98,6 +98,20 @@ class Plan:
         md = _capi.fill_model_desc(model)
         self._check(self.lib.dial_plan_set_ensemble_model(self.handle, int(b), int(k), C.byref(md), _stream()))
 
+    def set_ensemble_risk(self, b: int, mode: int, alpha: float = 1.0) -> None:
+        """Instance b's risk measure over its members' rewards (``_capi.DEFINES["DIAL_ENS_MEAN"]`` or
+        ``["DIAL_ENS_CVAR"]`` with ``alpha`` in (0, 1]) from the next ``mpc_step`` on; a stream-ordered copy
+        on the current stream that keeps the captured graphs (``dial_plan_set_ensemble_risk``)."""
+        self._check(self.lib.dial_plan_set_ensemble_risk(self.handle, int(b), int(mode), float(alpha), _stream()))
+
+    def member_rewards(self, out: torch.Tensor) -> torch.Tensor:
+        """Copy the member rewards of the last reverse_once of ``mpc_step`` into ``out``
+        [n_inst * n_ens * (Nsample+1)] elements, instance-, then member-major (``dial_plan_member_rewards``)."""
+        n = max(self.desc.n_inst, 1) * self.desc.n_ens * (self.N + 1)
+        assert self.desc.n_ens < 1 or out.numel() == n, f"need {n} elements, got {tuple(out.shape)}"
+        self._check(self.lib.dial_plan_member_rewards(self.handle, _ptr(out), _stream()))
+        return out
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

@@ -146,7 +146,8 @@ typedef struct dial_plan_desc {
    * default).  K >= 1: instance b plans against K member models (dial_plan_set_ensemble_model) while its
    * env step runs its instance model (dial_plan_set_instance_model), the plant.  Each reverse_once of
    * dial_mpc_step rolls all Nsample+1 rows of instance b once per member, with the same perturbations,
-   * and scores sample i by the fp32 mean of its K rewards, summed in member order, then divided by K.
+   * and scores sample i by a risk measure of its K rewards: the fp32 mean (summed in member order, then
+   * divided by K) unless dial_plan_set_ensemble_risk chose CVaR or the worst case for instance b.
    * Sharded plans reject n_ens >= 1. */
   int32_t n_ens;
 } dial_plan_desc;
@@ -353,7 +354,8 @@ typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound 
   const dial_task* tasks;
   /* Per-instance and ensemble models are not buffers: dial_plan_set_instance_model and
    * dial_plan_set_ensemble_model (below) write them into plan-owned arrays that dial_mpc_step reads.
-   * With n_ens = K >= 1, rews [B,Nsample+1] receives the member mean of each sample's reward, and
+   * With n_ens = K >= 1, rews [B,Nsample+1] receives each sample's score over its member rewards (the
+   * member mean, or the measure dial_plan_set_ensemble_risk sets per instance), and
    * qbar / qdbar / xbar are the weighted means of member 0's trajectories: member 0 is the prediction
    * the caller reads. */
 } dial_mpc_buffers;
@@ -388,6 +390,37 @@ int dial_plan_set_instance_model(dial_plan* plan, int b, const dial_model_desc* 
  * give each member's Nsample+1 rows CTAs of their own, as per-instance models do per instance. */
 int dial_plan_set_ensemble_model(dial_plan* plan, int b, int k, const dial_model_desc* m, void* stream);
 
+/* Risk measures of an ensemble plan: how instance b turns the K member rewards r_0..r_{K-1} of sample i
+ * into its score rews[b][i] (dial_plan_set_ensemble_risk). */
+#define DIAL_ENS_MEAN 0 /* (((r_0 + r_1) + ...) + r_{K-1}) / K in fp32, round-to-nearest: the default */
+#define DIAL_ENS_CVAR 1 /* CVaR_alpha: the mean of the worst alpha-fraction of the members */
+
+/* Instance b's risk measure on a plan with n_ens >= 1, from the next reverse_once of dial_mpc_step on.
+ * mode DIAL_ENS_MEAN (alpha is ignored) or DIAL_ENS_CVAR with alpha finite and in (0, 1]; alpha <= 1/K
+ * is the worst case, the minimum.  With t = alpha K in fp64, the host derives once:
+ *   t <= 1 + 1e-6:                 n_tail = 1,        frac = 0,                 denom = 1
+ *   |t - round(t)| <= 1e-6 K:      n_tail = round(t), frac = 0,                 denom = n_tail
+ *   otherwise:                     n_tail = floor(t), frac = (float)(t - n_tail), denom = (float)t
+ * and the reduction sorts the K rewards ascending (stable in member order: -0 stays before +0 if it
+ * comes first), sets acc = s_0, adds s_1 .. s_{n_tail-1} in that order, adds fmul(frac, s_{n_tail})
+ * when frac > 0 (a separate multiply and add), and writes acc / denom, all fp32 round-to-nearest.
+ * CVaR with alpha = 1 is the mean up to rounding only (another summation order); DIAL_ENS_MEAN alone
+ * reproduces a plan without the call.  A NaN member reward makes the score NaN; infinities go through
+ * the arithmetic.  A non-finite score gets weight 0 in the update, as with the mean.
+ * The copy of the 16-byte setting is stream-ordered on `stream`, out of plan-owned pinned staging that
+ * dial_plan_create allocates with the setting array (n_ens >= 2; every instance starts at the mean), so
+ * the call may be issued between dial_mpc_step calls.  The captured graphs read the array, so they are
+ * kept: the setting takes effect at their next replay.  On a plan with n_ens = 1 any valid setting is
+ * accepted and changes nothing (every measure of one reward is that reward).  Fails on a plan with
+ * n_ens == 0, for b out of range, an unknown mode or a bad alpha. */
+int dial_plan_set_ensemble_risk(dial_plan* plan, int b, int mode, float alpha, void* stream);
+
+/* The member rewards of the last reverse_once of dial_mpc_step, out [dev] [n_inst, n_ens, Nsample+1]
+ * (member k of instance b at (b n_ens + k)(Nsample+1)): the per-member rewards the risk measure reduced
+ * (n_ens >= 2), or the bound rews (n_ens = 1).  A stream-ordered copy on `stream`.  Fails on a plan with
+ * n_ens == 0 and before dial_mpc_bind. */
+int dial_plan_member_rewards(dial_plan* plan, float* out, void* stream);
+
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops
  * previously captured graphs. */
@@ -402,7 +435,8 @@ int dial_mpc_step(dial_plan* plan, int n_diffuse, int env_step, void* stream);
 /* A batched plan advances all B loops in the same graph: the env step rolls B rows, the shift runs
  * one CTA per instance, every reverse_once is one rollout launch over B (Nsample+1) rows and one
  * fused update launch over B instances.  With n_ens = K >= 2 the rollout covers B K (Nsample+1) rows,
- * row ((b K) + k)(Nsample+1) + i, and one more small launch averages the members' rewards into rews.  DIAL_NO_FUSED_UPDATE is an error on a batched plan.  The
+ * row ((b K) + k)(Nsample+1) + i, and one more small launch reduces the members' rewards into rews
+ * under each instance's risk measure.  DIAL_NO_FUSED_UPDATE is an error on a batched plan.  The
  * eager dial_reverse_rollout / _update(_x) / _trajbar / _trajectories reject batched plans;
  * dial_rollout, dial_env_step(_kin) and dial_pipeline_init keep their single-instance meaning. */
 

@@ -14,9 +14,10 @@ runs its own physical model (base mass +3 kg * b / B, foot friction 1 - 0.5 b / 
 feet ``FR FL RR RL``, else every pair's friction scaled so; a per-instance model bound through
 ``dial_plan_set_instance_model``).  ``--ensemble K``: every instance plans against K member models
 (dial_plan_desc.n_ens) spread as ``--distinct-models`` spreads the instances (member k: base mass
-+3 kg * k / K, friction 1 - 0.5 k / K), bound through ``dial_plan_set_ensemble_model``.
++3 kg * k / K, friction 1 - 0.5 k / K), bound through ``dial_plan_set_ensemble_model``, and scores each
+sample by the ``--risk`` measure of its member rewards (mean, worst or cvar:ALPHA; default mean).
 ``--profile-kernels``: instead of the timing, run the steps without graph capture under torch.profiler and
-print the mean device time per launch of the rollout, update and ensemble-mean kernels."""
+print the mean device time per launch of the rollout, update and ensemble reduction kernels."""
 import argparse
 import copy
 import json
@@ -37,6 +38,17 @@ def gpu_info():
         return f"nvidia-smi unavailable: {e}"
 
 
+def risk_spec(tok: str) -> dict:
+    """A --risk token (mean, worst or cvar:ALPHA) -> the risk spec of DeviceLoop(..., risk=...)."""
+    agg, colon, a = tok.partition(":")
+    if not colon:
+        return {"aggregate": agg}
+    try:
+        return {"aggregate": agg, "alpha": float(a)}
+    except ValueError:
+        raise ValueError(f"alpha must be a number, got {a!r}") from None
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", type=int, default=0)
@@ -49,11 +61,15 @@ def main():
                     help="bind one physical model per instance: B distinct base masses and foot frictions")
     ap.add_argument("--ensemble", type=int, default=0, metavar="K",
                     help="plan every instance against K member models: K distinct base masses and foot frictions")
+    ap.add_argument("--risk", default="mean", metavar="MEASURE",
+                    help="with --ensemble: the risk measure of every instance, mean, worst or cvar:ALPHA")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
     if args.instances < 1 or args.steps < 1:
         ap.error("--instances and --steps must be at least 1")
+    if args.risk != "mean" and not args.ensemble:
+        ap.error("--risk needs --ensemble K")
     if args.profile_kernels:
         os.environ["DIAL_NO_GRAPH"] = "1"     # kernels of a replayed graph are not listed one by one
     import numpy as np
@@ -90,11 +106,15 @@ def main():
         base = [env if envs is None else envs[i] for i in range(B)]
         envs = [spread(e, i / B) for i, e in enumerate(base)]
     members = [spread(env, k / args.ensemble).sys for k in range(args.ensemble)] if args.ensemble else None
+    try:
+        risk = risk_spec(args.risk) if args.ensemble else None
+    except ValueError as e:
+        ap.error(f"--risk {args.risk}: {e}")
     if B == 1:
-        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members)
+        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
-                          ensemble=members)
+                          ensemble=members, risk=risk)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=mb.device)
     for _ in range(max(args.warmup, 3)):
         loop.step(cfg.Ndiffuse, env_step=2)
@@ -107,12 +127,12 @@ def main():
             torch.cuda.synchronize()
         acc = {}
         for ev in prof.events():
-            for key in ("rollout_kernel", "update_kernel", "ensemble_mean_kernel", "trajbar"):
+            for key in ("rollout_kernel", "update_kernel", "ensemble_reduce_kernel", "trajbar"):
                 if key in ev.name and ev.device_type.name == "CUDA":
                     n, tot = acc.get(key, (0, 0.0))
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
         print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
-                              kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              risk=args.risk, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
                               launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
         return
     evs = []
@@ -127,7 +147,7 @@ def main():
     t = sum(a.elapsed_time(e) for a, e in evs) / 1e3 / args.steps
     rows = B * max(args.ensemble, 1) * (cfg.Nsample + 1)
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
-                          distinct_models=args.distinct_models, ensemble=args.ensemble, rows_per_rollout=rows,
+                          distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
                           value=B * cfg.Ndiffuse * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))

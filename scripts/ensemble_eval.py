@@ -1,12 +1,13 @@
 """Closed-loop comparison of a nominal planner and an ensemble planner on robots that differ from the model.
 
-    python scripts/ensemble_eval.py --plants 8 --steps 200 --ensemble 4
+    python scripts/ensemble_eval.py --plants 8 --steps 200 --ensemble 4 [--risk mean worst cvar:0.5]
 
 Go2 trot at BASELINE configs[0] size.  B plants span a payload on the base of +0 ... +6 kg and a foot friction
 of 1.0 ... 0.4 (plant b: payload 6 b / (B-1) kg, friction 1 - 0.6 b / (B-1)); every instance starts from the
 same reset state and its own planner rng.  Planner A plans on the nominal model (n_ens = 1, the plain mismatch
 experiment).  Planner B plans on a K-member ensemble spanning the same range (member k: payload 6 k / (K-1) kg,
-friction 1 - 0.6 k / (K-1)) and weights every sample by its reward averaged over the members.  Both run the
+friction 1 - 0.6 k / (K-1)) and weights every sample by a risk measure of its member rewards; --risk lists
+the measures (mean, worst, cvar:ALPHA; default mean), one ensemble planner each.  Every planner runs the
 reference's closed loop (env step, shift, Ndiffuse iterations) for --steps control steps in one control-step
 graph per step, B instances at a time.  Prints a table per plant: mean env-step reward, minimum base height
 and whether the robot fell (base height below --fall-height at any step), and one JSON line."""
@@ -18,7 +19,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from scripts.bench_instances import gpu_info  # noqa: E402
+from scripts.bench_instances import gpu_info, risk_spec  # noqa: E402
 
 
 def main():
@@ -27,9 +28,20 @@ def main():
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--ensemble", type=int, default=4)
     ap.add_argument("--fall-height", type=float, default=0.15)
+    ap.add_argument("--risk", nargs="+", default=["mean"], metavar="MEASURE",
+                    help="one ensemble planner per measure: mean, worst or cvar:ALPHA (default: mean)")
     args = ap.parse_args()
     if args.plants < 2 or args.ensemble < 2 or args.steps < 1:
         ap.error("--plants and --ensemble must be at least 2, --steps at least 1")
+    from dial_mpc_b200.core.dial_core import risk_setting
+    risks = []
+    for tok in args.risk:
+        try:
+            spec = risk_spec(tok)
+            risk_setting(spec, args.ensemble)
+        except ValueError as e:
+            ap.error(f"--risk {tok}: {e}")
+        risks.append((tok, spec))
     import numpy as np
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
@@ -56,11 +68,13 @@ def main():
     members = [model(k / (K - 1)).sys for k in range(K)]
     rng, rng_reset = drandom.split(drandom.PRNGKey(cfg.seed))
     results = {}
-    for name, ens in (("nominal", [env.sys]), (f"ensemble{K}", members)):
+    planners = [("nominal", [env.sys], None)]
+    planners += [(f"ensemble{K}" if tok == "mean" else f"ensemble{K}-{tok}", members, spec) for tok, spec in risks]
+    for name, ens, risk in planners:
         mb = MBDPI(cfg, env, n_instances=B, n_ensemble=len(ens))
         states = [p.reset(rng_reset) for p in plants]
         rngs = np.stack([drandom.split(drandom.PRNGKey(cfg.seed + b))[1] for b in range(B)])
-        loop = DeviceLoop(mb, states, rngs, envs=plants, ensemble=ens)
+        loop = DeviceLoop(mb, states, rngs, envs=plants, ensemble=ens, risk=risk)
         rew, height = [], []
         for t in range(args.steps):
             loop.step(cfg.Ndiffuse_init if t == 0 else cfg.Ndiffuse)
@@ -83,7 +97,7 @@ def main():
     for n in names:
         r = results[n]
         print(f"{n}: mean reward {np.mean(r['mean_reward']):.4f}, falls {sum(r['fell'])} of {B}")
-    print(json.dumps(dict(steps=args.steps, plants=B, ensemble=K, results=results, gpu=gpu_info())))
+    print(json.dumps(dict(steps=args.steps, plants=B, ensemble=K, risk=args.risk, results=results, gpu=gpu_info())))
 
 
 if __name__ == "__main__":
