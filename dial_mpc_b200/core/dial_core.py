@@ -304,7 +304,7 @@ class DeviceLoop:
     the GPUs inside the kernels (peer-memory exchange), so no host collective sits in the step."""
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
-                 compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None):
+                 compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -333,7 +333,13 @@ class DeviceLoop:
 
         ``risk`` (an ensemble ``mbdpi``): how each sample's member rewards become its score, one risk spec
         for every instance or a list of B (``risk_setting``: ``{"aggregate": "mean"}``, the default,
-        ``{"aggregate": "worst"}`` or ``{"aggregate": "cvar", "alpha": a}``)."""
+        ``{"aggregate": "worst"}`` or ``{"aggregate": "cvar", "alpha": a}``).
+
+        ``adapt`` (an ensemble ``mbdpi`` with K >= 2): instances that adapt their belief over the members to
+        their plant at every env step and score samples by the belief-weighted risk measure, one adapt spec
+        for every instance or a list of B specs or None (``adapt_setting``: ``{"sigma": s, "forget": 1.0,
+        "prune": 0.0}``).  ``prior``: the starting belief, K weights >= 0 with a positive sum for every
+        instance or B such lists (default uniform; ``set_belief``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -422,6 +428,26 @@ class DeviceLoop:
             settings = [risk_setting(s, mbdpi.n_ensemble) for s in specs]   # every spec checked before any upload
             for b, (mode, alpha) in enumerate(settings):
                 pl.set_ensemble_risk(b, mode, alpha)
+        for name, arg in (("adapt", adapt), ("prior", prior)):
+            if arg is not None and mbdpi.n_ensemble < 2:
+                raise ValueError(f"{name}= needs an MBDPI built with n_ensemble >= 2")
+        if prior is not None:
+            rows = list(prior)
+            per_instance = len(rows) > 0 and all(isinstance(r, (list, tuple, np.ndarray)) for r in rows)
+            rows = rows if per_instance else [rows] * B
+            if len(rows) != B:
+                raise ValueError(f"prior must be K weights or a list of {B} such lists, got a list of {len(rows)}")
+            weights = [prior_setting(r, mbdpi.n_ensemble) for r in rows]
+            for b, w in enumerate(weights):
+                pl.set_ensemble_belief(b, w)
+        if adapt is not None:
+            specs = list(adapt) if isinstance(adapt, (list, tuple)) else [adapt] * B
+            if len(specs) != B:
+                raise ValueError(f"adapt must be one adapt spec or a list of {B}, got a list of {len(specs)}")
+            settings = [None if s is None else adapt_setting(s, mbdpi.n_ensemble, m.nv) for s in specs]
+            for b, st in enumerate(settings):
+                if st is not None:
+                    pl.set_ensemble_adapt(b, True, *st)
 
     @staticmethod
     def _model(env_or_sys):
@@ -513,6 +539,49 @@ class DeviceLoop:
         if not 0 <= b < self.n_instances:
             raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
         self.plan.set_ensemble_risk(b, *risk_setting(spec, self.mbdpi.n_ensemble))
+
+    def _adapt_instance(self, what: str, b) -> int:
+        if self.mbdpi.n_ensemble < 2:
+            raise RuntimeError(f"{what} needs an MBDPI built with n_ensemble >= 2")
+        b = int(b)
+        if not 0 <= b < self.n_instances:
+            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        return b
+
+    def set_adapt(self, b: int, spec) -> None:
+        """Instance b adapts its belief to its plant from the next env step on (an adapt spec,
+        ``adapt_setting``), or stops adapting (None; the belief is kept).  A stream-ordered copy on the
+        current stream; the first instance of a loop to adapt makes the next steps capture their graphs
+        again, later calls keep them."""
+        b = self._adapt_instance("set_adapt", b)
+        if spec is None:
+            self.plan.set_ensemble_adapt(b, False)
+        else:
+            self.plan.set_ensemble_adapt(b, True, *adapt_setting(spec, self.mbdpi.n_ensemble, self.mbdpi.env.sys.nv))
+
+    def set_belief(self, b: int, w) -> None:
+        """Instance b's belief from K weights >= 0 with a positive sum (``prior_setting``), e.g. from an
+        outside estimator; a stream-ordered copy that keeps the captured graphs."""
+        b = self._adapt_instance("set_belief", b)
+        self.plan.set_ensemble_belief(b, prior_setting(w, self.mbdpi.n_ensemble))
+
+    def _belief(self, which: int) -> torch.Tensor:
+        K = self.mbdpi.n_ensemble
+        if K < 2:
+            raise RuntimeError(f"{('belief', 'member_loglik')[which]} needs an MBDPI built with n_ensemble >= 2")
+        out = self.plan.empty(*((self.n_instances,) if self.n_instances > 1 else ()), K)
+        self.plan.ensemble_belief(*((out, None) if which == 0 else (None, out)))
+        return out
+
+    def belief(self) -> torch.Tensor:
+        """The belief over the members after the steps launched so far, a new tensor [B, K] ([K] for one
+        instance).  Asynchronous on the current stream."""
+        return self._belief(0)
+
+    def member_loglik(self) -> torch.Tensor:
+        """The members' log-likelihoods l of each instance's last belief update, [B, K] ([K] for one
+        instance; 0 before the first).  Asynchronous on the current stream."""
+        return self._belief(1)
 
     def member_rewards(self) -> torch.Tensor:
         """The member rewards of the last diffusion iteration of the steps launched so far, a new tensor
@@ -672,15 +741,101 @@ def load_risk(spec, K: int):
     return dict(spec["risk"])
 
 
+def adapt_setting(spec, K: int, nv: int):
+    """An adapt spec -> (forget, prune, sigma [nv] fp32) of ``dial_plan_set_ensemble_adapt`` for K members
+    and nv dofs.  ``sigma`` (required): the scale of each qvel residual, one number for every dof or nv
+    numbers, each finite and > 0; ``forget`` (default 1.0): in (0, 1], how much of the old log-belief each
+    env step keeps; ``prune`` (default 0.0): in [0, 1/K), members with a smaller weight are left out of
+    the score.  Raises ValueError naming the bad key or value."""
+    if not isinstance(spec, dict):
+        raise ValueError(f"an adapt spec maps 'sigma' and optionally 'forget' and 'prune'; got {spec!r}")
+    extra = sorted(set(spec) - {"sigma", "forget", "prune"}, key=str)
+    if extra:
+        raise ValueError(f"unknown key {extra[0]!r} (an adapt spec takes 'sigma', 'forget' and 'prune')")
+    if "sigma" not in spec:
+        raise ValueError("adapt needs sigma, the scale of the qvel residuals: one number or one per dof")
+
+    def num(x):
+        return not isinstance(x, bool) and isinstance(x, (int, float)) and math.isfinite(x)
+
+    s = spec["sigma"]
+    if isinstance(s, (list, tuple)):
+        if len(s) != nv:
+            raise ValueError(f"sigma must be one number or a list of {nv} (one per dof), got a list of {len(s)}")
+        bad = [x for x in s if not (num(x) and np.float32(x) > 0)]
+        if bad:
+            raise ValueError(f"sigma must be finite and > 0, got {bad[0]!r}")
+        sigma = np.asarray(s, np.float32)
+    elif num(s) and np.float32(s) > 0:
+        sigma = np.full(nv, s, np.float32)
+    else:
+        raise ValueError(f"sigma must be a finite number > 0 or a list of {nv}, got {s!r}")
+    forget = spec.get("forget", 1.0)
+    if not (num(forget) and 0 < np.float32(forget) <= 1):
+        raise ValueError(f"forget must be a finite number in (0, 1], got {forget!r}")
+    prune = spec.get("prune", 0.0)
+    if not (num(prune) and 0 <= np.float32(prune) and float(np.float32(prune)) < 1.0 / K):
+        raise ValueError(f"prune must be a number in [0, 1/K) = [0, {1.0 / K:g}), got {prune!r}")
+    return float(forget), float(prune), sigma
+
+
+def prior_setting(w, K: int):
+    """A belief given as K weights, each finite and >= 0 with a positive sum -> fp32 [K].  Raises ValueError
+    naming the bad value."""
+    if isinstance(w, torch.Tensor):
+        w = w.detach().cpu().tolist()
+    w = list(w) if isinstance(w, (list, tuple, np.ndarray)) else w
+    if not isinstance(w, list) or len(w) != K:
+        raise ValueError(f"a belief is a list of {K} weights (one per member), got {w!r}")
+    for x in w:
+        if isinstance(x, bool) or not isinstance(x, (int, float, np.floating, np.integer)) or \
+                not math.isfinite(x) or not np.float32(x) >= 0:
+            raise ValueError(f"every weight must be finite and >= 0, got {x!r}")
+    a = np.asarray(w, np.float32)
+    if not a.astype(np.float64).sum() > 0:
+        raise ValueError("the weights must have a positive sum")
+    return a
+
+
+def load_adapt(spec, K: int, nv: int):
+    """The ``adapt`` entry of an ``--ensemble`` file or an ``--instance-overrides`` mapping: the checked
+    adapt spec (``adapt_setting``), or None when ``spec`` has no ``adapt``.  Raises ValueError starting
+    with 'adapt: '."""
+    if not isinstance(spec, dict) or spec.get("adapt") is None:
+        return None
+    if K < 2:
+        raise ValueError(f"adapt: needs an ensemble of at least 2 members, got {K}")
+    try:
+        adapt_setting(spec["adapt"], K, nv)
+    except ValueError as e:
+        raise ValueError(f"adapt: {e}") from None
+    return dict(spec["adapt"])
+
+
+def load_prior(spec, K: int):
+    """The ``prior`` entry of an ``--ensemble`` file: K weights (``prior_setting``) or None.  Raises
+    ValueError starting with 'prior: '."""
+    if not isinstance(spec, dict) or spec.get("prior") is None:
+        return None
+    if K < 2:
+        raise ValueError(f"prior: needs an ensemble of at least 2 members, got {K}")
+    try:
+        return prior_setting(spec["prior"], K).tolist()
+    except ValueError as e:
+        raise ValueError(f"prior: {e}") from None
+
+
 def load_ensemble(spec, env):
     """The ``--ensemble`` file's mapping -> (K member ``System``s, the plant's ``sys`` mapping or None).
     ``members``: a list of K ``System.tree_replace`` mappings of ``env``'s model (``{}``: the nominal
     model); ``plant`` (optional): one such mapping for every instance's plant; ``risk`` (optional): the
-    risk spec of every instance, read by ``load_risk``.  Raises ValueError naming the entry that is
+    risk spec of every instance, read by ``load_risk``; ``adapt`` / ``prior`` (optional): adaptation to
+    the plant, read by ``load_adapt`` / ``load_prior``.  Raises ValueError naming the entry that is
     malformed."""
-    if not isinstance(spec, dict) or set(spec) - {"members", "plant", "risk"} or "members" not in spec:
-        raise ValueError("must map 'members' (a list of sys mappings) and optionally 'plant' (one sys mapping) and "
-                         f"'risk' (a risk spec), got {sorted(spec) if isinstance(spec, dict) else spec!r}")
+    if not isinstance(spec, dict) or set(spec) - {"members", "plant", "risk", "adapt", "prior"} or "members" not in spec:
+        raise ValueError("must map 'members' (a list of sys mappings) and optionally 'plant' (one sys mapping), "
+                         "'risk' (a risk spec), 'adapt' (an adapt spec) and 'prior' (K weights), got "
+                         f"{sorted(spec) if isinstance(spec, dict) else spec!r}")
     members, plant = spec["members"], spec.get("plant")
     kmax = _capi.DEFINES["DIAL_MAXENS"]
     if not isinstance(members, list) or not 1 <= len(members) <= kmax:
@@ -705,19 +860,20 @@ def load_ensemble(spec, env):
     return out, plant
 
 
-def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None):
+def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
     ``ensemble``: K planning models shared by every instance (``DeviceLoop(..., ensemble=...)``), scored
-    under ``risk`` (one risk spec or B of them, ``DeviceLoop(..., risk=...)``)."""
+    under ``risk`` (one risk spec or B of them, ``DeviceLoop(..., risk=...)``), adapting to the plant under
+    ``adapt`` from the belief ``prior`` (``DeviceLoop(..., adapt=..., prior=...)``)."""
     mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
         rng, rng_reset = drandom.split(drandom.PRNGKey(seed=dial_config.seed + b))
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
-    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk)
+    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -734,9 +890,19 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
             t0, tlast = time.time(), t
     rew = torch.stack(rews).mean(0).cpu().numpy()
     print("mean reward per instance = " + " ".join(f"{r:.2e}" for r in rew))
+    _print_belief(loop)
     timestamp = time.strftime("%Y%m%d-%H%M%S")
     for b in range(B):
         save_run(dial_config.output_dir, [r[b] for r in rollout], [x[b] for x in infos], timestamp=f"{timestamp}_inst{b}")
+
+
+def _print_belief(loop) -> None:
+    """The final belief over the members of each instance of an ensemble loop (K >= 2)."""
+    if loop.mbdpi.n_ensemble < 2:
+        return
+    w = loop.belief().cpu().numpy().reshape(loop.n_instances, -1)
+    for b, row in enumerate(w):
+        print(f"belief instance {b} = " + " ".join(f"{x:.3f}" for x in row))
 
 
 def main():
@@ -762,7 +928,10 @@ def main():
                              "every instance's simulated robot before its own --instance-overrides sys, and "
                              "optionally 'risk', how a sample's member rewards become its score: {aggregate: mean} "
                              "(default), {aggregate: worst} or {aggregate: cvar, alpha: A}; an --instance-overrides "
-                             "mapping may carry its own 'risk'")
+                             "mapping may carry its own 'risk'; optionally 'adapt', {sigma: S, forget: F, prune: P}: "
+                             "weight the members by how well they predict each env step's qvel (S: one scale or one "
+                             "per dof), from 'prior', K weights (default uniform); an --instance-overrides mapping "
+                             "may carry its own 'adapt'")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -787,7 +956,7 @@ def main():
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
     env = dial_envs.get_environment(dial_config.env_name, config=env_config)
     envs = None
-    members, plant, risk = None, None, None
+    members, plant, risk, adapt, prior = None, None, None, None, None
     if args.ensemble is not None:
         if args.eager:
             parser.error("--ensemble runs on the CUDA-graph loop; it excludes --eager")
@@ -795,6 +964,8 @@ def main():
             ens_spec = yaml.safe_load(open(args.ensemble))
             members, plant = load_ensemble(ens_spec, env)
             risk = load_risk(ens_spec, len(members))
+            adapt = load_adapt(ens_spec, len(members), env.sys.nv)
+            prior = load_prior(ens_spec, len(members))
         except (ValueError, yaml.YAMLError) as e:
             parser.error(f"--ensemble {args.ensemble}: {e}")
     if args.instance_overrides is not None:
@@ -804,13 +975,14 @@ def main():
         if not isinstance(overrides, list) or len(overrides) != args.instances:
             parser.error(f"--instance-overrides must hold a list of {args.instances} mappings (one per instance), "
                          f"got {len(overrides) if isinstance(overrides, list) else type(overrides).__name__}")
-        known = {f.name for f in dataclasses.fields(env_config_type)} | {"sys", "risk"}
+        known = {f.name for f in dataclasses.fields(env_config_type)} | {"sys", "risk", "adapt"}
         envs = []
         risks = [risk] * args.instances
+        adapts = [adapt] * args.instances
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys or risk, got "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk or adapt, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
             sys_ov = ov.pop("sys", None)
@@ -822,6 +994,14 @@ def main():
                 except ValueError as e:
                     parser.error(f"--instance-overrides entry {b}: {e}")
             ov.pop("risk", None)
+            if ov.get("adapt") is not None:
+                if members is None:
+                    parser.error(f"--instance-overrides entry {b}: adapt needs --ensemble (it weights the members)")
+                try:
+                    adapts[b] = load_adapt(ov, len(members), env.sys.nv)
+                except ValueError as e:
+                    parser.error(f"--instance-overrides entry {b}: {e}")
+            ov.pop("adapt", None)
             cfg_b = load_dataclass_from_dict(env_config_type, dict(config_dict, **ov), convert_list_to_array=True)
             envs.append(dial_envs.get_environment(dial_config.env_name, config=cfg_b))
             try:
@@ -845,8 +1025,10 @@ def main():
     if args.instances > 1:
         if args.instance_overrides is not None and any(r is not None for r in risks):
             risk = [r or {"aggregate": "mean"} for r in risks]
+        if args.instance_overrides is not None and any(a is not None for a in adapts):
+            adapt = adapts
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
-                      ensemble=members, risk=risk)
+                      ensemble=members, risk=risk, adapt=adapt, prior=prior)
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
@@ -857,7 +1039,8 @@ def main():
     rews, rollout, infos = [], [], []
     if mbdpi.world_size == 1 and not args.eager:
         # one CUDA graph per control step; the host launches it and logs
-        loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk)
+        loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk,
+                          adapt=adapt, prior=prior)
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):
@@ -886,6 +1069,8 @@ def main():
                 print(f"step {t}: rew={float(state.reward):.3e} freq={freq:.1f} Hz")
     rew = torch.stack([torch.as_tensor(r) for r in rews]).mean()
     print(f"mean reward = {float(rew):.2e}")
+    if mbdpi.world_size == 1 and not args.eager:
+        _print_belief(loop)
     save_run(dial_config.output_dir, rollout, infos)
 
 

@@ -31,6 +31,11 @@ inline float __fmaf_rn(float a, float b, float c) { return a * b + c; }
 inline float __fadd_rn(float a, float b) { return a + b; }
 inline float __fmul_rn(float a, float b) { return a * b; }
 inline float __fdiv_rn(float a, float b) { return a / b; }
+inline float __fsub_rn(float a, float b) { return a - b; }
+inline double __dadd_rn(double a, double b) { return a + b; }
+inline double __dsub_rn(double a, double b) { return a - b; }
+inline double __dmul_rn(double a, double b) { return a * b; }
+inline double __ddiv_rn(double a, double b) { return a / b; }
 #else
 #define HD __host__ __device__ __forceinline__
 #define DEV __device__ __forceinline__
@@ -209,15 +214,21 @@ struct alignas(16) EnsRisk {
   int32_t n_tail;   // CVaR: the n_tail lowest rewards count in full
   float frac;       // CVaR: the weight of the next-lowest reward s_{n_tail} (0: none)
   float denom;      // CVaR: the divisor (alpha K; n_tail when frac == 0)
+  // read by the belief-weighted branches only (ens_risk_reduce_weighted)
+  float alpha;      // CVaR: the fraction of the belief's mass averaged
+  int32_t worst;    // CVaR with alpha K <= 1 + 1e-6: the minimum
+  int32_t pad_[2];
 };
 
 // (K, mode, alpha) -> the setting, in fp64 (include/dial_b200.h: dial_plan_set_ensemble_risk)
 inline EnsRisk ens_risk_derive(int K, int mode, float alpha) {
   EnsRisk R;
   R.mode = mode; R.n_tail = K; R.frac = 0.f; R.denom = (float)K;
+  R.alpha = 1.f; R.worst = 0; R.pad_[0] = R.pad_[1] = 0;
   if (mode != DIAL_ENS_CVAR) return R;
+  R.alpha = alpha;
   const double t = (double)alpha * K;
-  if (t <= 1.0 + 1e-6) { R.n_tail = 1; R.denom = 1.f; }                       // the worst case: the minimum
+  if (t <= 1.0 + 1e-6) { R.n_tail = 1; R.denom = 1.f; R.worst = 1; }          // the worst case: the minimum
   else if (fabs(t - round(t)) <= 1e-6 * K) { R.n_tail = (int)round(t); R.denom = (float)R.n_tail; }
   else { R.n_tail = (int)floor(t); R.frac = (float)(t - R.n_tail); R.denom = (float)t; }
   return R;
@@ -262,6 +273,120 @@ DEV float ens_risk_reduce(const float* r, size_t stride, int K, const EnsRisk& R
   }
   if (R.frac > 0.f) acc = __fadd_rn(acc, __fmul_rn(R.frac, next));
   return nan ? NAN : __fdiv_rn(acc, R.denom);
+}
+
+// ---------------------------------------------------------------------------------
+// Adapting an ensemble plan to its plant (dial_plan_set_ensemble_adapt): instance b keeps a belief over
+// its K members, log-weights L [K] in fp64 and w_k = (float) exp(L_k), updated at every env step from how
+// well each member predicted the plant's post-step qvel, and scores samples by the belief-weighted risk
+// measure.  ens_belief_kernel and ensemble_reduce_kernel (dial_kernels.cu) run the functions below,
+// which the emulator build also runs on the CPU.  DEV, not HD, for the reason given at ens_risk_reduce:
+// every operation is a pinned round-to-nearest intrinsic, so that no multiply-add is fused on the GPU.
+// ---------------------------------------------------------------------------------
+#define DIAL_ENS_LOGLIK_CAP 1.0e4   // C: a member's log-likelihood of one step is at least -C
+
+struct alignas(16) EnsAdapt {
+  int32_t on;                 // 0: the instance keeps its belief and scores as without adaptation
+  float forget;               // in (0, 1]: L <- forget L + l at every update
+  float prune;                // in [0, 1/K): members with w < prune are left out of the score
+  int32_t pad_;
+  float sigma[DIAL_MAXV];     // the scale of each qvel residual (> 0)
+};
+
+// l_k = -min(e_k / 2, C) with e_k = sum_j ((vhat_j - v_j) / sigma_j)^2 in fp64 from the fp32 values, j
+// ascending.  A NaN or infinite e_k gives -C.  e_k = 0 gives -0.
+DEV double ens_member_loglik(const float* vhat, const float* v, const float* sigma, int nv) {
+  double e = 0.0;
+  for (int j = 0; j < nv; ++j) {
+    const double d = __ddiv_rn(__dsub_rn((double)vhat[j], (double)v[j]), (double)sigma[j]);
+    e = __dadd_rn(e, __dmul_rn(d, d));
+  }
+  const double h = __dmul_rn(e, 0.5);
+  return h <= DIAL_ENS_LOGLIK_CAP ? -h : -DIAL_ENS_LOGLIK_CAP;
+}
+
+// L_k <- forget L_k + l_k, then L_k <- L_k - (M + log sum_k exp(L_k - M)) with M = max_k L_k, the sum in
+// member order; w_k = (float) exp(L_k).  A member at L = -inf stays there with w = 0.
+DEV void ens_belief_update(double* L, float* w, const double* ell, int K, double forget) {
+  double M = -INFINITY;
+  for (int k = 0; k < K; ++k) {
+    L[k] = __dadd_rn(__dmul_rn(forget, L[k]), ell[k]);
+    M = L[k] > M ? L[k] : M;
+  }
+  double s = 0.0;
+  for (int k = 0; k < K; ++k) s = __dadd_rn(s, exp(__dsub_rn(L[k], M)));
+  const double lse = __dadd_rn(M, log(s));
+  for (int k = 0; k < K; ++k) {
+    L[k] = __dsub_rn(L[k], lse);
+    w[k] = (float)exp(L[k]);
+  }
+}
+
+// The score of one sample under the belief w [K]: member k's reward at r[k * stride].  Member k is kept
+// when w_k > 0 and w_k >= prune, or when w_k is the largest weight (so prune < 1/K never empties the
+// set); v_k = w_k for the kept members, 0 for the rest, whose rewards are never read into the
+// arithmetic.  W = sum_k v_k in member order.  With s_j, v_j the pairs sorted ascending by reward
+// (stable in member order, the same transposition sort as ens_risk_reduce):
+//   mean:  (sum_k v_k r_k) / W, the sum in member order;
+//   worst: the minimum reward of the kept members (the first in member order on ties);
+//   CVaR:  tau = alpha W; walking the sorted pairs with v_j > 0 while m < tau: t = min(v_j, tau - m),
+//          acc += t s_j, m += t; the score is acc / m: the mean of the worst alpha of the belief's mass.
+// Sums start at -0, the exact identity of fp32 addition.  Every operation is fp32 round-to-nearest.  A
+// NaN reward of a kept member makes the score NaN.  With uniform weights these equal ens_risk_reduce
+// only up to rounding.  Control flow depends on K, the setting and the belief only (uniform per CTA).
+DEV float ens_risk_reduce_weighted(const float* r, size_t stride, int K, const EnsRisk& R, const float* w, float prune) {
+  float wmax = 0.f;
+  for (int k = 0; k < K; ++k) wmax = w[k] > wmax ? w[k] : wmax;
+  float s[DIAL_MAXENS], v[DIAL_MAXENS];
+  float W = -0.f;
+  bool nan = false;
+#pragma unroll
+  for (int k = 0; k < DIAL_MAXENS; ++k) {
+    const float wk = k < K ? w[k] : 0.f;
+    const bool kept = wk > 0.f && (wk >= prune || wk == wmax);
+    s[k] = kept ? r[(size_t)k * stride] : INFINITY;
+    v[k] = kept ? wk : 0.f;
+    nan = nan || isnan(s[k]);
+    if (kept) W = __fadd_rn(W, wk);
+  }
+  if (R.mode == DIAL_ENS_MEAN) {
+    float acc = -0.f;
+#pragma unroll
+    for (int k = 0; k < DIAL_MAXENS; ++k)
+      if (v[k] > 0.f) acc = __fadd_rn(acc, __fmul_rn(v[k], s[k]));
+    return nan ? NAN : __fdiv_rn(acc, W);
+  }
+  if (R.worst) {
+    float m = INFINITY;
+#pragma unroll
+    for (int k = 0; k < DIAL_MAXENS; ++k)
+      if (v[k] > 0.f && s[k] < m) m = s[k];
+    return nan ? NAN : m;
+  }
+#pragma unroll
+  for (int pass = 0; pass < DIAL_MAXENS; ++pass) {
+    if (pass >= K) break;
+#pragma unroll
+    for (int j = pass & 1; j + 1 < DIAL_MAXENS; j += 2) {
+      const float a = s[j], b = s[j + 1], va = v[j], vb = v[j + 1];
+      const bool swap = a > b;
+      s[j] = swap ? b : a;
+      s[j + 1] = swap ? a : b;
+      v[j] = swap ? vb : va;
+      v[j + 1] = swap ? va : vb;
+    }
+  }
+  const float tau = __fmul_rn(R.alpha, W);
+  float acc = -0.f, m = 0.f;
+#pragma unroll
+  for (int j = 0; j < DIAL_MAXENS; ++j) {
+    if (v[j] > 0.f && m < tau) {
+      const float t = fminf(v[j], __fsub_rn(tau, m));
+      acc = __fadd_rn(acc, __fmul_rn(t, s[j]));
+      m = __fadd_rn(m, t);
+    }
+  }
+  return nan ? NAN : __fdiv_rn(acc, m);
 }
 
 // ---------------------------------------------------------------------------------

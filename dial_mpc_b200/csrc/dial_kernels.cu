@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <float.h>
 #include <string>
 #include <vector>
 #include <new>
@@ -555,13 +556,44 @@ __global__ void __launch_bounds__(128, 8) trajbar_final_kernel(const TrajArgs T)
 // Ensemble plans (n_ens = K >= 2): rews[b][i] = instance b's risk measure risk[b] of the member rewards
 // r[b][0..K-1][i] (ens_risk_reduce; the mean: (((r0 + r1) + ...) + r_{K-1}) / K), fp32 with
 // round-to-nearest (the library is built with -use_fast_math, whose `/` is approximate).  One thread per
-// (instance, sample); grid.y is the instance, so a CTA reads one setting and takes one branch.
+// (instance, sample); grid.y is the instance, so a CTA reads one setting and takes one branch.  An
+// instance adapting to its plant (adapt[b].on) takes the belief-weighted branch of its measure
+// (ens_risk_reduce_weighted) over its belief w [B][K].
 __global__ void __launch_bounds__(256) ensemble_reduce_kernel(const float* __restrict__ r, const EnsRisk* __restrict__ risk,
+                                                              const EnsAdapt* __restrict__ adapt, const float* __restrict__ belief,
                                                               int K, int n1, float* __restrict__ rews) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
   if (i >= n1) return;
   const EnsRisk R = risk[b];
-  rews[(size_t)b * n1 + i] = ens_risk_reduce(r + (size_t)b * K * n1 + i, (size_t)n1, K, R);
+  const float* rb = r + (size_t)b * K * n1 + i;
+  rews[(size_t)b * n1 + i] = adapt[b].on ? ens_risk_reduce_weighted(rb, (size_t)n1, K, R, belief + (size_t)b * K, adapt[b].prune)
+                                         : ens_risk_reduce(rb, (size_t)n1, K, R);
+}
+
+// Ensemble adaptation, before the plant's env step: us [B K][nu] row b K + k = Y[b][0], the action of
+// instance b, so that the member-prediction launch reads its action at the rollout kernel's row stride.
+__global__ void __launch_bounds__(128) ens_gather_kernel(const float* __restrict__ Y, int K, int n1, int nu,
+                                                         float* __restrict__ us) {
+  const int b = blockIdx.x;
+  for (int i = threadIdx.x; i < K * nu; i += blockDim.x) us[(size_t)b * K * nu + i] = Y[(size_t)b * n1 * nu + i % nu];
+}
+
+// Ensemble adaptation, after the plant's env step: one warp per instance.  Lane k < K scores member k's
+// predicted qvel vhat [B K][nv] against the observed qvel [B][nv] (ens_member_loglik); lane 0 then
+// updates the belief L / w [B][K] in member order (ens_belief_update).  ell [B][K] keeps the last l.
+// Instances that do not adapt are left as they are.
+__global__ void __launch_bounds__(32) ens_belief_kernel(const float* __restrict__ vhat, const float* __restrict__ qvel,
+                                                        const EnsAdapt* __restrict__ adapt, int K, int nv,
+                                                        double* __restrict__ L, float* __restrict__ w, float* __restrict__ ell) {
+  const int b = blockIdx.x, lane = threadIdx.x;
+  if (!adapt[b].on) return;
+  __shared__ double l[DIAL_MAXENS];
+  if (lane < K) {
+    l[lane] = ens_member_loglik(vhat + ((size_t)b * K + lane) * nv, qvel + (size_t)b * nv, adapt[b].sigma, nv);
+    ell[(size_t)b * K + lane] = (float)l[lane];
+  }
+  __syncwarp();
+  if (lane == 0) ens_belief_update(L + (size_t)b * K, w + (size_t)b * K, l, K, (double)adapt[b].forget);
 }
 
 // ---------------------------------------------------------------------------------
@@ -620,6 +652,22 @@ struct dial_plan {
   EnsRisk* dRisk = nullptr;
   EnsRisk* hRisk = nullptr;
   std::vector<cudaEvent_t> risk_ev;
+  // adaptation to the plant (dial_plan_set_ensemble_adapt / _belief, n_ens >= 2): the settings [n_inst]
+  // with their pinned staging and copy events, as for the risk measure; the belief L [n_inst, n_ens] in
+  // fp64, w and the last update's l in fp32, with pinned staging for L and w and one copy event per
+  // instance.  pred_us [n_inst n_ens, nu] / pred_qd [n_inst n_ens, nv] (the members' predictions) are
+  // allocated by the first call that turns adaptation on; until then the graphs hold no adaptation launch.
+  EnsAdapt* dAdapt = nullptr;
+  EnsAdapt* hAdapt = nullptr;
+  std::vector<cudaEvent_t> adapt_ev;
+  double* dL = nullptr;
+  double* hL = nullptr;
+  float* dW = nullptr;
+  float* hW = nullptr;
+  float* dEll = nullptr;
+  std::vector<cudaEvent_t> belief_ev;
+  float* pred_us = nullptr;
+  float* pred_qd = nullptr;
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -837,6 +885,23 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     for (size_t b = 0; b < B; ++b) p->hRisk[b] = ens_risk_derive(p->n_ens, DIAL_ENS_MEAN, 1.f);
     if ((e = cudaMemcpy(p->dRisk, p->hRisk, B * sizeof(EnsRisk), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(risk)");
     p->risk_ev.assign(B, nullptr);
+    // no instance adapts; every belief starts uniform
+    const size_t BK = B * p->n_ens;
+    if ((e = cudaMallocHost(&p->hAdapt, B * sizeof(EnsAdapt))) != cudaSuccess) return bad(e, "cudaMallocHost(adapt)");
+    if ((e = cudaMalloc(&p->dAdapt, B * sizeof(EnsAdapt))) != cudaSuccess) return bad(e, "cudaMalloc(adapt)");
+    memset(p->hAdapt, 0, B * sizeof(EnsAdapt));
+    if ((e = cudaMemcpy(p->dAdapt, p->hAdapt, B * sizeof(EnsAdapt), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(adapt)");
+    p->adapt_ev.assign(B, nullptr);
+    if ((e = cudaMallocHost(&p->hL, BK * sizeof(double))) != cudaSuccess) return bad(e, "cudaMallocHost(belief)");
+    if ((e = cudaMallocHost(&p->hW, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMallocHost(belief)");
+    if ((e = cudaMalloc(&p->dL, BK * sizeof(double))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
+    if ((e = cudaMalloc(&p->dW, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
+    if ((e = cudaMalloc(&p->dEll, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
+    for (size_t i = 0; i < BK; ++i) { p->hL[i] = log(1.0 / p->n_ens); p->hW[i] = (float)exp(p->hL[i]); }
+    if ((e = cudaMemcpy(p->dL, p->hL, BK * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(belief)");
+    if ((e = cudaMemcpy(p->dW, p->hW, BK * sizeof(float), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(belief)");
+    if ((e = cudaMemset(p->dEll, 0, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMemset(belief)");
+    p->belief_ev.assign(B, nullptr);
   }
   if ((e = cudaMalloc(&p->weights, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
   if ((e = cudaMalloc(&p->weights2, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
@@ -883,6 +948,11 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   cudaFree(p->dMembers); cudaFreeHost(p->hMembers); cudaFree(p->ens_rews);
   for (cudaEvent_t e : p->risk_ev) if (e) cudaEventDestroy(e);
   cudaFree(p->dRisk); cudaFreeHost(p->hRisk);
+  for (cudaEvent_t e : p->adapt_ev) if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : p->belief_ev) if (e) cudaEventDestroy(e);
+  cudaFree(p->dAdapt); cudaFreeHost(p->hAdapt);
+  cudaFree(p->dL); cudaFree(p->dW); cudaFree(p->dEll); cudaFreeHost(p->hL); cudaFreeHost(p->hW);
+  cudaFree(p->pred_us); cudaFree(p->pred_qd);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   cudaFree(p->weights2);
@@ -1037,6 +1107,105 @@ extern "C" int dial_plan_member_rewards(dial_plan* p, float* out, void* stream) 
   const size_t n = (size_t)p->n_inst * p->n_ens * ((size_t)p->hP.c.Nsample + 1);
   const float* src = p->n_ens > 1 ? p->ens_rews : p->mpc.rews;   // n_ens = 1: the rollout writes rews itself
   CUDA_OK(cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+
+static std::string fmt_g(double x) {
+  char buf[64];
+  snprintf(buf, sizeof(buf), "%g", x);
+  return buf;
+}
+
+// the checks every adaptation call shares: a plan with n_ens >= 2 and b in range
+static int adapt_target(const dial_plan* p, const char* fn, int b) {
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (p->n_ens < 2) return fail(std::string(fn) + ": the plan needs an ensemble of n_ens >= 2 members, it has " + std::to_string(p->n_ens));
+  if (b < 0 || b >= p->n_inst) return fail(std::string(fn) + ": instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
+  return 0;
+}
+
+extern "C" int dial_plan_set_ensemble_adapt(dial_plan* p, int b, int on, float forget, float prune, const float* sigma, void* stream) {
+  static const char* fn = "dial_plan_set_ensemble_adapt";
+  if (int rc = adapt_target(p, fn, b)) return rc;
+  if (on != 0 && on != 1) return fail(std::string(fn) + ": on must be 0 or 1, got " + std::to_string(on));
+  const int K = p->n_ens, nv = p->hM.m.nv;
+  if (on) {   // also rejects NaN and infinities
+    if (!(forget > 0.f && forget <= 1.f)) return fail(std::string(fn) + ": forget must be in (0, 1], got " + fmt_g(forget));
+    if (!(prune >= 0.f && (double)prune < 1.0 / K))
+      return fail(std::string(fn) + ": prune must be in [0, 1/K) = [0, " + fmt_g(1.0 / K) + "), got " + fmt_g(prune));
+    if (!sigma) return fail(std::string(fn) + ": null sigma");
+    for (int j = 0; j < nv; ++j)
+      if (!(sigma[j] > 0.f && sigma[j] <= FLT_MAX))
+        return fail(std::string(fn) + ": sigma[" + std::to_string(j) + "] must be finite and > 0, got " + fmt_g(sigma[j]));
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (on && !p->pred_qd) {
+    // first instance to adapt: the prediction workspaces; the graphs captured so far hold no adaptation
+    // launches and are recaptured on their next use
+    const size_t rows = (size_t)p->n_inst * K;
+    if ((e = cudaMalloc(&p->pred_us, rows * p->hM.m.nu * sizeof(float))) == cudaSuccess)
+      e = cudaMalloc(&p->pred_qd, rows * nv * sizeof(float));
+    if (e != cudaSuccess) {
+      cudaFree(p->pred_us); cudaFree(p->pred_qd); p->pred_us = p->pred_qd = nullptr;
+      return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+    }
+    for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+    p->mpc_graphs.clear();
+  }
+  // stream-ordered copy out of the slot's pinned staging, rewritten only after its previous copy has run;
+  // the captured graphs hold the array's pointer and read the new setting at their next replay
+  cudaEvent_t& ev = p->adapt_ev[b];
+  e = ev ? cudaEventSynchronize(ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) {
+    EnsAdapt& a = p->hAdapt[b];
+    a.on = on;
+    if (on) {
+      a.forget = forget; a.prune = prune;
+      for (int j = 0; j < DIAL_MAXV; ++j) a.sigma[j] = j < nv ? sigma[j] : 1.f;
+    }
+    e = cudaMemcpyAsync(p->dAdapt + b, p->hAdapt + b, sizeof(EnsAdapt), cudaMemcpyHostToDevice, st);
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int dial_plan_set_ensemble_belief(dial_plan* p, int b, const float* w, void* stream) {
+  static const char* fn = "dial_plan_set_ensemble_belief";
+  if (int rc = adapt_target(p, fn, b)) return rc;
+  if (!w) return fail(std::string(fn) + ": null w");
+  const int K = p->n_ens;
+  double sum = 0.0;
+  for (int k = 0; k < K; ++k) {
+    if (!(w[k] >= 0.f && w[k] <= FLT_MAX)) return fail(std::string(fn) + ": w[" + std::to_string(k) + "] must be finite and >= 0, got " + fmt_g(w[k]));
+    sum += (double)w[k];
+  }
+  if (!(sum > 0.0)) return fail(std::string(fn) + ": the weights must have a positive sum");
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaEvent_t& ev = p->belief_ev[b];
+  cudaError_t e = ev ? cudaEventSynchronize(ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) {
+    double* L = p->hL + (size_t)b * K;
+    float* W = p->hW + (size_t)b * K;
+    for (int k = 0; k < K; ++k) {
+      L[k] = w[k] > 0.f ? log((double)w[k] / sum) : -INFINITY;
+      W[k] = (float)exp(L[k]);
+    }
+    e = cudaMemcpyAsync(p->dL + (size_t)b * K, L, K * sizeof(double), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(p->dW + (size_t)b * K, W, K * sizeof(float), cudaMemcpyHostToDevice, st);
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int dial_plan_ensemble_belief(dial_plan* p, float* w, float* loglik, void* stream) {
+  if (int rc = adapt_target(p, "dial_plan_ensemble_belief", 0)) return rc;
+  const size_t n = (size_t)p->n_inst * p->n_ens * sizeof(float);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (w) CUDA_OK(cudaMemcpyAsync(w, p->dW, n, cudaMemcpyDeviceToDevice, st));
+  if (loglik) CUDA_OK(cudaMemcpyAsync(loglik, p->dEll, n, cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -1300,6 +1469,22 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
   const bool batched = ni > 1;
   float* Y[2] = {B.Y, p->mpc_Y1};
   int cur = 0;
+  // ensemble adaptation, once some instance has turned it on: before the plant's env step, member (b, k)
+  // makes the same env step on its own model, from instance b's state, counters and task with the action
+  // Y[b][0] (row b K + k, its CTA staging member slot b K + k); only the post-step qvel is kept
+  const bool adapt = env_step == 1 && p->pred_qd;
+  if (adapt) {
+    ens_gather_kernel<<<ni, 128, 0, st>>>(Y[cur], K, n1, nu, p->pred_us);
+    p->launches++;
+    CUDA_OK(cudaGetLastError());
+    RolloutArgs A; memset(&A, 0, sizeof(A));
+    A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart; A.counters_in = B.counters;
+    A.nrows = ni * K; A.H = 1; A.mode = 0; A.us = p->pred_us;
+    A.rows_per_inst = K; A.rows_per_model = 1; A.models = p->dMembers;
+    if (B.tasks) { A.tasks = B.tasks; A.task_rows = K; }
+    A.qd = p->pred_qd;
+    CUDA_OK(launch_rollout(p, A, 1, st));
+  }
   if (env_step == 1) {
     // state = step_env(state, Y0[0])  (dial_core.py:245): in place, counters advanced by the kernel;
     // batched: row b is instance b, its action Y[b][0]
@@ -1312,6 +1497,11 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     A.models = p->dModels;
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
     CUDA_OK(launch_rollout(p, A, 1, st));
+  }
+  if (adapt) {   // each adapting instance's belief from its members' predictions and the observed qvel
+    ens_belief_kernel<<<ni, 32, 0, st>>>(p->pred_qd, B.qvel, p->dAdapt, K, p->hM.m.nv, p->dL, p->dW, p->dEll);
+    p->launches++;
+    CUDA_OK(cudaGetLastError());
   }
   if (env_step == 1 || env_step == 2) {
     // Y0 = shift(Y0)  (dial_core.py:252)
@@ -1355,7 +1545,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     CUDA_OK(launch_rollout_any(p, A, st));
     if (K > 1) {   // each sample's score under its instance's risk measure (K = 1: the reward itself)
       const dim3 grid((c.Nsample + 1 + 255) / 256, ni);
-      ensemble_reduce_kernel<<<grid, 256, 0, st>>>(p->ens_rews, p->dRisk, K, c.Nsample + 1, B.rews);
+      ensemble_reduce_kernel<<<grid, 256, 0, st>>>(p->ens_rews, p->dRisk, p->dAdapt, p->dW, K, c.Nsample + 1, B.rews);
       p->launches++;
       CUDA_OK(cudaGetLastError());
     }

@@ -112,6 +112,35 @@ class Plan:
         self._check(self.lib.dial_plan_member_rewards(self.handle, _ptr(out), _stream()))
         return out
 
+    def set_ensemble_adapt(self, b: int, on: bool, forget: float = 1.0, prune: float = 0.0, sigma=None) -> None:
+        """Instance b adapts its belief over its members to the plant at every env step (``on``), with
+        ``forget`` in (0, 1], ``prune`` in [0, 1/K) and ``sigma`` [nv] > 0; or stops (the belief is kept).
+        A stream-ordered copy on the current stream; the first call that turns adaptation on in a plan
+        makes the next steps capture their graphs again (``dial_plan_set_ensemble_adapt``)."""
+        s = None
+        if sigma is not None:
+            a = np.ascontiguousarray(sigma, dtype=np.float32).ravel()
+            assert a.size == self.nv, f"sigma needs {self.nv} values, got {a.size}"
+            s = (C.c_float * len(a))(*a.tolist())
+        self._check(self.lib.dial_plan_set_ensemble_adapt(self.handle, int(b), int(bool(on)), float(forget),
+                                                          float(prune), s, _stream()))
+
+    def set_ensemble_belief(self, b: int, w) -> None:
+        """Instance b's belief from K weights >= 0 with a positive sum, normalised in fp64 on the host
+        (``dial_plan_set_ensemble_belief``)."""
+        a = np.ascontiguousarray(w, dtype=np.float32).ravel()
+        assert self.desc.n_ens < 2 or a.size == self.desc.n_ens, f"need {self.desc.n_ens} weights, got {a.size}"
+        self._check(self.lib.dial_plan_set_ensemble_belief(self.handle, int(b), (C.c_float * a.size)(*a.tolist()),
+                                                           _stream()))
+
+    def ensemble_belief(self, w: Optional[torch.Tensor], loglik: Optional[torch.Tensor] = None) -> None:
+        """Copy the belief [n_inst * n_ens] and the last update's log-likelihoods into ``w`` / ``loglik``
+        (either may be None; ``dial_plan_ensemble_belief``)."""
+        n = max(self.desc.n_inst, 1) * self.desc.n_ens
+        for t in (w, loglik):
+            assert t is None or t.numel() == n, f"need {n} elements, got {tuple(t.shape)}"
+        self._check(self.lib.dial_plan_ensemble_belief(self.handle, _ptr(w), _ptr(loglik), _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

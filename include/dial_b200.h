@@ -407,7 +407,7 @@ int dial_plan_set_ensemble_model(dial_plan* plan, int b, int k, const dial_model
  * CVaR with alpha = 1 is the mean up to rounding only (another summation order); DIAL_ENS_MEAN alone
  * reproduces a plan without the call.  A NaN member reward makes the score NaN; infinities go through
  * the arithmetic.  A non-finite score gets weight 0 in the update, as with the mean.
- * The copy of the 16-byte setting is stream-ordered on `stream`, out of plan-owned pinned staging that
+ * The copy of the 32-byte setting is stream-ordered on `stream`, out of plan-owned pinned staging that
  * dial_plan_create allocates with the setting array (n_ens >= 2; every instance starts at the mean), so
  * the call may be issued between dial_mpc_step calls.  The captured graphs read the array, so they are
  * kept: the setting takes effect at their next replay.  On a plan with n_ens = 1 any valid setting is
@@ -420,6 +420,50 @@ int dial_plan_set_ensemble_risk(dial_plan* plan, int b, int mode, float alpha, v
  * (n_ens >= 2), or the bound rews (n_ens = 1).  A stream-ordered copy on `stream`.  Fails on a plan with
  * n_ens == 0 and before dial_mpc_bind. */
 int dial_plan_member_rewards(dial_plan* plan, float* out, void* stream);
+
+/* Adapting an ensemble plan (n_ens = K >= 2) to its plant.  Instance b keeps a belief over its K members:
+ * log-weights L [K] in fp64 and w_k = (float) exp(L_k).  Every instance starts uniform.  While instance b
+ * adapts, each dial_mpc_step with env_step == 1 first lets every member (b, k) make the plant's env step on
+ * its own model, from the instance's pre-step state and counters with the action Y[b][0], and keeps its
+ * post-step qvel vhat_k.  After the plant's step, with v its observed qvel, in fp64:
+ *   e_k = sum_j ((vhat_kj - v_j) / sigma_j)^2  (j ascending, from the fp32 values)
+ *   l_k = -min(e_k / 2, C), C = 1e4            (a NaN or infinite e_k gives -C: a NaN plant state
+ *                                               shifts every member equally)
+ *   L_k <- forget L_k + l_k;  L_k <- L_k - (M + log sum_k exp(L_k - M)), M = max_k L_k (member order).
+ * With env_step 0 or 2, and on instances that do not adapt, the belief stays as it is.
+ * An adapting instance scores each sample by its risk measure weighted by the belief.  Member k is kept
+ * when w_k > 0 and w_k >= prune, or w_k is the largest weight; v_k = w_k for kept members, else 0, and
+ * W = sum_k v_k in member order.  All fp32 round-to-nearest:
+ *   DIAL_ENS_MEAN: (sum_k v_k r_k) / W, member order;
+ *   CVaR, alpha K <= 1 + 1e-6 (the worst case): the minimum reward of the kept members;
+ *   CVaR otherwise: tau = alpha W; over the (r, v) pairs sorted ascending by r (stable in member order),
+ *     skipping v = 0, while m < tau: t = min(v_j, tau - m), acc += t r_j, m += t; the score is acc / m.
+ * Sums start at -0.  A NaN reward of a kept member makes the score NaN; a pruned member's reward is never
+ * read.  With uniform weights these equal the unweighted measures only up to rounding.  The GPU flushes
+ * subnormal fp32 values to zero, so a weight below FLT_MIN counts as 0 there.
+ * Each prediction is one more rollout launch over n_inst K rows and a small gather launch before the
+ * plant's env step, and one belief launch after it: only in plans where some instance turned
+ * adaptation on; a plan that never does keeps its launches. */
+
+/* Instance b adapts (on = 1) or stops adapting (on = 0; the other arguments are then ignored and the
+ * belief is kept).  forget in (0, 1], prune in [0, 1/K), sigma [host][nv] finite and > 0: the scale of
+ * each qvel residual.  The 128-byte setting is copied stream-ordered on `stream` out of plan-owned pinned
+ * staging, as for dial_plan_set_ensemble_risk.  The first call with on = 1 on a plan allocates the
+ * prediction workspaces and drops the captured graphs; later calls keep them, and their setting takes
+ * effect at the next replay.  Fails on a plan with n_ens < 2, for b out of range and for a bad argument,
+ * which the error names. */
+int dial_plan_set_ensemble_adapt(dial_plan* plan, int b, int on, float forget, float prune, const float* sigma,
+                                 void* stream);
+
+/* Instance b's belief from w [host][K]: each finite and >= 0, with a positive sum.  In fp64 the host
+ * sets L_k = log(w_k / sum w) (-inf for w_k = 0: that member stays excluded) and w_k = (float) exp(L_k);
+ * a stream-ordered copy on `stream`, as above.  The graphs are kept.  Lets an outside estimator drive the
+ * belief where the plan does not step the plant (env_step 0). */
+int dial_plan_set_ensemble_belief(dial_plan* plan, int b, const float* w, void* stream);
+
+/* The current belief w [dev][n_inst, K] and the l [dev][n_inst, K] of each instance's last update (0
+ * before the first), each nullable; stream-ordered copies on `stream`.  Fails on a plan with n_ens < 2. */
+int dial_plan_ensemble_belief(dial_plan* plan, float* w, float* loglik, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops

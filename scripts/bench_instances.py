@@ -49,6 +49,15 @@ def risk_spec(tok: str) -> dict:
         raise ValueError(f"alpha must be a number, got {a!r}") from None
 
 
+def adapt_spec(tok: str) -> dict:
+    """An --adapt token (SIGMA or SIGMA:FORGET) -> the adapt spec of DeviceLoop(..., adapt=...)."""
+    s, colon, f = tok.partition(":")
+    try:
+        return dict({"sigma": float(s)}, **({"forget": float(f)} if colon else {}))
+    except ValueError:
+        raise ValueError(f"SIGMA[:FORGET] must be numbers, got {tok!r}") from None
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", type=int, default=0)
@@ -63,6 +72,11 @@ def main():
                     help="plan every instance against K member models: K distinct base masses and foot frictions")
     ap.add_argument("--risk", default="mean", metavar="MEASURE",
                     help="with --ensemble: the risk measure of every instance, mean, worst or cvar:ALPHA")
+    ap.add_argument("--adapt", default=None, metavar="SIGMA[:FORGET]",
+                    help="with --ensemble K >= 2: every instance adapts its belief over the members to its plant")
+    ap.add_argument("--env-step", type=int, default=2, choices=(1, 2),
+                    help="the timed steps' env_step: 2 (shift + plan, the default) or 1 (env step + shift + plan; "
+                         "--adapt runs its predictions and belief update in env steps only)")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
@@ -70,6 +84,8 @@ def main():
         ap.error("--instances and --steps must be at least 1")
     if args.risk != "mean" and not args.ensemble:
         ap.error("--risk needs --ensemble K")
+    if args.adapt is not None and args.ensemble < 2:
+        ap.error("--adapt needs --ensemble K with K >= 2")
     if args.profile_kernels:
         os.environ["DIAL_NO_GRAPH"] = "1"     # kernels of a replayed graph are not listed one by one
     import numpy as np
@@ -110,29 +126,44 @@ def main():
         risk = risk_spec(args.risk) if args.ensemble else None
     except ValueError as e:
         ap.error(f"--risk {args.risk}: {e}")
+    try:
+        adapt = adapt_spec(args.adapt) if args.adapt is not None else None
+    except ValueError as e:
+        ap.error(f"--adapt {args.adapt}: {e}")
     if B == 1:
-        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk)
+        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
-                          ensemble=members, risk=risk)
+                          ensemble=members, risk=risk, adapt=adapt)
+    es = args.env_step
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=mb.device)
     for _ in range(max(args.warmup, 3)):
-        loop.step(cfg.Ndiffuse, env_step=2)
+        loop.step(cfg.Ndiffuse, env_step=es)
     torch.cuda.synchronize()
     if args.profile_kernels:
         from torch.profiler import ProfilerActivity, profile
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(args.steps):
-                loop.step(cfg.Ndiffuse, env_step=2)
+                loop.step(cfg.Ndiffuse, env_step=es)
             torch.cuda.synchronize()
-        acc = {}
+        acc, rollouts = {}, []
         for ev in prof.events():
-            for key in ("rollout_kernel", "update_kernel", "ensemble_reduce_kernel", "trajbar"):
-                if key in ev.name and ev.device_type.name == "CUDA":
+            if ev.device_type.name != "CUDA":
+                continue
+            if "rollout_kernel" in ev.name:
+                rollouts.append((ev.time_range.start, ev.time_range.elapsed_us()))
+            for key in ("update_kernel", "ensemble_reduce_kernel", "trajbar", "ens_gather_kernel", "ens_belief_kernel"):
+                if key in ev.name:
                     n, tot = acc.get(key, (0, 0.0))
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
+        # the rollout launches of one step in order: [member prediction, env step (env_step 1)], the planner's
+        per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) + ["plan"] * cfg.Ndiffuse
+        for i, (_, us) in enumerate(sorted(rollouts)):
+            key = f"rollout_kernel ({per_step[i % len(per_step)]})"
+            n, tot = acc.get(key, (0, 0.0))
+            acc[key] = (n + 1, tot + us)
         print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
-                              risk=args.risk, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              risk=args.risk, adapt=args.adapt, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
                               launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
         return
     evs = []
@@ -140,14 +171,14 @@ def main():
         flush.zero_()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        loop.step(cfg.Ndiffuse, env_step=2)
+        loop.step(cfg.Ndiffuse, env_step=es)
         e1.record()
         evs.append((e0, e1))
     torch.cuda.synchronize()
     t = sum(a.elapsed_time(e) for a, e in evs) / 1e3 / args.steps
     rows = B * max(args.ensemble, 1) * (cfg.Nsample + 1)
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
-                          distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, rows_per_rollout=rows,
+                          distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
                           value=B * cfg.Ndiffuse * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))

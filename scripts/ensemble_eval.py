@@ -9,8 +9,11 @@ experiment).  Planner B plans on a K-member ensemble spanning the same range (me
 friction 1 - 0.6 k / (K-1)) and weights every sample by a risk measure of its member rewards; --risk lists
 the measures (mean, worst, cvar:ALPHA; default mean), one ensemble planner each.  Every planner runs the
 reference's closed loop (env step, shift, Ndiffuse iterations) for --steps control steps in one control-step
-graph per step, B instances at a time.  Prints a table per plant: mean env-step reward, minimum base height
-and whether the robot fell (base height below --fall-height at any step), and one JSON line."""
+graph per step, B instances at a time.  --adapt SIGMA[:FORGET] adds, for each measure, an ensemble planner
+that adapts its belief over the members to its plant at every env step (DeviceLoop(..., adapt=...)), and
+reports the final belief on the member nearest the plant.  Prints a table per plant: mean env-step reward,
+minimum base height and whether the robot fell (base height below --fall-height at any step), and one JSON
+line."""
 import argparse
 import copy
 import json
@@ -19,7 +22,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from scripts.bench_instances import gpu_info, risk_spec  # noqa: E402
+from scripts.bench_instances import adapt_spec, gpu_info, risk_spec  # noqa: E402
 
 
 def main():
@@ -30,6 +33,8 @@ def main():
     ap.add_argument("--fall-height", type=float, default=0.15)
     ap.add_argument("--risk", nargs="+", default=["mean"], metavar="MEASURE",
                     help="one ensemble planner per measure: mean, worst or cvar:ALPHA (default: mean)")
+    ap.add_argument("--adapt", default=None, metavar="SIGMA[:FORGET]",
+                    help="also run, per measure, an ensemble planner adapting its belief to the plant")
     args = ap.parse_args()
     if args.plants < 2 or args.ensemble < 2 or args.steps < 1:
         ap.error("--plants and --ensemble must be at least 2, --steps at least 1")
@@ -42,6 +47,12 @@ def main():
         except ValueError as e:
             ap.error(f"--risk {tok}: {e}")
         risks.append((tok, spec))
+    adapt = None
+    if args.adapt is not None:
+        try:
+            adapt = adapt_spec(args.adapt)
+        except ValueError as e:
+            ap.error(f"--adapt {args.adapt}: {e}")
     import numpy as np
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
@@ -68,13 +79,17 @@ def main():
     members = [model(k / (K - 1)).sys for k in range(K)]
     rng, rng_reset = drandom.split(drandom.PRNGKey(cfg.seed))
     results = {}
-    planners = [("nominal", [env.sys], None)]
-    planners += [(f"ensemble{K}" if tok == "mean" else f"ensemble{K}-{tok}", members, spec) for tok, spec in risks]
-    for name, ens, risk in planners:
+    # the member nearest plant b: payload and friction both move with f, so the nearest f
+    nearest = [int(round(b / (B - 1) * (K - 1))) for b in range(B)]
+    planners = [("nominal", [env.sys], None, None)]
+    planners += [(f"ensemble{K}" if tok == "mean" else f"ensemble{K}-{tok}", members, spec, None) for tok, spec in risks]
+    if adapt is not None:
+        planners += [(f"adapt{K}" if tok == "mean" else f"adapt{K}-{tok}", members, spec, adapt) for tok, spec in risks]
+    for name, ens, risk, ad in planners:
         mb = MBDPI(cfg, env, n_instances=B, n_ensemble=len(ens))
         states = [p.reset(rng_reset) for p in plants]
         rngs = np.stack([drandom.split(drandom.PRNGKey(cfg.seed + b))[1] for b in range(B)])
-        loop = DeviceLoop(mb, states, rngs, envs=plants, ensemble=ens, risk=risk)
+        loop = DeviceLoop(mb, states, rngs, envs=plants, ensemble=ens, risk=risk, adapt=ad)
         rew, height = [], []
         for t in range(args.steps):
             loop.step(cfg.Ndiffuse_init if t == 0 else cfg.Ndiffuse)
@@ -83,6 +98,9 @@ def main():
         rew, height = torch.stack(rew).cpu().numpy(), torch.stack(height).cpu().numpy()
         results[name] = dict(mean_reward=rew.mean(0).tolist(), min_height=height.min(0).tolist(),
                              fell=(height < args.fall_height).any(0).tolist())
+        if ad is not None:
+            w = loop.belief().cpu().numpy()
+            results[name]["belief_nearest"] = [float(w[b, nearest[b]]) for b in range(B)]
     print(f"Go2 trot, configs[0] size (N={cfg.Nsample}, H={cfg.Hsample}, Ndiffuse={cfg.Ndiffuse}), {args.steps} steps")
     names = list(results)
     print("| payload kg | friction | " + " | ".join(f"{n} reward | {n} min height | {n} fell" for n in names) + " |")
@@ -94,10 +112,19 @@ def main():
             r = results[n]
             cells += [f"{r['mean_reward'][b]:.3f}", f"{r['min_height'][b]:.3f}", "yes" if r["fell"][b] else "no"]
         print(f"| {6 * f:.2f} | {1 - 0.6 * f:.2f} | " + " | ".join(cells) + " |")
+    adaptive = [n for n in names if "belief_nearest" in results[n]]
+    if adaptive:
+        print("| payload kg | friction | nearest member | " + " | ".join(f"{n} belief on it" for n in adaptive) + " |")
+        print("|---|---|---|" + "---|" * len(adaptive))
+        for b in range(B):
+            f = b / (B - 1)
+            print(f"| {6 * f:.2f} | {1 - 0.6 * f:.2f} | {nearest[b]} | "
+                  + " | ".join(f"{results[n]['belief_nearest'][b]:.3f}" for n in adaptive) + " |")
     for n in names:
         r = results[n]
         print(f"{n}: mean reward {np.mean(r['mean_reward']):.4f}, falls {sum(r['fell'])} of {B}")
-    print(json.dumps(dict(steps=args.steps, plants=B, ensemble=K, risk=args.risk, results=results, gpu=gpu_info())))
+    print(json.dumps(dict(steps=args.steps, plants=B, ensemble=K, risk=args.risk, adapt=args.adapt, results=results,
+                          gpu=gpu_info())))
 
 
 if __name__ == "__main__":
