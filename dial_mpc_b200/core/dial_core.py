@@ -369,6 +369,36 @@ class DeviceLoop:
             raise ValueError(f"rng must have shape {lead + (2,)}, got {key.shape}")
         if Y0 is not None and tuple(np.shape(Y0)) != lead + (a.Hnode + 1, mbdpi.nu):
             raise ValueError(f"Y0 must have shape {lead + (a.Hnode + 1, mbdpi.nu)}, got {tuple(np.shape(Y0))}")
+        # the ensemble settings: B of each, every one checked before anything is bound or uploaded
+        K = mbdpi.n_ensemble
+        members = []
+        if ensemble is not None:
+            self._need_ensemble("ensemble=", 1, ValueError)
+            shape = f"a list of {K} models or {B} such lists"
+            members = self._per_instance("ensemble", list(ensemble), shape,
+                                         lambda e: len(e) > 0 and all(isinstance(r, (list, tuple)) for r in e))
+            if any(len(r) != K for r in members):
+                raise ValueError(f"ensemble must be {shape}, got {[len(r) for r in members]}")
+        if risk is not None:
+            self._need_ensemble("risk=", 1, ValueError)
+            risk = self._per_instance("risk", risk, f"one risk spec or a list of {B}",
+                                      lambda r: isinstance(r, (list, tuple)))
+            for spec in risk:
+                risk_setting(spec, K)
+        for name, arg in (("adapt", adapt), ("prior", prior)):
+            if arg is not None:
+                self._need_ensemble(f"{name}=", 2, ValueError)
+        if prior is not None:
+            prior = self._per_instance("prior", list(prior), f"K weights or a list of {B} such lists",
+                                       lambda p: len(p) > 0 and all(isinstance(r, (list, tuple, np.ndarray)) for r in p))
+            for w in prior:
+                prior_setting(w, K)
+        if adapt is not None:
+            adapt = self._per_instance("adapt", adapt, f"one adapt spec or a list of {B}",
+                                       lambda s: isinstance(s, (list, tuple)))
+            for spec in adapt:
+                if spec is not None:
+                    adapt_setting(spec, K, m.nv)
         ps = [s.pipeline_state for s in states]
         per = (lambda t: t[0]) if B == 1 else torch.stack   # one instance: the buffers keep their plain shapes
         counters = [[int(s.info.get("step", 0)), int(s.info.get("contact_stage", 0))] for s in states]
@@ -408,46 +438,23 @@ class DeviceLoop:
         elif self._rand and hasattr(mbdpi.env, "stage_tables"):
             # seq-jump: the jump sequence drawn at reset is constant afterwards; one upload at bind time
             pl.set_stages(mbdpi.env.stage_tables(states[0].info))
-        members = self._ensemble_lists(mbdpi, ensemble)
         pl.mpc_bind(self.buf, mbdpi.M_shift.cpu().numpy())
-        base = bytes(_capi.fill_model_desc(mbdpi.env.sys.model))
-        if envs is not None:
-            for b, env_b in enumerate(envs):
-                if bytes(_capi.fill_model_desc(env_b.sys.model)) != base:
-                    pl.set_instance_model(b, env_b.sys)
+        # a model equal to mbdpi.env's is not uploaded: without one the plan allocates no model slots
+        base = bytes(_capi.fill_model_desc(m.model))
+        for b, env_b in enumerate(envs or ()):
+            if bytes(_capi.fill_model_desc(env_b.sys.model)) != base:
+                self.set_model(b, env_b)
         for b, row in enumerate(members):
-            for k, m in enumerate(row):
-                if bytes(_capi.fill_model_desc(m)) != base:
-                    pl.set_ensemble_model(b, k, m)
-        if risk is not None:
-            if mbdpi.n_ensemble < 1:
-                raise ValueError("risk= needs an MBDPI built with n_ensemble >= 1")
-            specs = list(risk) if isinstance(risk, (list, tuple)) else [risk] * B
-            if len(specs) != B:
-                raise ValueError(f"risk must be one risk spec or a list of {B}, got a list of {len(specs)}")
-            settings = [risk_setting(s, mbdpi.n_ensemble) for s in specs]   # every spec checked before any upload
-            for b, (mode, alpha) in enumerate(settings):
-                pl.set_ensemble_risk(b, mode, alpha)
-        for name, arg in (("adapt", adapt), ("prior", prior)):
-            if arg is not None and mbdpi.n_ensemble < 2:
-                raise ValueError(f"{name}= needs an MBDPI built with n_ensemble >= 2")
-        if prior is not None:
-            rows = list(prior)
-            per_instance = len(rows) > 0 and all(isinstance(r, (list, tuple, np.ndarray)) for r in rows)
-            rows = rows if per_instance else [rows] * B
-            if len(rows) != B:
-                raise ValueError(f"prior must be K weights or a list of {B} such lists, got a list of {len(rows)}")
-            weights = [prior_setting(r, mbdpi.n_ensemble) for r in rows]
-            for b, w in enumerate(weights):
-                pl.set_ensemble_belief(b, w)
-        if adapt is not None:
-            specs = list(adapt) if isinstance(adapt, (list, tuple)) else [adapt] * B
-            if len(specs) != B:
-                raise ValueError(f"adapt must be one adapt spec or a list of {B}, got a list of {len(specs)}")
-            settings = [None if s is None else adapt_setting(s, mbdpi.n_ensemble, m.nv) for s in specs]
-            for b, st in enumerate(settings):
-                if st is not None:
-                    pl.set_ensemble_adapt(b, True, *st)
+            for k, member in enumerate(row):
+                if bytes(_capi.fill_model_desc(self._model(member))) != base:
+                    self.set_ensemble_model(b, k, member)
+        for b, spec in enumerate(risk or ()):
+            self.set_risk(b, spec)
+        for b, w in enumerate(prior or ()):
+            self.set_belief(b, w)
+        for b, spec in enumerate(adapt or ()):
+            if spec is not None:
+                self.set_adapt(b, spec)
 
     @staticmethod
     def _model(env_or_sys):
@@ -455,20 +462,23 @@ class DeviceLoop:
         m = getattr(env_or_sys, "sys", env_or_sys)
         return getattr(m, "model", m)
 
-    def _ensemble_lists(self, mbdpi, ensemble) -> list:
-        """``ensemble`` as B lists of K models ([] when None)."""
-        if ensemble is None:
-            return []
-        K, B = mbdpi.n_ensemble, mbdpi.n_instances
-        if K < 1:
-            raise ValueError("ensemble= needs an MBDPI built with n_ensemble >= 1")
-        ens = list(ensemble)
-        per_instance = len(ens) > 0 and all(isinstance(e, (list, tuple)) for e in ens)
-        rows = [list(e) for e in ens] if per_instance else [ens] * B
-        if len(rows) != B or any(len(r) != K for r in rows):
-            raise ValueError(f"ensemble must be a list of {K} models or {B} such lists, got "
-                             f"{[len(r) for r in rows] if per_instance else len(ens)}")
-        return [[self._model(m) for m in r] for r in rows]
+    def _per_instance(self, name: str, value, shape: str, per_instance) -> list:
+        """``value`` as B values: its items when ``per_instance(value)``, else ``value`` for every instance.
+        Raises ValueError '<name> must be <shape>' when the items are not B."""
+        rows = list(value) if per_instance(value) else [value] * self.n_instances
+        if len(rows) != self.n_instances:
+            raise ValueError(f"{name} must be {shape}, got a list of {len(rows)}")
+        return rows
+
+    def _instance(self, b) -> int:
+        b = int(b)
+        if not 0 <= b < self.n_instances:
+            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        return b
+
+    def _need_ensemble(self, what: str, k: int, exc=RuntimeError) -> None:
+        if self.mbdpi.n_ensemble < k:
+            raise exc(f"{what} needs an MBDPI built with n_ensemble >= {k}")
 
     @staticmethod
     def _check_shared(ref_env, env) -> None:
@@ -495,9 +505,7 @@ class DeviceLoop:
         one-step random command on top."""
         if self._tasks_host is None:
             raise RuntimeError("set_task needs per-instance tasks: build the DeviceLoop with envs=[...]")
-        b = int(b)
-        if not 0 <= b < self.n_instances:
-            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        b = self._instance(b)
         if isinstance(env_or_task, _capi.dial_task):
             t = _capi.check_task(_capi.dial_task.from_buffer_copy(env_or_task))
         else:
@@ -512,20 +520,14 @@ class DeviceLoop:
         ``System`` or a ``CompiledModel`` with the structure, timestep, joint and control ranges of
         ``mbdpi.env``'s model.  A stream-ordered copy on the current stream.  The first per-instance
         model of a loop makes the next steps capture their graphs again."""
-        b = int(b)
-        if not 0 <= b < self.n_instances:
-            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
-        self.plan.set_instance_model(b, getattr(env_or_sys, "sys", env_or_sys))
+        self.plan.set_instance_model(self._instance(b), getattr(env_or_sys, "sys", env_or_sys))
 
     def set_ensemble_model(self, b: int, k: int, env_or_sys) -> None:
         """Replace member k of instance b's planning ensemble before the next ``step``: an env, a ``System``
         or a ``CompiledModel`` (``Plan.set_ensemble_model``).  The first member set on a loop makes the next
         steps capture their graphs again."""
-        b, k = int(b), int(k)
-        if self.mbdpi.n_ensemble < 1:
-            raise RuntimeError("set_ensemble_model needs an MBDPI built with n_ensemble >= 1")
-        if not 0 <= b < self.n_instances:
-            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
+        self._need_ensemble("set_ensemble_model", 1)
+        b, k = self._instance(b), int(k)
         if not 0 <= k < self.mbdpi.n_ensemble:
             raise IndexError(f"member {k} out of range (0..{self.mbdpi.n_ensemble - 1})")
         self.plan.set_ensemble_model(b, k, self._model(env_or_sys))
@@ -533,27 +535,16 @@ class DeviceLoop:
     def set_risk(self, b: int, spec) -> None:
         """Instance b's risk measure over its members' rewards from the next ``step`` on (a risk spec,
         ``risk_setting``).  A stream-ordered copy on the current stream; the captured graphs are kept."""
-        b = int(b)
-        if self.mbdpi.n_ensemble < 1:
-            raise RuntimeError("set_risk needs an MBDPI built with n_ensemble >= 1")
-        if not 0 <= b < self.n_instances:
-            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
-        self.plan.set_ensemble_risk(b, *risk_setting(spec, self.mbdpi.n_ensemble))
-
-    def _adapt_instance(self, what: str, b) -> int:
-        if self.mbdpi.n_ensemble < 2:
-            raise RuntimeError(f"{what} needs an MBDPI built with n_ensemble >= 2")
-        b = int(b)
-        if not 0 <= b < self.n_instances:
-            raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
-        return b
+        self._need_ensemble("set_risk", 1)
+        self.plan.set_ensemble_risk(self._instance(b), *risk_setting(spec, self.mbdpi.n_ensemble))
 
     def set_adapt(self, b: int, spec) -> None:
         """Instance b adapts its belief to its plant from the next env step on (an adapt spec,
         ``adapt_setting``), or stops adapting (None; the belief is kept).  A stream-ordered copy on the
         current stream; the first instance of a loop to adapt makes the next steps capture their graphs
         again, later calls keep them."""
-        b = self._adapt_instance("set_adapt", b)
+        self._need_ensemble("set_adapt", 2)
+        b = self._instance(b)
         if spec is None:
             self.plan.set_ensemble_adapt(b, False)
         else:
@@ -562,14 +553,12 @@ class DeviceLoop:
     def set_belief(self, b: int, w) -> None:
         """Instance b's belief from K weights >= 0 with a positive sum (``prior_setting``), e.g. from an
         outside estimator; a stream-ordered copy that keeps the captured graphs."""
-        b = self._adapt_instance("set_belief", b)
-        self.plan.set_ensemble_belief(b, prior_setting(w, self.mbdpi.n_ensemble))
+        self._need_ensemble("set_belief", 2)
+        self.plan.set_ensemble_belief(self._instance(b), prior_setting(w, self.mbdpi.n_ensemble))
 
     def _belief(self, which: int) -> torch.Tensor:
-        K = self.mbdpi.n_ensemble
-        if K < 2:
-            raise RuntimeError(f"{('belief', 'member_loglik')[which]} needs an MBDPI built with n_ensemble >= 2")
-        out = self.plan.empty(*((self.n_instances,) if self.n_instances > 1 else ()), K)
+        self._need_ensemble(("belief", "member_loglik")[which], 2)
+        out = self.plan.empty(*((self.n_instances,) if self.n_instances > 1 else ()), self.mbdpi.n_ensemble)
         self.plan.ensemble_belief(*((out, None) if which == 0 else (None, out)))
         return out
 
@@ -587,11 +576,9 @@ class DeviceLoop:
         """The member rewards of the last diffusion iteration of the steps launched so far, a new tensor
         [B, K, Nsample+1] ([K, Nsample+1] for one instance): the rewards each sample's score reduces
         (``Plan.member_rewards``).  Asynchronous on the current stream."""
-        K = self.mbdpi.n_ensemble
-        if K < 1:
-            raise RuntimeError("member_rewards needs an MBDPI built with n_ensemble >= 1")
+        self._need_ensemble("member_rewards", 1)
         lead = (self.n_instances,) if self.n_instances > 1 else ()
-        return self.plan.member_rewards(self.plan.empty(*lead, K, self.mbdpi.Nlocal + 1))
+        return self.plan.member_rewards(self.plan.empty(*lead, self.mbdpi.n_ensemble, self.mbdpi.Nlocal + 1))
 
     def step(self, n_diffuse: Optional[int] = None, env_step=True) -> None:
         """One control step (asynchronous on the current stream).  env_step: True = env step + shift
@@ -728,19 +715,6 @@ def risk_setting(spec, K: int):
     return cvar, float(a)
 
 
-def load_risk(spec, K: int):
-    """The ``risk`` entry of an ``--ensemble`` file or an ``--instance-overrides`` mapping: the checked
-    risk spec (``risk_setting``), or None when ``spec`` has no ``risk``.  Raises ValueError starting with
-    'risk: '."""
-    if not isinstance(spec, dict) or spec.get("risk") is None:
-        return None
-    try:
-        risk_setting(spec["risk"], K)
-    except ValueError as e:
-        raise ValueError(f"risk: {e}") from None
-    return dict(spec["risk"])
-
-
 def adapt_setting(spec, K: int, nv: int):
     """An adapt spec -> (forget, prune, sigma [nv] fp32) of ``dial_plan_set_ensemble_adapt`` for K members
     and nv dofs.  ``sigma`` (required): the scale of each qvel residual, one number for every dof or nv
@@ -797,41 +771,33 @@ def prior_setting(w, K: int):
     return a
 
 
-def load_adapt(spec, K: int, nv: int):
-    """The ``adapt`` entry of an ``--ensemble`` file or an ``--instance-overrides`` mapping: the checked
-    adapt spec (``adapt_setting``), or None when ``spec`` has no ``adapt``.  Raises ValueError starting
-    with 'adapt: '."""
-    if not isinstance(spec, dict) or spec.get("adapt") is None:
+def load_setting(spec, key: str, K: int, nv: Optional[int] = None):
+    """The ``risk``, ``adapt`` or ``prior`` entry ``key`` of an ``--ensemble`` file or an
+    ``--instance-overrides`` mapping, checked for K members and nv dofs (``risk_setting``,
+    ``adapt_setting``, ``prior_setting``), or None when ``spec`` has no such entry.  Raises ValueError
+    starting with '<key>: '."""
+    if not isinstance(spec, dict) or spec.get(key) is None:
         return None
-    if K < 2:
-        raise ValueError(f"adapt: needs an ensemble of at least 2 members, got {K}")
     try:
-        adapt_setting(spec["adapt"], K, nv)
+        if key == "risk":
+            risk_setting(spec[key], K)
+        elif K < 2:
+            raise ValueError(f"needs an ensemble of at least 2 members, got {K}")
+        elif key == "adapt":
+            adapt_setting(spec[key], K, nv)
+        else:
+            prior_setting(spec[key], K)
     except ValueError as e:
-        raise ValueError(f"adapt: {e}") from None
-    return dict(spec["adapt"])
-
-
-def load_prior(spec, K: int):
-    """The ``prior`` entry of an ``--ensemble`` file: K weights (``prior_setting``) or None.  Raises
-    ValueError starting with 'prior: '."""
-    if not isinstance(spec, dict) or spec.get("prior") is None:
-        return None
-    if K < 2:
-        raise ValueError(f"prior: needs an ensemble of at least 2 members, got {K}")
-    try:
-        return prior_setting(spec["prior"], K).tolist()
-    except ValueError as e:
-        raise ValueError(f"prior: {e}") from None
+        raise ValueError(f"{key}: {e}") from None
+    return spec[key]
 
 
 def load_ensemble(spec, env):
     """The ``--ensemble`` file's mapping -> (K member ``System``s, the plant's ``sys`` mapping or None).
     ``members``: a list of K ``System.tree_replace`` mappings of ``env``'s model (``{}``: the nominal
     model); ``plant`` (optional): one such mapping for every instance's plant; ``risk`` (optional): the
-    risk spec of every instance, read by ``load_risk``; ``adapt`` / ``prior`` (optional): adaptation to
-    the plant, read by ``load_adapt`` / ``load_prior``.  Raises ValueError naming the entry that is
-    malformed."""
+    risk spec of every instance; ``adapt`` / ``prior`` (optional): adaptation to the plant; the last three
+    are read by ``load_setting``.  Raises ValueError naming the entry that is malformed."""
     if not isinstance(spec, dict) or set(spec) - {"members", "plant", "risk", "adapt", "prior"} or "members" not in spec:
         raise ValueError("must map 'members' (a list of sys mappings) and optionally 'plant' (one sys mapping), "
                          "'risk' (a risk spec), 'adapt' (an adapt spec) and 'prior' (K weights), got "
@@ -963,9 +929,8 @@ def main():
         try:
             ens_spec = yaml.safe_load(open(args.ensemble))
             members, plant = load_ensemble(ens_spec, env)
-            risk = load_risk(ens_spec, len(members))
-            adapt = load_adapt(ens_spec, len(members), env.sys.nv)
-            prior = load_prior(ens_spec, len(members))
+            risk, adapt, prior = (load_setting(ens_spec, key, len(members), env.sys.nv)
+                                  for key in ("risk", "adapt", "prior"))
         except (ValueError, yaml.YAMLError) as e:
             parser.error(f"--ensemble {args.ensemble}: {e}")
     if args.instance_overrides is not None:
@@ -977,8 +942,8 @@ def main():
                          f"got {len(overrides) if isinstance(overrides, list) else type(overrides).__name__}")
         known = {f.name for f in dataclasses.fields(env_config_type)} | {"sys", "risk", "adapt"}
         envs = []
-        risks = [risk] * args.instances
-        adapts = [adapt] * args.instances
+        settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
+        uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
@@ -986,22 +951,15 @@ def main():
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
             sys_ov = ov.pop("sys", None)
-            if ov.get("risk") is not None:
-                if members is None:
-                    parser.error(f"--instance-overrides entry {b}: risk needs --ensemble (it scores the members' rewards)")
-                try:
-                    risks[b] = load_risk(ov, len(members))
-                except ValueError as e:
-                    parser.error(f"--instance-overrides entry {b}: {e}")
-            ov.pop("risk", None)
-            if ov.get("adapt") is not None:
-                if members is None:
-                    parser.error(f"--instance-overrides entry {b}: adapt needs --ensemble (it weights the members)")
-                try:
-                    adapts[b] = load_adapt(ov, len(members), env.sys.nv)
-                except ValueError as e:
-                    parser.error(f"--instance-overrides entry {b}: {e}")
-            ov.pop("adapt", None)
+            for key in ("risk", "adapt"):
+                if ov.get(key) is not None:
+                    if members is None:
+                        parser.error(f"--instance-overrides entry {b}: {key} needs --ensemble ({uses[key]})")
+                    try:
+                        settings[key][b] = load_setting(ov, key, len(members), env.sys.nv)
+                    except ValueError as e:
+                        parser.error(f"--instance-overrides entry {b}: {e}")
+                ov.pop(key, None)
             cfg_b = load_dataclass_from_dict(env_config_type, dict(config_dict, **ov), convert_list_to_array=True)
             envs.append(dial_envs.get_environment(dial_config.env_name, config=cfg_b))
             try:
@@ -1023,10 +981,10 @@ def main():
         if args.instances > 1:
             envs = [plant_env] * args.instances
     if args.instances > 1:
-        if args.instance_overrides is not None and any(r is not None for r in risks):
-            risk = [r or {"aggregate": "mean"} for r in risks]
-        if args.instance_overrides is not None and any(a is not None for a in adapts):
-            adapt = adapts
+        if args.instance_overrides is not None and any(r is not None for r in settings["risk"]):
+            risk = [r or {"aggregate": "mean"} for r in settings["risk"]]
+        if args.instance_overrides is not None and any(a is not None for a in settings["adapt"]):
+            adapt = settings["adapt"]
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
                       ensemble=members, risk=risk, adapt=adapt, prior=prior)
         return

@@ -13,6 +13,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <float.h>
+#include <memory>
 #include <string>
 #include <vector>
 #include <new>
@@ -599,6 +600,47 @@ __global__ void __launch_bounds__(32) ens_belief_kernel(const float* __restrict_
 // ---------------------------------------------------------------------------------
 // plan object
 // ---------------------------------------------------------------------------------
+// A per-instance setting the captured graphs read between replays: the device array of n slots of `width`
+// elements, its pinned host staging and, per slot, the event of the last copy out of the staging slot.
+// `d` stays null until allocate(): the launches tell an unset setting by it.
+template <class T> struct Staged {
+  T* d = nullptr;
+  T* h = nullptr;
+  size_t width = 1;
+  std::vector<cudaEvent_t> ev;
+  // every element starts as `init`, uploaded synchronously; on failure nothing stays allocated
+  cudaError_t allocate(size_t n, size_t w, const T& init) {
+    width = w;
+    cudaError_t e = cudaMallocHost(&h, n * w * sizeof(T));
+    if (e == cudaSuccess) e = cudaMalloc(&d, n * w * sizeof(T));
+    if (e == cudaSuccess) {
+      for (size_t i = 0; i < n * w; ++i) h[i] = init;
+      e = cudaMemcpy(d, h, n * w * sizeof(T), cudaMemcpyHostToDevice);
+    }
+    if (e != cudaSuccess) { release(); return e; }
+    ev.assign(n, nullptr);
+    return cudaSuccess;
+  }
+  // `fill(h_slot)` rewrites slot `s` of the staging, once the previous copy out of it has run; the slot is
+  // then copied stream-ordered on `st`, and the captured graphs read it at their next replay
+  template <class F> cudaError_t put(size_t s, F fill, cudaStream_t st) {
+    cudaEvent_t& e_s = ev[s];
+    cudaError_t e = e_s ? cudaEventSynchronize(e_s) : cudaEventCreateWithFlags(&e_s, cudaEventDisableTiming);
+    if (e == cudaSuccess) {
+      fill(h + s * width);
+      e = cudaMemcpyAsync(d + s * width, h + s * width, width * sizeof(T), cudaMemcpyHostToDevice, st);
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(e_s, st);
+    return e;
+  }
+  void release() {
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    ev.clear();
+    cudaFree(d); cudaFreeHost(h);
+    d = nullptr; h = nullptr;
+  }
+};
+
 struct dial_plan {
   DevModel hM;
   DevPlan hP;
@@ -636,36 +678,23 @@ struct dial_plan {
   uint32_t* mpc_key = nullptr;  // sampling key of the current reverse_once
   struct MpcGraph { int n_diffuse, env_step, seen; cudaGraphExec_t exec; int64_t launches; };
   std::vector<MpcGraph> mpc_graphs;
-  // per-instance models (dial_plan_set_instance_model): device array [n_inst] read by dial_mpc_step,
-  // its pinned host staging [n_inst] and, per slot, the event of the last copy out of the staging slot
-  DevModel* dModels = nullptr;
-  DevModel* hModels = nullptr;
-  std::vector<cudaEvent_t> model_ev;
+  // per-instance models (dial_plan_set_instance_model): [n_inst] slots read by dial_mpc_step, allocated by
+  // the first call
+  Staged<DevModel> models;
   // ensemble members (dial_plan_set_ensemble_model): the same for [n_inst * n_ens] member slots, and the
   // members' rewards [n_inst, n_ens, Nsample+1] of one reverse_once (n_ens >= 2)
-  DevModel* dMembers = nullptr;
-  DevModel* hMembers = nullptr;
-  std::vector<cudaEvent_t> member_ev;
+  Staged<DevModel> members;
   float* ens_rews = nullptr;
-  // risk measure per instance (dial_plan_set_ensemble_risk, n_ens >= 2): device array [n_inst] read by
-  // the reduction, its pinned staging and the per-slot events of the last copy, as for the models
-  EnsRisk* dRisk = nullptr;
-  EnsRisk* hRisk = nullptr;
-  std::vector<cudaEvent_t> risk_ev;
-  // adaptation to the plant (dial_plan_set_ensemble_adapt / _belief, n_ens >= 2): the settings [n_inst]
-  // with their pinned staging and copy events, as for the risk measure; the belief L [n_inst, n_ens] in
-  // fp64, w and the last update's l in fp32, with pinned staging for L and w and one copy event per
-  // instance.  pred_us [n_inst n_ens, nu] / pred_qd [n_inst n_ens, nv] (the members' predictions) are
+  // risk measure per instance (dial_plan_set_ensemble_risk, n_ens >= 2): [n_inst] slots read by the reduction
+  Staged<EnsRisk> risk;
+  // adaptation to the plant (dial_plan_set_ensemble_adapt / _belief, n_ens >= 2): the settings [n_inst]; the
+  // belief L [n_inst, n_ens] in fp64 and w in fp32, one slot of n_ens per instance; the last update's l in
+  // fp32.  pred_us [n_inst n_ens, nu] / pred_qd [n_inst n_ens, nv] (the members' predictions) are
   // allocated by the first call that turns adaptation on; until then the graphs hold no adaptation launch.
-  EnsAdapt* dAdapt = nullptr;
-  EnsAdapt* hAdapt = nullptr;
-  std::vector<cudaEvent_t> adapt_ev;
-  double* dL = nullptr;
-  double* hL = nullptr;
-  float* dW = nullptr;
-  float* hW = nullptr;
+  Staged<EnsAdapt> adapt;
+  Staged<double> belief_L;
+  Staged<float> belief_w;
   float* dEll = nullptr;
-  std::vector<cudaEvent_t> belief_ev;
   float* pred_us = nullptr;
   float* pred_qd = nullptr;
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
@@ -686,6 +715,12 @@ struct dial_plan {
     uint32_t* bseq() const { return base[rank] + o_local + 3; }
   } xch;
 };
+
+// the control-step graphs captured so far: dial_mpc_step captures them again on their next use
+static void drop_graphs(dial_plan* p) {
+  for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+  p->mpc_graphs.clear();
+}
 
 static void fill_xch(const dial_plan* p, RolloutArgs& A) {
   if (!p->xch.on) return;
@@ -879,29 +914,15 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
   }
   if (p->n_ens > 1) {
     if ((e = cudaMalloc(&p->ens_rews, rows * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(ens_rews)");
-    // every instance starts at the mean
-    if ((e = cudaMallocHost(&p->hRisk, B * sizeof(EnsRisk))) != cudaSuccess) return bad(e, "cudaMallocHost(risk)");
-    if ((e = cudaMalloc(&p->dRisk, B * sizeof(EnsRisk))) != cudaSuccess) return bad(e, "cudaMalloc(risk)");
-    for (size_t b = 0; b < B; ++b) p->hRisk[b] = ens_risk_derive(p->n_ens, DIAL_ENS_MEAN, 1.f);
-    if ((e = cudaMemcpy(p->dRisk, p->hRisk, B * sizeof(EnsRisk), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(risk)");
-    p->risk_ev.assign(B, nullptr);
-    // no instance adapts; every belief starts uniform
-    const size_t BK = B * p->n_ens;
-    if ((e = cudaMallocHost(&p->hAdapt, B * sizeof(EnsAdapt))) != cudaSuccess) return bad(e, "cudaMallocHost(adapt)");
-    if ((e = cudaMalloc(&p->dAdapt, B * sizeof(EnsAdapt))) != cudaSuccess) return bad(e, "cudaMalloc(adapt)");
-    memset(p->hAdapt, 0, B * sizeof(EnsAdapt));
-    if ((e = cudaMemcpy(p->dAdapt, p->hAdapt, B * sizeof(EnsAdapt), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(adapt)");
-    p->adapt_ev.assign(B, nullptr);
-    if ((e = cudaMallocHost(&p->hL, BK * sizeof(double))) != cudaSuccess) return bad(e, "cudaMallocHost(belief)");
-    if ((e = cudaMallocHost(&p->hW, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMallocHost(belief)");
-    if ((e = cudaMalloc(&p->dL, BK * sizeof(double))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
-    if ((e = cudaMalloc(&p->dW, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
-    if ((e = cudaMalloc(&p->dEll, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
-    for (size_t i = 0; i < BK; ++i) { p->hL[i] = log(1.0 / p->n_ens); p->hW[i] = (float)exp(p->hL[i]); }
-    if ((e = cudaMemcpy(p->dL, p->hL, BK * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(belief)");
-    if ((e = cudaMemcpy(p->dW, p->hW, BK * sizeof(float), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(belief)");
-    if ((e = cudaMemset(p->dEll, 0, BK * sizeof(float))) != cudaSuccess) return bad(e, "cudaMemset(belief)");
-    p->belief_ev.assign(B, nullptr);
+    // every instance starts at the mean, no instance adapts, every belief starts uniform
+    const size_t K = p->n_ens;
+    const double L0 = log(1.0 / p->n_ens);
+    if ((e = p->risk.allocate(B, 1, ens_risk_derive(p->n_ens, DIAL_ENS_MEAN, 1.f))) != cudaSuccess) return bad(e, "allocate(risk)");
+    if ((e = p->adapt.allocate(B, 1, EnsAdapt{})) != cudaSuccess) return bad(e, "allocate(adapt)");
+    if ((e = p->belief_L.allocate(B, K, L0)) != cudaSuccess) return bad(e, "allocate(belief)");
+    if ((e = p->belief_w.allocate(B, K, (float)exp(L0))) != cudaSuccess) return bad(e, "allocate(belief)");
+    if ((e = cudaMalloc(&p->dEll, B * K * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
+    if ((e = cudaMemset(p->dEll, 0, B * K * sizeof(float))) != cudaSuccess) return bad(e, "cudaMemset(belief)");
   }
   if ((e = cudaMalloc(&p->weights, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
   if ((e = cudaMalloc(&p->weights2, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
@@ -935,24 +956,16 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   if (!p) return;
   cudaFree(p->dM); cudaFree(p->dP);
   for (int b = 0; b < 2; ++b) { cudaFree(p->traj_q[b]); cudaFree(p->traj_qd[b]); cudaFree(p->traj_x[b]); }
-  for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+  drop_graphs(p);
   for (int r = 0; r < DIAL_MAXRANK; ++r) {
     if (!p->xch.base[r]) continue;
     if (r == p->xch.rank) cudaFree(p->xch.base[r]); else cudaIpcCloseMemHandle(p->xch.base[r]);
   }
   cudaFree(p->xch.bars_partial);
   cudaFree(p->mpc_Msh); cudaFree(p->mpc_Y1); cudaFree(p->mpc_key);
-  for (cudaEvent_t e : p->model_ev) if (e) cudaEventDestroy(e);
-  cudaFree(p->dModels); cudaFreeHost(p->hModels);
-  for (cudaEvent_t e : p->member_ev) if (e) cudaEventDestroy(e);
-  cudaFree(p->dMembers); cudaFreeHost(p->hMembers); cudaFree(p->ens_rews);
-  for (cudaEvent_t e : p->risk_ev) if (e) cudaEventDestroy(e);
-  cudaFree(p->dRisk); cudaFreeHost(p->hRisk);
-  for (cudaEvent_t e : p->adapt_ev) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : p->belief_ev) if (e) cudaEventDestroy(e);
-  cudaFree(p->dAdapt); cudaFreeHost(p->hAdapt);
-  cudaFree(p->dL); cudaFree(p->dW); cudaFree(p->dEll); cudaFreeHost(p->hL); cudaFreeHost(p->hW);
-  cudaFree(p->pred_us); cudaFree(p->pred_qd);
+  p->models.release(); p->members.release(); p->risk.release();
+  p->adapt.release(); p->belief_L.release(); p->belief_w.release();
+  cudaFree(p->ens_rews); cudaFree(p->dEll); cudaFree(p->pred_us); cudaFree(p->pred_qd);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   cudaFree(p->weights2);
@@ -1009,124 +1022,95 @@ extern "C" int dial_plan_set_stages(dial_plan* p, int n_stage, const float* pose
   return 0;
 }
 
-// Derive `m`, check it against the plan's model and copy it into slot `slot` of the model array `d`
-// [n] (pinned staging `h`, copy events `ev`), allocating the array on first use with every slot holding
-// the plan's own model and dropping the captured graphs then.  `fn` names the public call in errors.
-static int set_model_slot(dial_plan* p, const char* fn, DevModel*& d, DevModel*& h, std::vector<cudaEvent_t>& evs,
-                          size_t n, size_t slot, const dial_model_desc* m, cudaStream_t st) {
-  DevModel* D = new (std::nothrow) DevModel();
-  if (!D) return fail("out of memory");
-  std::string err;
-  if (!derive_model(*m, *D, err)) { delete D; return fail(std::string(fn) + ": " + err); }
-  const char* diff = instance_model_difference(p->hM, *D);
-  if (diff) {
-    delete D;
-    return fail(std::string(fn) + ": field '" + diff + "' differs from the plan's model "
-                "(an instance's model may differ in floats other than timestep, jnt_range and actuator_ctrlrange only)");
-  }
-  cudaError_t e = cudaSuccess;
-  if (!d) {
-    // first call: every slot starts as the plan's own model; the graphs captured so far launch without
-    // this array and are recaptured on their next use
-    if ((e = cudaMallocHost(&h, n * sizeof(DevModel))) == cudaSuccess &&
-        (e = cudaMalloc(&d, n * sizeof(DevModel))) == cudaSuccess) {
-      for (size_t i = 0; i < n; ++i) h[i] = p->hM;
-      e = cudaMemcpy(d, h, n * sizeof(DevModel), cudaMemcpyHostToDevice);
-    }
-    if (e != cudaSuccess) {
-      cudaFree(d); cudaFreeHost(h); d = nullptr; h = nullptr;
-      delete D;
-      return fail(std::string(fn) + ": " + cudaGetErrorString(e));
-    }
-    evs.assign(n, nullptr);
-    for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    p->mpc_graphs.clear();
-  }
-  // stream-ordered copy out of the slot's pinned staging; the staging slot is rewritten only after the
-  // previous copy out of it has run
-  cudaEvent_t& ev = evs[slot];
-  if (ev) e = cudaEventSynchronize(ev);
-  else e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) {
-    h[slot] = *D;
-    e = cudaMemcpyAsync(d + slot, h + slot, sizeof(DevModel), cudaMemcpyHostToDevice, st);
-  }
-  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
-  delete D;
-  CUDA_OK(e);
-  return 0;
-}
-
-extern "C" int dial_plan_set_instance_model(dial_plan* p, int b, const dial_model_desc* m, void* stream) {
-  if (!p || !m) return fail("dial_plan_set_instance_model: null argument");
-  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_instance_model: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
-  if (p->hP.c.Ntotal != p->hP.c.Nsample) return fail("dial_plan_set_instance_model: sharded plans (Ntotal != Nsample) share one model");
-  return set_model_slot(p, "dial_plan_set_instance_model", p->dModels, p->hModels, p->model_ev, (size_t)p->n_inst,
-                        (size_t)b, m, (cudaStream_t)stream);
-}
-
-extern "C" int dial_plan_set_ensemble_model(dial_plan* p, int b, int k, const dial_model_desc* m, void* stream) {
-  if (!p || !m) return fail("dial_plan_set_ensemble_model: null argument");
-  if (p->n_ens < 1) return fail("dial_plan_set_ensemble_model: the plan has no ensemble (dial_plan_desc.n_ens = 0)");
-  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_ensemble_model: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
-  if (k < 0 || k >= p->n_ens) return fail("dial_plan_set_ensemble_model: member " + std::to_string(k) + " out of range (0.." + std::to_string(p->n_ens - 1) + ")");
-  return set_model_slot(p, "dial_plan_set_ensemble_model", p->dMembers, p->hMembers, p->member_ev,
-                        (size_t)p->n_inst * p->n_ens, (size_t)b * p->n_ens + k, m, (cudaStream_t)stream);
-}
-
-extern "C" int dial_plan_set_ensemble_risk(dial_plan* p, int b, int mode, float alpha, void* stream) {
-  if (!p) return fail("dial_plan_set_ensemble_risk: null plan");
-  if (p->n_ens < 1) return fail("dial_plan_set_ensemble_risk: the plan has no ensemble (dial_plan_desc.n_ens = 0)");
-  if (b < 0 || b >= p->n_inst) return fail("dial_plan_set_ensemble_risk: instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
-  if (mode != DIAL_ENS_MEAN && mode != DIAL_ENS_CVAR)
-    return fail("dial_plan_set_ensemble_risk: mode " + std::to_string(mode) + " is neither DIAL_ENS_MEAN (0) nor DIAL_ENS_CVAR (1)");
-  if (mode == DIAL_ENS_CVAR && !(alpha > 0.f && alpha <= 1.f)) {   // also rejects NaN and infinities
-    char buf[64];
-    snprintf(buf, sizeof(buf), "%g", (double)alpha);
-    return fail(std::string("dial_plan_set_ensemble_risk: alpha must be finite and in (0, 1] for DIAL_ENS_CVAR, got ") + buf);
-  }
-  if (p->n_ens < 2) return 0;   // one member: every risk measure of one reward is that reward
-  // stream-ordered copy out of the slot's pinned staging, rewritten only after its previous copy has run;
-  // the captured graphs hold the array's pointer and read the new setting at their next replay
-  cudaStream_t st = (cudaStream_t)stream;
-  cudaEvent_t& ev = p->risk_ev[b];
-  cudaError_t e = ev ? cudaEventSynchronize(ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) {
-    p->hRisk[b] = ens_risk_derive(p->n_ens, mode, alpha);
-    e = cudaMemcpyAsync(p->dRisk + b, p->hRisk + b, sizeof(EnsRisk), cudaMemcpyHostToDevice, st);
-  }
-  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
-  if (e != cudaSuccess) return fail(std::string("dial_plan_set_ensemble_risk: ") + cudaGetErrorString(e));
-  return 0;
-}
-
-extern "C" int dial_plan_member_rewards(dial_plan* p, float* out, void* stream) {
-  if (!p || !out) return fail("dial_plan_member_rewards: null argument");
-  if (p->n_ens < 1) return fail("dial_plan_member_rewards: the plan has no ensemble (dial_plan_desc.n_ens = 0)");
-  if (!p->mpc_bound) return fail("dial_plan_member_rewards: call dial_mpc_bind first");
-  const size_t n = (size_t)p->n_inst * p->n_ens * ((size_t)p->hP.c.Nsample + 1);
-  const float* src = p->n_ens > 1 ? p->ens_rews : p->mpc.rews;   // n_ens = 1: the rollout writes rews itself
-  CUDA_OK(cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  return 0;
-}
-
 static std::string fmt_g(double x) {
   char buf[64];
   snprintf(buf, sizeof(buf), "%g", x);
   return buf;
 }
 
-// the checks every adaptation call shares: a plan with n_ens >= 2 and b in range
-static int adapt_target(const dial_plan* p, const char* fn, int b) {
+// The checks the per-instance setters share; `fn` names the public call in errors.  A plan (not null) with
+// an ensemble of at least k (1 or 2) members:
+static int need_ensemble(const dial_plan* p, const char* fn, int k) {
   if (!p) return fail(std::string(fn) + ": null plan");
-  if (p->n_ens < 2) return fail(std::string(fn) + ": the plan needs an ensemble of n_ens >= 2 members, it has " + std::to_string(p->n_ens));
-  if (b < 0 || b >= p->n_inst) return fail(std::string(fn) + ": instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
+  if (p->n_ens >= k) return 0;
+  if (k == 1) return fail(std::string(fn) + ": the plan has no ensemble (dial_plan_desc.n_ens = 0)");
+  return fail(std::string(fn) + ": the plan needs an ensemble of n_ens >= " + std::to_string(k) + " members, it has " + std::to_string(p->n_ens));
+}
+// b is an instance of the plan:
+static int need_instance(const dial_plan* p, const char* fn, int b) {
+  if (b >= 0 && b < p->n_inst) return 0;
+  return fail(std::string(fn) + ": instance " + std::to_string(b) + " out of range (0.." + std::to_string(p->n_inst - 1) + ")");
+}
+
+// Derive `m`, check it against the plan's model and copy it into slot `slot` of the model slots `a` [n],
+// allocating them on first use with every slot holding the plan's own model and dropping the captured
+// graphs then.  `fn` names the public call in errors.
+static int set_model_slot(dial_plan* p, const char* fn, Staged<DevModel>& a, size_t n, size_t slot,
+                          const dial_model_desc* m, cudaStream_t st) {
+  std::unique_ptr<DevModel> D(new (std::nothrow) DevModel());
+  if (!D) return fail("out of memory");
+  std::string err;
+  if (!derive_model(*m, *D, err)) return fail(std::string(fn) + ": " + err);
+  if (const char* diff = instance_model_difference(p->hM, *D))
+    return fail(std::string(fn) + ": field '" + diff + "' differs from the plan's model "
+                "(an instance's model may differ in floats other than timestep, jnt_range and actuator_ctrlrange only)");
+  cudaError_t e = cudaSuccess;
+  if (!a.d) {
+    // first call: the graphs captured so far launch without these slots
+    if ((e = a.allocate(n, 1, p->hM)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+    drop_graphs(p);
+  }
+  e = a.put(slot, [&](DevModel* h) { *h = *D; }, st);
+  CUDA_OK(e);
+  return 0;
+}
+
+extern "C" int dial_plan_set_instance_model(dial_plan* p, int b, const dial_model_desc* m, void* stream) {
+  static const char* fn = "dial_plan_set_instance_model";
+  if (!p || !m) return fail(std::string(fn) + ": null argument");
+  if (int rc = need_instance(p, fn, b)) return rc;
+  if (p->hP.c.Ntotal != p->hP.c.Nsample) return fail(std::string(fn) + ": sharded plans (Ntotal != Nsample) share one model");
+  return set_model_slot(p, fn, p->models, (size_t)p->n_inst, (size_t)b, m, (cudaStream_t)stream);
+}
+
+extern "C" int dial_plan_set_ensemble_model(dial_plan* p, int b, int k, const dial_model_desc* m, void* stream) {
+  static const char* fn = "dial_plan_set_ensemble_model";
+  if (!p || !m) return fail(std::string(fn) + ": null argument");
+  if (int rc = need_ensemble(p, fn, 1)) return rc;
+  if (int rc = need_instance(p, fn, b)) return rc;
+  if (k < 0 || k >= p->n_ens) return fail(std::string(fn) + ": member " + std::to_string(k) + " out of range (0.." + std::to_string(p->n_ens - 1) + ")");
+  return set_model_slot(p, fn, p->members, (size_t)p->n_inst * p->n_ens, (size_t)b * p->n_ens + k, m, (cudaStream_t)stream);
+}
+
+extern "C" int dial_plan_set_ensemble_risk(dial_plan* p, int b, int mode, float alpha, void* stream) {
+  static const char* fn = "dial_plan_set_ensemble_risk";
+  if (int rc = need_ensemble(p, fn, 1)) return rc;
+  if (int rc = need_instance(p, fn, b)) return rc;
+  if (mode != DIAL_ENS_MEAN && mode != DIAL_ENS_CVAR)
+    return fail(std::string(fn) + ": mode " + std::to_string(mode) + " is neither DIAL_ENS_MEAN (0) nor DIAL_ENS_CVAR (1)");
+  if (mode == DIAL_ENS_CVAR && !(alpha > 0.f && alpha <= 1.f))   // also rejects NaN and infinities
+    return fail(std::string(fn) + ": alpha must be finite and in (0, 1] for DIAL_ENS_CVAR, got " + fmt_g(alpha));
+  if (p->n_ens < 2) return 0;   // one member: every risk measure of one reward is that reward
+  cudaError_t e = p->risk.put(b, [&](EnsRisk* r) { *r = ens_risk_derive(p->n_ens, mode, alpha); }, (cudaStream_t)stream);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int dial_plan_member_rewards(dial_plan* p, float* out, void* stream) {
+  static const char* fn = "dial_plan_member_rewards";
+  if (!p || !out) return fail(std::string(fn) + ": null argument");
+  if (int rc = need_ensemble(p, fn, 1)) return rc;
+  if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
+  const size_t n = (size_t)p->n_inst * p->n_ens * ((size_t)p->hP.c.Nsample + 1);
+  const float* src = p->n_ens > 1 ? p->ens_rews : p->mpc.rews;   // n_ens = 1: the rollout writes rews itself
+  CUDA_OK(cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return 0;
 }
 
 extern "C" int dial_plan_set_ensemble_adapt(dial_plan* p, int b, int on, float forget, float prune, const float* sigma, void* stream) {
   static const char* fn = "dial_plan_set_ensemble_adapt";
-  if (int rc = adapt_target(p, fn, b)) return rc;
+  if (int rc = need_ensemble(p, fn, 2)) return rc;
+  if (int rc = need_instance(p, fn, b)) return rc;
   if (on != 0 && on != 1) return fail(std::string(fn) + ": on must be 0 or 1, got " + std::to_string(on));
   const int K = p->n_ens, nv = p->hM.m.nv;
   if (on) {   // also rejects NaN and infinities
@@ -1150,30 +1134,23 @@ extern "C" int dial_plan_set_ensemble_adapt(dial_plan* p, int b, int on, float f
       cudaFree(p->pred_us); cudaFree(p->pred_qd); p->pred_us = p->pred_qd = nullptr;
       return fail(std::string(fn) + ": " + cudaGetErrorString(e));
     }
-    for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    p->mpc_graphs.clear();
+    drop_graphs(p);
   }
-  // stream-ordered copy out of the slot's pinned staging, rewritten only after its previous copy has run;
-  // the captured graphs hold the array's pointer and read the new setting at their next replay
-  cudaEvent_t& ev = p->adapt_ev[b];
-  e = ev ? cudaEventSynchronize(ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) {
-    EnsAdapt& a = p->hAdapt[b];
-    a.on = on;
+  e = p->adapt.put(b, [&](EnsAdapt* a) {   // off: the staged forget, prune and sigma are kept
+    a->on = on;
     if (on) {
-      a.forget = forget; a.prune = prune;
-      for (int j = 0; j < DIAL_MAXV; ++j) a.sigma[j] = j < nv ? sigma[j] : 1.f;
+      a->forget = forget; a->prune = prune;
+      for (int j = 0; j < DIAL_MAXV; ++j) a->sigma[j] = j < nv ? sigma[j] : 1.f;
     }
-    e = cudaMemcpyAsync(p->dAdapt + b, p->hAdapt + b, sizeof(EnsAdapt), cudaMemcpyHostToDevice, st);
-  }
-  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
+  }, st);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   return 0;
 }
 
 extern "C" int dial_plan_set_ensemble_belief(dial_plan* p, int b, const float* w, void* stream) {
   static const char* fn = "dial_plan_set_ensemble_belief";
-  if (int rc = adapt_target(p, fn, b)) return rc;
+  if (int rc = need_ensemble(p, fn, 2)) return rc;
+  if (int rc = need_instance(p, fn, b)) return rc;
   if (!w) return fail(std::string(fn) + ": null w");
   const int K = p->n_ens;
   double sum = 0.0;
@@ -1183,28 +1160,22 @@ extern "C" int dial_plan_set_ensemble_belief(dial_plan* p, int b, const float* w
   }
   if (!(sum > 0.0)) return fail(std::string(fn) + ": the weights must have a positive sum");
   cudaStream_t st = (cudaStream_t)stream;
-  cudaEvent_t& ev = p->belief_ev[b];
-  cudaError_t e = ev ? cudaEventSynchronize(ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) {
-    double* L = p->hL + (size_t)b * K;
-    float* W = p->hW + (size_t)b * K;
-    for (int k = 0; k < K; ++k) {
-      L[k] = w[k] > 0.f ? log((double)w[k] / sum) : -INFINITY;
-      W[k] = (float)exp(L[k]);
-    }
-    e = cudaMemcpyAsync(p->dL + (size_t)b * K, L, K * sizeof(double), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(p->dW + (size_t)b * K, W, K * sizeof(float), cudaMemcpyHostToDevice, st);
-  }
-  if (e == cudaSuccess) e = cudaEventRecord(ev, st);
+  cudaError_t e = p->belief_L.put(b, [&](double* L) {
+    for (int k = 0; k < K; ++k) L[k] = w[k] > 0.f ? log((double)w[k] / sum) : -INFINITY;
+  }, st);
+  const double* L = p->belief_L.h + (size_t)b * K;   // w from the L just staged
+  if (e == cudaSuccess) e = p->belief_w.put(b, [&](float* W) {
+    for (int k = 0; k < K; ++k) W[k] = (float)exp(L[k]);
+  }, st);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   return 0;
 }
 
 extern "C" int dial_plan_ensemble_belief(dial_plan* p, float* w, float* loglik, void* stream) {
-  if (int rc = adapt_target(p, "dial_plan_ensemble_belief", 0)) return rc;
+  if (int rc = need_ensemble(p, "dial_plan_ensemble_belief", 2)) return rc;
   const size_t n = (size_t)p->n_inst * p->n_ens * sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
-  if (w) CUDA_OK(cudaMemcpyAsync(w, p->dW, n, cudaMemcpyDeviceToDevice, st));
+  if (w) CUDA_OK(cudaMemcpyAsync(w, p->belief_w.d, n, cudaMemcpyDeviceToDevice, st));
   if (loglik) CUDA_OK(cudaMemcpyAsync(loglik, p->dEll, n, cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -1448,8 +1419,7 @@ extern "C" int dial_mpc_bind(dial_plan* p, const dial_mpc_buffers* b, const floa
   if (c.Ntotal != c.Nsample && !b->rews_all) return fail("dial_mpc_bind: sharded plans need rews_all [Ntotal+1]");
   if (p->n_inst > 1 && b->rews_all) return fail("dial_mpc_bind: rews_all must be NULL on a batched plan");
   const int n1 = c.Hnode + 1, nu = p->hM.m.nu;
-  for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-  p->mpc_graphs.clear();
+  drop_graphs(p);
   if (!p->mpc_Msh) CUDA_OK(cudaMalloc(&p->mpc_Msh, DIAL_MAXNODE * DIAL_MAXNODE * sizeof(float)));
   if (!p->mpc_Y1) CUDA_OK(cudaMalloc(&p->mpc_Y1, (size_t)p->n_inst * DIAL_MAXNODE * DIAL_MAXU * sizeof(float)));
   if (!p->mpc_key) CUDA_OK(cudaMalloc(&p->mpc_key, 2 * sizeof(uint32_t)));
@@ -1480,7 +1450,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     RolloutArgs A; memset(&A, 0, sizeof(A));
     A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart; A.counters_in = B.counters;
     A.nrows = ni * K; A.H = 1; A.mode = 0; A.us = p->pred_us;
-    A.rows_per_inst = K; A.rows_per_model = 1; A.models = p->dMembers;
+    A.rows_per_inst = K; A.rows_per_model = 1; A.models = p->members.d;
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = K; }
     A.qd = p->pred_qd;
     CUDA_OK(launch_rollout(p, A, 1, st));
@@ -1494,12 +1464,12 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     A.nrows = ni; A.H = 1; A.mode = 0; A.us = Y[cur]; A.rewss = B.reward;
     if (batched) { A.rows_per_inst = 1; A.us_row = n1 * nu; }
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
-    A.models = p->dModels;
+    A.models = p->models.d;
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
     CUDA_OK(launch_rollout(p, A, 1, st));
   }
   if (adapt) {   // each adapting instance's belief from its members' predictions and the observed qvel
-    ens_belief_kernel<<<ni, 32, 0, st>>>(p->pred_qd, B.qvel, p->dAdapt, K, p->hM.m.nv, p->dL, p->dW, p->dEll);
+    ens_belief_kernel<<<ni, 32, 0, st>>>(p->pred_qd, B.qvel, p->adapt.d, K, p->hM.m.nv, p->belief_L.d, p->belief_w.d, p->dEll);
     p->launches++;
     CUDA_OK(cudaGetLastError());
   }
@@ -1534,8 +1504,8 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     if (batched || p->n_ens > 0) A.rows_per_inst = K * (c.Nsample + 1);
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? K * (c.Nsample + 1) : 0; }
     // the planner's models: the members (n_ens >= 1; the plan's model until one is set), else the instances'
-    if (p->n_ens > 0) { A.rows_per_model = c.Nsample + 1; A.models = p->dMembers; }
-    else A.models = p->dModels;
+    if (p->n_ens > 0) { A.rows_per_model = c.Nsample + 1; A.models = p->members.d; }
+    else A.models = p->models.d;
     A.Ybar = Y[cur]; A.noise = noise;
     if (fused) A.rng_dev = B.rng; else A.key_dev = p->mpc_key;
     p->cur ^= 1;
@@ -1545,7 +1515,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     CUDA_OK(launch_rollout_any(p, A, st));
     if (K > 1) {   // each sample's score under its instance's risk measure (K = 1: the reward itself)
       const dim3 grid((c.Nsample + 1 + 255) / 256, ni);
-      ensemble_reduce_kernel<<<grid, 256, 0, st>>>(p->ens_rews, p->dRisk, p->dAdapt, p->dW, K, c.Nsample + 1, B.rews);
+      ensemble_reduce_kernel<<<grid, 256, 0, st>>>(p->ens_rews, p->risk.d, p->adapt.d, p->belief_w.d, K, c.Nsample + 1, B.rews);
       p->launches++;
       CUDA_OK(cudaGetLastError());
     }

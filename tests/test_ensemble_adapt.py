@@ -333,7 +333,7 @@ def test_prediction_rows_equal_single_instance_env_steps(lib):
 
 # ---- adapt specs and the CLI ---------------------------------------------------------------------------
 def test_adapt_setting():
-    from dial_mpc_b200.core.dial_core import adapt_setting, load_adapt, load_ensemble, load_prior, prior_setting
+    from dial_mpc_b200.core.dial_core import adapt_setting, load_ensemble, load_setting, prior_setting
     forget, prune, sigma = adapt_setting({"sigma": 0.1}, 4, 18)
     assert (forget, prune) == (1.0, 0.0) and sigma.dtype == f32 and sigma.shape == (18,) and (sigma == f32(0.1)).all()
     s = [0.1] * 6 + [0.5] * 12
@@ -344,8 +344,10 @@ def test_adapt_setting():
     spec = {"members": [{}, {}], "adapt": {"sigma": 0.2, "forget": 0.95}, "prior": [3, 1]}
     members, plant = load_ensemble(spec, env)
     assert len(members) == 2
-    assert load_adapt(spec, 2, env.sys.nv) == {"sigma": 0.2, "forget": 0.95} and load_prior(spec, 2) == [3.0, 1.0]
-    assert load_adapt({"members": [{}, {}]}, 2, 18) is None and load_prior({"members": [{}, {}]}, 2) is None
+    assert load_setting(spec, "adapt", 2, env.sys.nv) == {"sigma": 0.2, "forget": 0.95}
+    assert load_setting(spec, "prior", 2) == [3.0, 1.0]
+    assert load_setting({"members": [{}, {}]}, "adapt", 2, 18) is None
+    assert load_setting({"members": [{}, {}]}, "prior", 2) is None
 
 
 BAD_ADAPT = [

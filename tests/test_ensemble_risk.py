@@ -183,7 +183,7 @@ def test_ties_keep_member_order(lib):
 
 # ---- risk specs and the CLI ----------------------------------------------------------------------------
 def test_risk_setting():
-    from dial_mpc_b200.core.dial_core import load_ensemble, load_risk, risk_setting
+    from dial_mpc_b200.core.dial_core import load_ensemble, load_setting, risk_setting
     from tests.test_ensemble import _go2
     assert risk_setting({"aggregate": "mean"}, 4) == (MEAN, 1.0)
     assert risk_setting({"aggregate": "worst"}, 4) == (CVAR, 0.25)
@@ -193,7 +193,8 @@ def test_risk_setting():
     spec = {"members": [{}, {}], "risk": {"aggregate": "cvar", "alpha": 0.5}}
     members, plant = load_ensemble(spec, _go2())
     assert len(members) == 2 and plant is None
-    assert load_risk(spec, 2) == {"aggregate": "cvar", "alpha": 0.5} and load_risk({"members": [{}]}, 1) is None
+    assert load_setting(spec, "risk", 2) == {"aggregate": "cvar", "alpha": 0.5}
+    assert load_setting({"members": [{}]}, "risk", 1) is None
 
 
 BAD_RISK = [

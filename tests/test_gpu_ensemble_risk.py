@@ -193,6 +193,37 @@ def test_set_risk_between_replays_keeps_the_graph(built, monkeypatch):
     assert not torch.equal(base.buf["rews"][1], other.buf["rews"][1])
 
 
+def test_set_risk_twice_before_a_replay_takes_the_second(built):
+    """Two settings of instance 1 written back to back into one staging slot, with no synchronisation
+    between them, before a replay of the captured (2, 1) graph: the replay scores instance 1 by the second
+    setting, bit for bit the restatement on its member rewards, and instance 0 computes what it computes
+    without either call."""
+    from dial_mpc_b200.core.dial_core import DeviceLoop, MBDPI, risk_setting
+    env, _ = make_pair("unitree_go2_walk")
+    members = _members(env)
+    K = len(members)
+    args = _config("unitree_go2_walk", 64, 12, 4)
+    states, rngs, Y0 = _instances(env, 2, 4)
+    loop = DeviceLoop(MBDPI(args, env, n_instances=2, n_ensemble=K), states, rngs, Y0, ensemble=members)
+    for nd, es in SCHEDULE[:4]:       # (3, 1) eager, (2, 1) eager, captured, replayed
+        loop.step(nd, env_step=es)
+    torch.cuda.synchronize()
+    snap = _snapshot(loop)
+    loop.set_risk(1, WORST)
+    loop.set_risk(1, CVAR_HALF)
+    loop.step(2, env_step=1)
+    mr = loop.member_rewards()
+    torch.cuda.synchronize()
+    assert torch.equal(loop.buf["rews"], _scores(mr, [risk_setting(MEAN_SPEC, K), risk_setting(CVAR_HALF, K)]))
+    assert not torch.equal(loop.buf["rews"][1], _scores(mr[1:], [risk_setting(WORST, K)])[0])
+    base = DeviceLoop(MBDPI(args, env, n_instances=2, n_ensemble=K), states, rngs, Y0, ensemble=members)
+    _load(base, snap)
+    base.step(2, env_step=1)
+    torch.cuda.synchronize()
+    for k in KEYS:
+        assert torch.equal(loop.buf[k][0], base.buf[k][0]), k
+
+
 def test_risk_error_paths(built):
     from dial_mpc_b200 import random as drandom
     from dial_mpc_b200.core.dial_core import DeviceLoop, MBDPI
