@@ -47,6 +47,17 @@ def softmax_update(weights, Y0s, sigma, mu_0t):
     return torch.einsum("n,nij->ij", weights, Y0s), sigma
 
 
+def schedule_table(args: DialConfig, n: int, device) -> torch.Tensor:
+    """The annealing schedule [n, Hnode+1] of ``args`` (dial_core.py:259-261): the control sigma
+    ``horizon_diffuse_factor ** arange(Hnode+1)[::-1] * sigma_scale`` in fp64, rounded to fp32, times
+    ``traj_diffuse_factor ** arange(n)`` computed on ``device``.  Every table a plan uses is built here on
+    the plan's device: torch's CUDA and CPU ``pow`` may differ in the last bit."""
+    sigma = (args.horizon_diffuse_factor ** np.arange(args.Hnode + 1)[::-1]) * args.sigma_scale
+    sigma = torch.as_tensor(np.asarray(sigma, dtype=np.float32), device=device)
+    f = args.traj_diffuse_factor ** torch.arange(n, device=device, dtype=torch.float32)
+    return sigma[None, :] * f[:, None]
+
+
 class MBDPI:
     def __init__(self, args: DialConfig, env, rank: int = 0, world_size: int = 1, process_group=None,
                  compute_bars: bool = True, plan_factory=None, n_instances: int = 1, n_ensemble: int = 0):
@@ -279,8 +290,7 @@ class MBDPI:
 
     def schedule(self, n_diffuse: int) -> torch.Tensor:
         """``sigma_control * traj_diffuse_factor ** arange(n_diffuse)[:, None]`` (dial_core.py:259-261)."""
-        f = self.args.traj_diffuse_factor ** torch.arange(n_diffuse, device=self.device, dtype=torch.float32)
-        return self.sigma_control[None, :] * f[:, None]
+        return schedule_table(self.args, n_diffuse, self.device)
 
     # -- shift (dial_core.py:160-172) -------------------------------------------------------------------
     def shift(self, Y):
@@ -304,7 +314,8 @@ class DeviceLoop:
     the GPUs inside the kernels (peer-memory exchange), so no host collective sits in the step."""
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
-                 compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None):
+                 compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
+                 schedule=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -339,7 +350,13 @@ class DeviceLoop:
         their plant at every env step and score samples by the belief-weighted risk measure, one adapt spec
         for every instance or a list of B specs or None (``adapt_setting``: ``{"sigma": s, "forget": 1.0,
         "prune": 0.0}``).  ``prior``: the starting belief, K weights >= 0 with a positive sum for every
-        instance or B such lists (default uniform; ``set_belief``)."""
+        instance or B such lists (default uniform; ``set_belief``).
+
+        ``schedule``: each instance's own sampling schedule, one schedule spec for every instance or a list of
+        B specs or None (the plan's; ``schedule_setting``: any of ``temp_sample``, ``sigma_scale``,
+        ``horizon_diffuse_factor``, ``traj_diffuse_factor``, ``Ndiffuse``, ``Ndiffuse_init``).  Instance b then
+        computes bitwise what a single-instance loop on an MBDPI with b's updated DialConfig computes
+        (``set_schedule``, ``step``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -399,6 +416,15 @@ class DeviceLoop:
             for spec in adapt:
                 if spec is not None:
                     adapt_setting(spec, K, m.nv)
+        if schedule is not None:
+            schedule = self._per_instance("schedule", schedule, f"one schedule spec or a list of {B}",
+                                          lambda s: isinstance(s, (list, tuple)))
+            for spec in schedule:
+                if spec is not None:
+                    schedule_setting(spec, a)
+        # each instance's DialConfig, whether it has a table of its own, and the iteration limits last
+        # uploaded (None: no limits, every instance runs every iteration of a step)
+        self._cfg, self._own, self._lims = [a] * B, [False] * B, None
         ps = [s.pipeline_state for s in states]
         per = (lambda t: t[0]) if B == 1 else torch.stack   # one instance: the buffers keep their plain shapes
         counters = [[int(s.info.get("step", 0)), int(s.info.get("contact_stage", 0))] for s in states]
@@ -455,6 +481,9 @@ class DeviceLoop:
         for b, spec in enumerate(adapt or ()):
             if spec is not None:
                 self.set_adapt(b, spec)
+        for b, spec in enumerate(schedule or ()):
+            if spec is not None:
+                self.set_schedule(b, spec)
 
     @staticmethod
     def _model(env_or_sys):
@@ -580,12 +609,41 @@ class DeviceLoop:
         lead = (self.n_instances,) if self.n_instances > 1 else ()
         return self.plan.member_rewards(self.plan.empty(*lead, self.mbdpi.n_ensemble, self.mbdpi.Nlocal + 1))
 
-    def step(self, n_diffuse: Optional[int] = None, env_step=True) -> None:
+    def set_schedule(self, b: int, spec) -> None:
+        """Instance b's sampling schedule from the next ``step`` on: a schedule spec (``schedule_setting``),
+        or None for the plan's own.  Its noise table (``schedule_table`` of the updated DialConfig, max(Ndiffuse,
+        Ndiffuse_init) rows, on the plan's device) and temperature go to the plan with a stream-ordered copy on
+        the current stream.  The first schedule of a loop makes the next steps capture their graphs again,
+        later calls keep them."""
+        b = self._instance(b)
+        if spec is None:
+            if self._own[b]:
+                self.plan.set_instance_schedule(b, noise=None)
+            self._cfg[b], self._own[b] = self.mbdpi.args, False
+            return
+        cfg = schedule_setting(spec, self.mbdpi.args)
+        table = schedule_table(cfg, max(cfg.Ndiffuse, cfg.Ndiffuse_init), self.mbdpi.device)
+        self.plan.set_instance_schedule(b, float(np.float32(cfg.temp_sample)), table)
+        self._cfg[b], self._own[b] = cfg, True
+
+    def step(self, n_diffuse: Optional[int] = None, env_step=True, initial: bool = False) -> None:
         """One control step (asynchronous on the current stream).  env_step: True = env step + shift
-        + plan (the reference's main loop), False = plan only, 2 = shift + plan (state untouched)."""
-        n = self.mbdpi.args.Ndiffuse if n_diffuse is None else int(n_diffuse)
-        if n > self.n_diffuse_max:
+        + plan (the reference's main loop), False = plan only, 2 = shift + plan (state untouched).
+        ``n_diffuse`` None: each instance runs its own ``Ndiffuse`` (``Ndiffuse_init`` with ``initial``); an
+        int: every instance runs that many iterations, each with its own table and temperature.  The step's
+        graph runs the largest count; instances with fewer skip the rest (iteration limits, uploaded when the
+        counts need other limits than those the plan holds)."""
+        if n_diffuse is None:
+            counts = [c.Ndiffuse_init if initial else c.Ndiffuse for c in self._cfg]
+        else:
+            counts = [int(n_diffuse)] * self.n_instances
+        n = max(counts)
+        if any(c > self.n_diffuse_max for c, own in zip(counts, self._own) if not own):
             raise ValueError("n_diffuse exceeds the bound noise schedule")
+        lim = self._lims or [n] * self.n_instances    # no limits: every instance runs all n iterations
+        if any(min(n, l) != c for l, c in zip(lim, counts)):
+            self.plan.set_instance_iterations(counts)
+            self._lims = list(counts)
         stepping = env_step is True or env_step == 1
         if self._rand:
             # the env step (if any) runs at info["step"], the rollouts cover the Hsample+1 steps after it
@@ -771,6 +829,36 @@ def prior_setting(w, K: int):
     return a
 
 
+SCHEDULE_FIELDS = ("temp_sample", "sigma_scale", "horizon_diffuse_factor", "traj_diffuse_factor", "Ndiffuse",
+                   "Ndiffuse_init")
+
+
+def schedule_setting(spec, args: DialConfig) -> DialConfig:
+    """A schedule spec -> ``args`` with the spec's sampling fields replaced: a mapping of any of
+    ``SCHEDULE_FIELDS``; missing keys keep ``args``'s values.  ``temp_sample``, ``horizon_diffuse_factor`` and
+    ``traj_diffuse_factor`` are finite numbers > 0, ``sigma_scale`` a finite number >= 0, ``Ndiffuse`` and
+    ``Ndiffuse_init`` ints in 1..64.  Raises ValueError naming the bad key or value; the other DialConfig
+    fields (Nsample, Hsample, Hnode, update_method, ...) are shared by every instance of a plan."""
+    if not isinstance(spec, dict):
+        raise ValueError(f"a schedule spec maps any of {', '.join(SCHEDULE_FIELDS)}; got {spec!r}")
+    shared = {f.name for f in dataclasses.fields(DialConfig)} - set(SCHEDULE_FIELDS)
+    for key in spec:
+        if key in shared:
+            raise ValueError(f"{key} is shared by every instance of the plan; a schedule sets only "
+                             f"{', '.join(SCHEDULE_FIELDS)}")
+        if key not in SCHEDULE_FIELDS:
+            raise ValueError(f"unknown key {key!r} (a schedule takes {', '.join(SCHEDULE_FIELDS)})")
+    nmax = _capi.DEFINES["DIAL_MAXDIFFUSE"]
+    for key, v in spec.items():
+        if key.startswith("Ndiffuse"):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= nmax:
+                raise ValueError(f"{key} must be an int in 1..{nmax}, got {v!r}")
+        elif isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or \
+                not (v >= 0 if key == "sigma_scale" else (v > 0 and np.float32(v) > 0)):
+            raise ValueError(f"{key} must be a finite number {'>= 0' if key == 'sigma_scale' else '> 0'}, got {v!r}")
+    return dataclasses.replace(args, **{k: (int(v) if k.startswith("Ndiffuse") else v) for k, v in spec.items()})
+
+
 def load_setting(spec, key: str, K: int, nv: Optional[int] = None):
     """The ``risk``, ``adapt`` or ``prior`` entry ``key`` of an ``--ensemble`` file or an
     ``--instance-overrides`` mapping, checked for K members and nv dofs (``risk_setting``,
@@ -826,25 +914,28 @@ def load_ensemble(spec, env):
     return out, plant
 
 
-def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None):
+def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
+                  schedule=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
     ``ensemble``: K planning models shared by every instance (``DeviceLoop(..., ensemble=...)``), scored
     under ``risk`` (one risk spec or B of them, ``DeviceLoop(..., risk=...)``), adapting to the plant under
-    ``adapt`` from the belief ``prior`` (``DeviceLoop(..., adapt=..., prior=...)``)."""
+    ``adapt`` from the belief ``prior`` (``DeviceLoop(..., adapt=..., prior=...)``).  ``schedule``: B schedule
+    specs or None (``DeviceLoop(..., schedule=...)``); each instance runs its own Ndiffuse_init, then Ndiffuse."""
     mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
         rng, rng_reset = drandom.split(drandom.PRNGKey(seed=dial_config.seed + b))
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
-    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior)
+    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior,
+                      schedule=schedule)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
     for t in range(Nstep):
-        loop.step(dial_config.Ndiffuse_init if t == 0 else dial_config.Ndiffuse)
+        loop.step(initial=(t == 0))
         tt = torch.full((B, 1), float(t), device=mbdpi.device)
         rollout.append(torch.cat([tt, buf["qpos"], buf["qvel"], buf["ctrl"]], 1))
         rews.append(buf["reward"].clone())
@@ -887,7 +978,9 @@ def main():
                              "resets from PRNGKey(seed + b) and writes its output files under the prefix <time>_inst<b>")
     parser.add_argument("--instance-overrides", type=str, default=None, metavar="FILE.yaml",
                         help="a YAML list of one mapping of env-config fields per instance (--instances of them): "
-                             "instance b runs the config updated by mapping b (its own commands, gait, targets, ...)")
+                             "instance b runs the config updated by mapping b (its own commands, gait, targets, ...); "
+                             "a mapping may also set the instance's sampling schedule: temp_sample, sigma_scale, "
+                             "horizon_diffuse_factor, traj_diffuse_factor, Ndiffuse, Ndiffuse_init")
     parser.add_argument("--ensemble", type=str, default=None, metavar="FILE.yaml",
                         help="plan against an ensemble of models: a YAML mapping with 'members', a list of K sys "
                              "mappings ({} = the nominal model), optionally 'plant', one sys mapping applied to "
@@ -940,16 +1033,29 @@ def main():
         if not isinstance(overrides, list) or len(overrides) != args.instances:
             parser.error(f"--instance-overrides must hold a list of {args.instances} mappings (one per instance), "
                          f"got {len(overrides) if isinstance(overrides, list) else type(overrides).__name__}")
-        known = {f.name for f in dataclasses.fields(env_config_type)} | {"sys", "risk", "adapt"}
+        env_fields = {f.name for f in dataclasses.fields(env_config_type)}
+        # DialConfig fields: the sampling schedule (SCHEDULE_FIELDS), or fields shared by the plan, which
+        # schedule_setting rejects by name
+        dial_fields = {f.name for f in dataclasses.fields(DialConfig)} - env_fields
+        known = env_fields | dial_fields | {"sys", "risk", "adapt"}
         envs = []
         settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
         uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
+        schedule = [None] * args.instances
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk or adapt, got "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt "
+                             f"or the sampling fields {', '.join(SCHEDULE_FIELDS)}, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
+            spec = {k: ov.pop(k) for k in list(ov) if k in dial_fields}
+            if spec:
+                try:
+                    schedule_setting(spec, dial_config)
+                except ValueError as e:
+                    parser.error(f"--instance-overrides entry {b}: {e}")
+                schedule[b] = spec
             sys_ov = ov.pop("sys", None)
             for key in ("risk", "adapt"):
                 if ov.get(key) is not None:
@@ -986,7 +1092,8 @@ def main():
         if args.instance_overrides is not None and any(a is not None for a in settings["adapt"]):
             adapt = settings["adapt"]
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
-                      ensemble=members, risk=risk, adapt=adapt, prior=prior)
+                      ensemble=members, risk=risk, adapt=adapt, prior=prior,
+                      schedule=schedule if args.instance_overrides is not None and any(schedule) else None)
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)

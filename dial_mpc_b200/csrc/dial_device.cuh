@@ -139,6 +139,24 @@ static_assert(DIAL_TASK_AT(vel_cmd) && DIAL_TASK_AT(ang_cmd) && DIAL_TASK_AT(pos
 
 HD const dial_task& plan_task(const dial_plan_desc& c) { return *reinterpret_cast<const dial_task*>(c.vel_cmd); }
 
+// Instance b's own sampling schedule (dial_plan_set_instance_schedule): while `on`, its rollout rows and
+// its update take noise row `iter` of its table and its temperature instead of the bound noise and the
+// plan's temp_sample.
+struct alignas(16) InstSchedule {
+  int32_t on;
+  float temp;
+  int32_t n_rows;   // rows of `noise` set (1..DIAL_MAXDIFFUSE)
+  int32_t pad;
+  float noise[DIAL_MAXDIFFUSE][DIAL_MAXNODE];
+};
+// the noise row of instance `inst` at diffusion iteration `iter`: its own, or `bound` (the plan's row)
+HD const float* schedule_noise(const InstSchedule* S, int inst, int iter, const float* bound) {
+  return (S && S[inst].on) ? S[inst].noise[iter] : bound;
+}
+// instance `inst` runs diffusion iteration `iter` of a control step (dial_plan_set_instance_iterations;
+// no limits: every instance runs every iteration)
+HD bool schedule_runs(const int32_t* lim, int inst, int iter) { return !lim || iter < lim[inst]; }
+
 // arguments of one rollout launch
 struct RolloutArgs {
   int32_t nrows;        // sample rows rolled by this launch
@@ -198,10 +216,30 @@ struct RolloutArgs {
   // rows_per_model = Nsample+1 rows each (rows_per_inst = K * rows_per_model); a member's row i takes
   // sample i's perturbation, and `models` holds one model per member block.  0: one block per instance.
   int32_t rows_per_model;
+  // per-instance sampling schedules (mode 1 of dial_mpc_step): `iter` is the diffusion iteration of the
+  // launch; `sched` [instances] or null (schedule_noise); `iter_lim` [instances] or null: the rows of
+  // instance b run only while iter < iter_lim[b], so the host then launches instance-aligned CTAs (the
+  // layout of `models`) and a skipped instance's CTAs exit whole (cta_instance)
+  const InstSchedule* sched;
+  const int32_t* iter_lim;
+  int32_t iter;
 };
 
 // rows of one model slot of `models`: a member block of an ensemble plan, else an instance
 HD int model_rows(const RolloutArgs& A) { return A.rows_per_model > 0 ? A.rows_per_model : A.rows_per_inst; }
+
+// The instance every row of CTA `cta` belongs to under rollout_kernel's row mapping for `wpc` warps per
+// CTA, or -1 when the CTA's rows straddle two instances (possible only without `models`).  With `models`
+// a CTA holds rows of one model slot: slot s of an ensemble plan is member s % K of instance s / K.
+HD int cta_instance(const RolloutArgs& A, int cta, int wpc) {
+  if (A.rows_per_inst <= 0) return 0;
+  if (A.models && model_rows(A) > 0) {
+    const int rps = model_rows(A), slot = cta / ((rps + wpc - 1) / wpc);
+    return (int)((int64_t)slot * rps / A.rows_per_inst);
+  }
+  const int r0 = cta * wpc, r1 = (r0 + wpc < A.nrows ? r0 + wpc : A.nrows) - 1;
+  return r0 / A.rows_per_inst == r1 / A.rows_per_inst ? r0 / A.rows_per_inst : -1;
+}
 
 // ---------------------------------------------------------------------------------
 // Risk measure of an ensemble plan (dial_plan_set_ensemble_risk): how the K >= 2 member rewards of one
@@ -3213,6 +3251,7 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
     const uint32_t ntot = (uint32_t)c.Ntotal * (uint32_t)Hn1 * (uint32_t)nu;
     uint32_t key0 = A.key_dev ? A.key_dev[2 * inst] : A.key0, key1 = A.key_dev ? A.key_dev[2 * inst + 1] : A.key1;
     if (A.rng_dev) split_key(A.rng_dev[2 * inst], A.rng_dev[2 * inst + 1], key0, key1);
+    const float* noise = schedule_noise(A.sched, inst, A.iter, A.noise);
 #pragma unroll
     for (int k = 0; k < DIAL_MAXNODE; ++k) {
       if (k < Hn1) {
@@ -3221,7 +3260,7 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
         if (!is_mean && k > 0) {
           uint32_t idx = (gidx * (uint32_t)Hn1 + (uint32_t)k) * (uint32_t)nu + (uint32_t)lane;
           float e = A.eps ? A.eps[idx] : jax_normal_legacy(key0, key1, idx, ntot);
-          y = e * A.noise[k] + yb;
+          y = e * noise[k] + yb;
         }
         Y[k] = fminf(fmaxf(y, -1.f), 1.f);
       }

@@ -362,7 +362,9 @@ __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __res
                                                                uint32_t* __restrict__ rng, const float* __restrict__ Ybar,
                                                                const float* __restrict__ noise, int Ntotal, int Hn1, int nu,
                                                                float* __restrict__ partial, unsigned int* __restrict__ counter,
-                                                               float* __restrict__ Ybar_out) {
+                                                               float* __restrict__ Ybar_out, const InstSchedule* __restrict__ sched,
+                                                               const int32_t* __restrict__ iter_lim, int iter,
+                                                               const float* weights_prev) {
   __shared__ __align__(8) float red[4 * 32];
   __shared__ float acc[YBAR_THREADS];
   __shared__ bool is_last;
@@ -371,6 +373,16 @@ __global__ void __launch_bounds__(YBAR_THREADS) update_kernel(const float* __res
     const size_t b = blockIdx.y, ne1 = (size_t)Hn1 * nu;
     rews += b * n; weights += b * n; rng += 2 * b; Ybar += b * ne1; Ybar_out += b * ne1;
     partial += b * gridDim.x * (ne1 + 1); counter += b;
+    if (!schedule_runs(iter_lim, b, iter)) {
+      // instance b is past its iteration limit: its knots and its last iteration's weights move on to this
+      // iteration's buffers unchanged; rng and counter stay as they are
+      if (blockIdx.x == 0)
+        for (int i = tid; i < (int)ne1; i += blockDim.x) Ybar_out[i] = Ybar[i];
+      if (weights_prev != weights - b * n)
+        for (int i = blockIdx.x * blockDim.x + tid; i < n; i += gridDim.x * blockDim.x) weights[i] = weights_prev[b * n + i];
+      return;
+    }
+    if (sched && sched[b].on) { temp = sched[b].temp; noise = sched[b].noise[iter]; }
   }
   if (X.mbox) {
     const uint32_t seq = *X.seq, buf = seq & 1u;
@@ -500,14 +512,16 @@ struct TrajArgs {
 
 // (32 registers: one CTA fits beside the 448-thread rollout CTA of the next iteration, which the bars overlap)
 // BATCH = false (single-instance plans) compiles to the instance-free code: the bars of a plain plan
-// pay nothing for the instance dimension
+// pay nothing for the instance dimension.  BATCH only: an instance past its iteration limit at iteration
+// `iter` (schedule_runs over iter_lim) keeps its bars.  (Outside TrajArgs: the instance-free code keeps
+// its parameter layout.)
 template <bool BATCH>
-__global__ void __launch_bounds__(256, 8) trajbar_partial_kernel(const TrajArgs T) {
+__global__ void __launch_bounds__(256, 8) trajbar_partial_kernel(const TrajArgs T, const int32_t* __restrict__ iter_lim, int iter) {
   const int chunk = blockIdx.y, arr = BATCH ? blockIdx.z % 3 : blockIdx.z, inst = BATCH ? blockIdx.z / 3 : 0;
   const int ncol = arr == 0 ? T.ncol[0] : (arr == 1 ? T.ncol[1] : T.ncol[2]), len = T.H * ncol;
   const int coloff = arr == 0 ? T.coloff[0] : (arr == 1 ? T.coloff[1] : T.coloff[2]);
   const int j = blockIdx.x * 256 + threadIdx.x;
-  if (blockIdx.x * 256 >= len) return;
+  if (blockIdx.x * 256 >= len || (BATCH && !schedule_runs(iter_lim, inst, iter))) return;
   const float* __restrict__ traj = (arr == 0 ? T.traj[0] : (arr == 1 ? T.traj[1] : T.traj[2])) + (size_t)inst * T.inst_rows * len;
   const float* wts = BATCH ? T.weights + (size_t)inst * (T.mean_weight_index + 1) : T.weights;
   const int per = (T.nrows + TB_CHUNKS - 1) / TB_CHUNKS;
@@ -539,8 +553,9 @@ __global__ void __launch_bounds__(256, 8) trajbar_partial_kernel(const TrajArgs 
 }
 
 template <bool BATCH>
-__global__ void __launch_bounds__(128, 8) trajbar_final_kernel(const TrajArgs T) {
+__global__ void __launch_bounds__(128, 8) trajbar_final_kernel(const TrajArgs T, const int32_t* __restrict__ iter_lim, int iter) {
   const int t = blockIdx.x, inst = BATCH ? blockIdx.y : 0;
+  if (BATCH && !schedule_runs(iter_lim, inst, iter)) return;
   const float* partial = T.partial + (size_t)inst * TB_CHUNKS * T.H * T.coltot;
   for (int col = threadIdx.x; col < T.coltot; col += blockDim.x) {
     float s = 0.f;
@@ -562,9 +577,10 @@ __global__ void __launch_bounds__(128, 8) trajbar_final_kernel(const TrajArgs T)
 // (ens_risk_reduce_weighted) over its belief w [B][K].
 __global__ void __launch_bounds__(256) ensemble_reduce_kernel(const float* __restrict__ r, const EnsRisk* __restrict__ risk,
                                                               const EnsAdapt* __restrict__ adapt, const float* __restrict__ belief,
-                                                              int K, int n1, float* __restrict__ rews) {
+                                                              int K, int n1, float* __restrict__ rews,
+                                                              const int32_t* __restrict__ iter_lim, int iter) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
-  if (i >= n1) return;
+  if (i >= n1 || !schedule_runs(iter_lim, b, iter)) return;   // a skipped instance keeps its scores
   const EnsRisk R = risk[b];
   const float* rb = r + (size_t)b * K * n1 + i;
   rews[(size_t)b * n1 + i] = adapt[b].on ? ens_risk_reduce_weighted(rb, (size_t)n1, K, R, belief + (size_t)b * K, adapt[b].prune)
@@ -697,6 +713,11 @@ struct dial_plan {
   float* dEll = nullptr;
   float* pred_us = nullptr;
   float* pred_qd = nullptr;
+  // per-instance sampling schedules (dial_plan_set_instance_schedule): [n_inst] slots; and the iteration
+  // limits (dial_plan_set_instance_iterations): one slot of n_inst counts.  Each is allocated by its first
+  // call; the staging `h` mirrors what the device holds
+  Staged<InstSchedule> sched;
+  Staged<int32_t> lims;
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -964,7 +985,7 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   cudaFree(p->xch.bars_partial);
   cudaFree(p->mpc_Msh); cudaFree(p->mpc_Y1); cudaFree(p->mpc_key);
   p->models.release(); p->members.release(); p->risk.release();
-  p->adapt.release(); p->belief_L.release(); p->belief_w.release();
+  p->adapt.release(); p->belief_L.release(); p->belief_w.release(); p->sched.release(); p->lims.release();
   cudaFree(p->ens_rews); cudaFree(p->dEll); cudaFree(p->pred_us); cudaFree(p->pred_qd);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
@@ -1180,6 +1201,71 @@ extern "C" int dial_plan_ensemble_belief(dial_plan* p, float* w, float* loglik, 
   return 0;
 }
 
+// The plans the per-instance schedule calls accept: not sharded, within the fused update's size.
+static int need_schedulable(const dial_plan* p, const char* fn) {
+  const dial_plan_desc& c = p->hP.c;
+  if (c.Ntotal != c.Nsample) return fail(std::string(fn) + ": sharded plans (Ntotal != Nsample) share the plan's schedule");
+  if (c.Ntotal + 1 > (1 << 17)) return fail(std::string(fn) + ": needs Ntotal + 1 <= 131072 (the fused update)");
+  return 0;
+}
+
+extern "C" int dial_plan_set_instance_schedule(dial_plan* p, int b, float temp, int n_rows, const float* noise, void* stream) {
+  static const char* fn = "dial_plan_set_instance_schedule";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (int rc = need_instance(p, fn, b)) return rc;
+  if (int rc = need_schedulable(p, fn)) return rc;
+  const int n1 = p->hP.c.Hnode + 1;
+  if (noise) {   // (the comparisons also reject NaN)
+    if (!(temp > 0.f && temp <= FLT_MAX)) return fail(std::string(fn) + ": temp must be finite and > 0, got " + fmt_g(temp));
+    if (n_rows < 1 || n_rows > DIAL_MAXDIFFUSE)
+      return fail(std::string(fn) + ": n_rows " + std::to_string(n_rows) + " out of range (1.." DIAL_STR(DIAL_MAXDIFFUSE) ")");
+    for (int i = 0; i < n_rows * n1; ++i)
+      if (!(fabsf(noise[i]) <= FLT_MAX))
+        return fail(std::string(fn) + ": noise[" + std::to_string(i / n1) + "][" + std::to_string(i % n1) + "] is not finite, got " + fmt_g(noise[i]));
+  } else if (!p->sched.d) {
+    return 0;   // no instance has a schedule: b already plans with the plan's own
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (!p->sched.d) {
+    // first call: the graphs captured so far launch without the schedules
+    if ((e = p->sched.allocate(p->n_inst, 1, InstSchedule{})) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+    drop_graphs(p);
+  }
+  e = p->sched.put(b, [&](InstSchedule* S) {
+    memset(S, 0, sizeof(*S));
+    if (!noise) return;
+    S->on = 1; S->temp = temp; S->n_rows = n_rows;
+    for (int r = 0; r < n_rows; ++r)
+      for (int k = 0; k < n1; ++k) S->noise[r][k] = noise[r * n1 + k];
+  }, st);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int dial_plan_set_instance_iterations(dial_plan* p, const int32_t* n_iter, void* stream) {
+  static const char* fn = "dial_plan_set_instance_iterations";
+  if (!p || !n_iter) return fail(std::string(fn) + ": null argument");
+  if (int rc = need_schedulable(p, fn)) return rc;
+  for (int b = 0; b < p->n_inst; ++b)
+    if (n_iter[b] < 0 || n_iter[b] > DIAL_MAXDIFFUSE)
+      return fail(std::string(fn) + ": n_iter[" + std::to_string(b) + "] = " + std::to_string(n_iter[b]) + " out of range (0.." DIAL_STR(DIAL_MAXDIFFUSE) ")");
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (!p->lims.d) {
+    // first call: the rollout launches need instance-aligned CTAs from now on, the layout of per-instance
+    // (or member) models, so those slots are allocated too, each holding the plan's model until one is set
+    Staged<DevModel>& M = p->n_ens > 0 ? p->members : p->models;
+    if (!M.d) e = M.allocate((size_t)p->n_inst * (p->n_ens > 0 ? p->n_ens : 1), 1, p->hM);
+    if (e == cudaSuccess) e = p->lims.allocate(1, p->n_inst, DIAL_MAXDIFFUSE);
+    if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+    drop_graphs(p);
+  }
+  e = p->lims.put(0, [&](int32_t* L) { memcpy(L, n_iter, sizeof(int32_t) * p->n_inst); }, st);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
 extern "C" int dial_plan_get_task(const dial_plan* p, dial_task* out) {
   if (!p || !out) return fail("dial_plan_get_task: null argument");
   const dial_task& t = plan_task(p->hP.c);   // the plan's task block (include/dial_b200.h)
@@ -1268,13 +1354,18 @@ extern "C" int dial_reverse_update_x(dial_plan* p, const float* eps, const uint3
 
 // The fused update of every instance of the plan: the one launch of update_kernel, used by the
 // control-step graph (mpc_enqueue) and by dial_reverse_update_fused.  Grid upd_grid x n_inst over the
-// plan's partials and per-instance counters.
+// plan's partials and per-instance counters.  The control-step graph passes the schedules, the limits, the
+// iteration `iter` and the previous iteration's weights buffer `weights_prev` (what a skipped instance
+// forwards); dial_reverse_update_fused passes none.
 static int launch_update(dial_plan* p, const float* rews, float* weights, const XchWait& X, uint32_t* rng,
-                         const float* Ybar, const float* noise, float* Ybar_out, cudaStream_t st) {
+                         const float* Ybar, const float* noise, float* Ybar_out, cudaStream_t st,
+                         const InstSchedule* sched = nullptr, const int32_t* iter_lim = nullptr, int iter = 0,
+                         const float* weights_prev = nullptr) {
   const dial_plan_desc& c = p->hP.c;
   update_kernel<<<dim3(p->upd_grid, p->n_inst), YBAR_THREADS, 0, st>>>(rews, c.Ntotal + 1, c.temp_sample, weights, X, rng, Ybar,
                                                                      noise, c.Ntotal, c.Hnode + 1, p->hM.m.nu, p->partial,
-                                                                     p->counter, Ybar_out);
+                                                                     p->counter, Ybar_out, sched, iter_lim, iter,
+                                                                     weights_prev ? weights_prev : weights);
   p->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
@@ -1290,9 +1381,10 @@ extern "C" int dial_reverse_update_fused(dial_plan* p, const float* rews, uint32
   return launch_update(p, rews, weights, X, rng, Ybar, noise_scale, Ybar_out, (cudaStream_t)stream);
 }
 
-// the bars of every instance of the plan (the control-step graph; the public call below is single-instance)
+// the bars of every instance of the plan (the control-step graph; the public call below is single-instance);
+// with iteration limits (iter_lim, iteration `iter`) the instance-indexed kernels run, also for one instance
 static int enqueue_trajbar(dial_plan* p, const float* weights, int rank, float* qbar, float* qdbar, float* xbar,
-                           cudaStream_t st) {
+                           cudaStream_t st, const int32_t* iter_lim = nullptr, int iter = 0) {
   const dial_plan_desc& c = p->hP.c;
   const dial_model_desc& m = p->hM.m;
   const float* w = weights ? weights : p->weights;
@@ -1311,12 +1403,13 @@ static int enqueue_trajbar(dial_plan* p, const float* weights, int rank, float* 
   T.mean_weight_index = c.Ntotal; T.include_mean = rank == 0 ? 1 : 0; T.partial = p->tb_partial;
   const int maxlen = H * (T.ncol[2] > T.ncol[0] ? T.ncol[2] : T.ncol[0]);   // nq = nv + 1 > nv always
   const dim3 g1((maxlen + 255) / 256, TB_CHUNKS, 3 * p->n_inst), g2(H, p->n_inst);
-  if (p->n_inst > 1) trajbar_partial_kernel<true><<<g1, 256, 0, st>>>(T);
-  else trajbar_partial_kernel<false><<<g1, 256, 0, st>>>(T);
+  const bool batch = p->n_inst > 1 || iter_lim;
+  if (batch) trajbar_partial_kernel<true><<<g1, 256, 0, st>>>(T, iter_lim, iter);
+  else trajbar_partial_kernel<false><<<g1, 256, 0, st>>>(T, nullptr, 0);
   p->launches++;
   CUDA_OK(cudaGetLastError());
-  if (p->n_inst > 1) trajbar_final_kernel<true><<<g2, 128, 0, st>>>(T);
-  else trajbar_final_kernel<false><<<g2, 128, 0, st>>>(T);
+  if (batch) trajbar_final_kernel<true><<<g2, 128, 0, st>>>(T, iter_lim, iter);
+  else trajbar_final_kernel<false><<<g2, 128, 0, st>>>(T, nullptr, 0);
   p->launches++;
   CUDA_OK(cudaGetLastError());
   if (xsum) {
@@ -1507,6 +1600,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     if (p->n_ens > 0) { A.rows_per_model = c.Nsample + 1; A.models = p->members.d; }
     else A.models = p->models.d;
     A.Ybar = Y[cur]; A.noise = noise;
+    A.sched = p->sched.d; A.iter_lim = p->lims.d; A.iter = i;
     if (fused) A.rng_dev = B.rng; else A.key_dev = p->mpc_key;
     p->cur ^= 1;
     A.rews = K > 1 ? p->ens_rews : B.rews; A.q = p->traj_q[p->cur]; A.qd = p->traj_qd[p->cur]; A.xpos = p->traj_x[p->cur];
@@ -1515,14 +1609,16 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     CUDA_OK(launch_rollout_any(p, A, st));
     if (K > 1) {   // each sample's score under its instance's risk measure (K = 1: the reward itself)
       const dim3 grid((c.Nsample + 1 + 255) / 256, ni);
-      ensemble_reduce_kernel<<<grid, 256, 0, st>>>(p->ens_rews, p->risk.d, p->adapt.d, p->belief_w.d, K, c.Nsample + 1, B.rews);
+      ensemble_reduce_kernel<<<grid, 256, 0, st>>>(p->ens_rews, p->risk.d, p->adapt.d, p->belief_w.d, K, c.Nsample + 1, B.rews,
+                                                   p->lims.d, i);
       p->launches++;
       CUDA_OK(cudaGetLastError());
     }
     float* w = wts[i & 1];
     XchWait X = xch_wait_args(p, B.rews_all);
     if (fused) {
-      int rc = launch_update(p, B.rews, w, X, B.rng, Y[cur], noise, Y[cur ^ 1], st);
+      int rc = launch_update(p, B.rews, w, X, B.rng, Y[cur], noise, Y[cur ^ 1], st, p->sched.d, p->lims.d, i,
+                             wts[i > 0 ? (i - 1) & 1 : 0]);
       if (rc) return rc;
     } else {
       weights_kernel<<<1, 1024, 0, st>>>(B.rews, c.Ntotal + 1, c.temp_sample, w, X);
@@ -1537,7 +1633,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     if (bars) {
       CUDA_OK(cudaEventRecord(p->ev_main[i & 1], st));
       CUDA_OK(cudaStreamWaitEvent(p->side, p->ev_main[i & 1], 0));
-      int rc = enqueue_trajbar(p, w, p->xch.on ? p->xch.rank : 0, B.qbar, B.qdbar, B.xbar, p->side);
+      int rc = enqueue_trajbar(p, w, p->xch.on ? p->xch.rank : 0, B.qbar, B.qdbar, B.xbar, p->side, p->lims.d, i);
       if (rc) return rc;
       CUDA_OK(cudaEventRecord(p->ev_side[i & 1], p->side));
     }
@@ -1559,6 +1655,16 @@ extern "C" int dial_mpc_step(dial_plan* p, int n_diffuse, int env_step, void* st
   if (env_step < 0 || env_step > 2) return fail("dial_mpc_step: env_step must be 0 (plan only), 1 (env step + shift) or 2 (shift only)");
   // batched plans use the fused update only (plan creation guarantees Nsample + 1 <= 2^17)
   if (p->n_inst > 1 && getenv("DIAL_NO_FUSED_UPDATE")) return fail("dial_mpc_step: batched plans need the fused update (unset DIAL_NO_FUSED_UPDATE)");
+  if ((p->sched.d || p->lims.d) && getenv("DIAL_NO_FUSED_UPDATE"))
+    return fail("dial_mpc_step: per-instance schedules and iteration limits need the fused update (unset DIAL_NO_FUSED_UPDATE)");
+  // every instance with its own table has a row for each iteration it runs (the staging mirrors the device)
+  for (int b = 0; p->sched.d && b < p->n_inst; ++b) {
+    const InstSchedule& S = p->sched.h[b];
+    const int runs = p->lims.d && p->lims.h[b] < n_diffuse ? p->lims.h[b] : n_diffuse;
+    if (S.on && runs > S.n_rows)
+      return fail("dial_mpc_step: instance " + std::to_string(b) + " runs " + std::to_string(runs) +
+                  " diffusion iterations, its schedule has " + std::to_string(S.n_rows) + " rows");
+  }
   cudaStream_t st = (cudaStream_t)stream;
   dial_plan::MpcGraph* g = nullptr;
   for (auto& e : p->mpc_graphs) if (e.n_diffuse == n_diffuse && e.env_step == env_step) g = &e;

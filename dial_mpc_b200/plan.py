@@ -141,6 +141,27 @@ class Plan:
             assert t is None or t.numel() == n, f"need {n} elements, got {tuple(t.shape)}"
         self._check(self.lib.dial_plan_ensemble_belief(self.handle, _ptr(w), _ptr(loglik), _stream()))
 
+    def set_instance_schedule(self, b: int, temp: float = 1.0, noise=None) -> None:
+        """Instance b's sampling schedule from the next ``mpc_step`` on: softmax temperature ``temp`` and
+        noise rows ``noise`` [n_rows, Hnode+1] (fp32, n_rows in 1..64); ``noise=None`` returns it to the
+        plan's temp_sample and the bound noise.  A stream-ordered copy on the current stream; the first
+        call on a plan makes the next steps capture their graphs again (``dial_plan_set_instance_schedule``)."""
+        if noise is None:
+            self._check(self.lib.dial_plan_set_instance_schedule(self.handle, int(b), float(temp), 0, None, _stream()))
+            return
+        a = np.ascontiguousarray(noise.cpu().numpy() if isinstance(noise, torch.Tensor) else noise, dtype=np.float32)
+        assert a.ndim == 2 and a.shape[1] == self.Hn + 1, f"noise must be [n_rows, {self.Hn + 1}], got {a.shape}"
+        self._check(self.lib.dial_plan_set_instance_schedule(self.handle, int(b), float(temp), int(a.shape[0]),
+                                                             a.ctypes.data_as(C.POINTER(C.c_float)), _stream()))
+
+    def set_instance_iterations(self, n_iter) -> None:
+        """Each instance's iteration limit (one int in 0..64 per instance) from the next ``mpc_step`` on: instance
+        b runs min(n_diffuse, n_iter[b]) diffusion iterations (``dial_plan_set_instance_iterations``)."""
+        a = np.ascontiguousarray(n_iter, dtype=np.int32).ravel()
+        assert a.size == max(self.desc.n_inst, 1), f"need {max(self.desc.n_inst, 1)} limits, got {a.size}"
+        self._check(self.lib.dial_plan_set_instance_iterations(self.handle, a.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                               _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

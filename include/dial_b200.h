@@ -43,6 +43,7 @@ extern "C" {
 #define DIAL_MAXUSER 64 /* user constants of a custom reward */
 #define DIAL_MAXRANK 8  /* GPUs of one NVLink domain sharing the samples */
 #define DIAL_MAXENS 16  /* planning models (ensemble members) of one instance */
+#define DIAL_MAXDIFFUSE 64 /* diffusion iterations of one control step (dial_mpc_step) */
 #define DIAL_IPC_HANDLE_BYTES 64
 
 /* environments (reward functors fused into the rollout kernel) */
@@ -464,6 +465,34 @@ int dial_plan_set_ensemble_belief(dial_plan* plan, int b, const float* w, void* 
 /* The current belief w [dev][n_inst, K] and the l [dev][n_inst, K] of each instance's last update (0
  * before the first), each nullable; stream-ordered copies on `stream`.  Fails on a plan with n_ens < 2. */
 int dial_plan_ensemble_belief(dial_plan* plan, float* w, float* loglik, void* stream);
+
+/* Per-instance sampling schedules of dial_mpc_step: instance b's softmax temperature, its noise rows and
+ * how many diffusion iterations it runs.  In dial_mpc_step(plan, n, env_step), instance b runs the
+ * iterations i < min(n, n_b) (n_b: its iteration limit, n when no limits are set), each with row i of its
+ * own table and its own temperature when it has a schedule, else with the bound noise row i and the plan's
+ * temp_sample.  In the iterations i >= min(n, n_b) instance b does nothing: none of its rollout rows run,
+ * its rng is not split, and Y, rews, qbar / qdbar / xbar and the weights of the last iteration keep what its
+ * last iteration produced (n_b = 0: it is only env-stepped and shifted).  Instance b then computes bitwise
+ * what a single-instance plan with temp_sample = temp and the bound noise = its table computes with
+ * dial_mpc_step(plan, min(n, n_b), env_step).  Every member of an ensemble instance uses the instance's
+ * rows.  A plan on which neither call is ever made launches what it launched before.
+ * Both calls copy stream-ordered on `stream` out of plan-owned pinned staging, so they may be issued
+ * between dial_mpc_step calls.  The first call of each allocates its array and drops the captured graphs;
+ * later calls keep them and take effect at the next replay.  Both reject sharded plans
+ * (Ntotal != Nsample) and plans past the fused update (Ntotal + 1 > 131072).  dial_mpc_step fails, naming
+ * the instance, when an instance with its own table would run more iterations than the table has rows,
+ * and fails with DIAL_NO_FUSED_UPDATE set once either call has been made. */
+
+/* Instance b's schedule: temp finite and > 0, noise [host][n_rows][Hn+1] finite with n_rows in 1..64.
+ * noise == NULL returns instance b to the plan's temp_sample and the bound noise (temp and n_rows are then
+ * ignored).  Fails for b out of range and for a bad argument, which the error names. */
+int dial_plan_set_instance_schedule(dial_plan* plan, int b, float temp, int n_rows, const float* noise, void* stream);
+
+/* The iteration limits n_iter [host][n_inst], each in 0..64.  While limits are set, the rollout launches
+ * give each instance CTAs of its own (the layout of per-instance models, whose slots the first call
+ * allocates with the plan's model when no model was set), so a skipped instance's CTAs exit whole; an
+ * instance's results do not depend on the launch shape. */
+int dial_plan_set_instance_iterations(dial_plan* plan, const int32_t* n_iter, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops

@@ -77,6 +77,9 @@ def main():
     ap.add_argument("--env-step", type=int, default=2, choices=(1, 2),
                     help="the timed steps' env_step: 2 (shift + plan, the default) or 1 (env step + shift + plan; "
                          "--adapt runs its predictions and belief update in env steps only)")
+    ap.add_argument("--schedules", default=None, metavar="FILE.yaml",
+                    help="a YAML list of one schedule spec per instance (null: the config's; DeviceLoop(..., "
+                         "schedule=...)); each instance then runs its own Ndiffuse")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
@@ -92,7 +95,7 @@ def main():
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop
+    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, schedule_setting
 
     B, b = args.instances, BASELINE[args.config]
     cfg = dial_config(args.config, world=1)
@@ -130,21 +133,34 @@ def main():
         adapt = adapt_spec(args.adapt) if args.adapt is not None else None
     except ValueError as e:
         ap.error(f"--adapt {args.adapt}: {e}")
+    schedule, n_diffuse = None, [cfg.Ndiffuse] * B
+    if args.schedules is not None:
+        import yaml
+        schedule = yaml.safe_load(open(args.schedules))
+        if not isinstance(schedule, list) or len(schedule) != B:
+            ap.error(f"--schedules must hold a list of {B} schedule specs (one per instance)")
+        try:
+            n_diffuse = [schedule_setting(s or {}, cfg).Ndiffuse for s in schedule]
+        except ValueError as e:
+            ap.error(f"--schedules {args.schedules}: {e}")
     if B == 1:
-        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt)
+        loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt,
+                          schedule=schedule)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
-                          ensemble=members, risk=risk, adapt=adapt)
+                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule)
     es = args.env_step
+    # without --schedules every step runs the config's Ndiffuse on every instance, as before
+    nd = None if schedule is not None else cfg.Ndiffuse
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=mb.device)
     for _ in range(max(args.warmup, 3)):
-        loop.step(cfg.Ndiffuse, env_step=es)
+        loop.step(nd, env_step=es)
     torch.cuda.synchronize()
     if args.profile_kernels:
         from torch.profiler import ProfilerActivity, profile
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(args.steps):
-                loop.step(cfg.Ndiffuse, env_step=es)
+                loop.step(nd, env_step=es)
             torch.cuda.synchronize()
         acc, rollouts = {}, []
         for ev in prof.events():
@@ -157,7 +173,7 @@ def main():
                     n, tot = acc.get(key, (0, 0.0))
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
         # the rollout launches of one step in order: [member prediction, env step (env_step 1)], the planner's
-        per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) + ["plan"] * cfg.Ndiffuse
+        per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) + ["plan"] * max(n_diffuse)
         for i, (_, us) in enumerate(sorted(rollouts)):
             key = f"rollout_kernel ({per_step[i % len(per_step)]})"
             n, tot = acc.get(key, (0, 0.0))
@@ -171,7 +187,7 @@ def main():
         flush.zero_()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        loop.step(cfg.Ndiffuse, env_step=es)
+        loop.step(nd, env_step=es)
         e1.record()
         evs.append((e0, e1))
     torch.cuda.synchronize()
@@ -180,7 +196,8 @@ def main():
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
                           distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
-                          value=B * cfg.Ndiffuse * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
+                          schedules=args.schedules, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
+                          value=sum(n_diffuse) * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
 
 
