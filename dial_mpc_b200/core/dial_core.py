@@ -315,7 +315,7 @@ class DeviceLoop:
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
                  compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                 schedule=None):
+                 schedule=None, delay=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -356,7 +356,13 @@ class DeviceLoop:
         B specs or None (the plan's; ``schedule_setting``: any of ``temp_sample``, ``sigma_scale``,
         ``horizon_diffuse_factor``, ``traj_diffuse_factor``, ``Ndiffuse``, ``Ndiffuse_init``).  Instance b then
         computes bitwise what a single-instance loop on an MBDPI with b's updated DialConfig computes
-        (``set_schedule``, ``step``)."""
+        (``set_schedule``, ``step``).
+
+        ``delay``: each instance's control latency, one delay spec for every instance or a list of B specs or
+        None (``delay_setting``: an int d, or ``{"steps": d, "predict": True}``).  The action planned at step t
+        reaches the plant at step t + d; a predicting instance plans from the plant state predicted d steps
+        ahead through its queued actions on its planning model (``set_delay``, ``pending_actions``,
+        ``planning_state``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -422,9 +428,17 @@ class DeviceLoop:
             for spec in schedule:
                 if spec is not None:
                     schedule_setting(spec, a)
+        if delay is not None:
+            if mbdpi.world_size != 1:
+                raise ValueError("delay= needs an unsharded plan (world_size 1)")
+            delay = self._per_instance("delay", delay, f"one delay spec or a list of {B}",
+                                       lambda s: isinstance(s, (list, tuple)))
+            delay = [None if spec is None else delay_setting(spec) for spec in delay]
         # each instance's DialConfig, whether it has a table of its own, and the iteration limits last
         # uploaded (None: no limits, every instance runs every iteration of a step)
         self._cfg, self._own, self._lims = [a] * B, [False] * B, None
+        # each instance's (steps, predict) as last set
+        self._delay = [(0, False)] * B
         ps = [s.pipeline_state for s in states]
         per = (lambda t: t[0]) if B == 1 else torch.stack   # one instance: the buffers keep their plain shapes
         counters = [[int(s.info.get("step", 0)), int(s.info.get("contact_stage", 0))] for s in states]
@@ -484,6 +498,9 @@ class DeviceLoop:
         for b, spec in enumerate(schedule or ()):
             if spec is not None:
                 self.set_schedule(b, spec)
+        for b, d in enumerate(delay or ()):
+            if d is not None and d != (0, False):   # a loop without delays keeps the plan's launches
+                self.set_delay(b, {"steps": d[0], "predict": d[1]})
 
     @staticmethod
     def _model(env_or_sys):
@@ -626,6 +643,37 @@ class DeviceLoop:
         self.plan.set_instance_schedule(b, float(np.float32(cfg.temp_sample)), table)
         self._cfg[b], self._own[b] = cfg, True
 
+    def set_delay(self, b: int, spec) -> None:
+        """Instance b's control latency from the next ``step`` on (a delay spec, ``delay_setting``).  Refills its
+        queue with d copies of its current ``Y[0]``: until then the plant applies the plan it holds.  A
+        stream-ordered copy on the current stream.  The first delay of a loop, and a call that changes the
+        largest delay or the largest delay of a predicting instance, make the next steps capture their graphs
+        again; other calls keep them."""
+        b = self._instance(b)
+        steps, predict = delay_setting(spec)
+        self.plan.set_instance_delay(b, steps, predict)
+        self._delay[b] = (steps, predict)
+
+    def pending_actions(self) -> torch.Tensor:
+        """Each instance's queued actions in the order the next env steps apply them, a new tensor [B, 16, nu]
+        ([16, nu] for one instance; rows past the instance's delay are zero).  Asynchronous on the current
+        stream."""
+        lead = (self.n_instances,) if self.n_instances > 1 else ()
+        return self.plan.pending_actions(self.plan.empty(*lead, _capi.DEFINES["DIAL_MAXDELAY"], self.mbdpi.nu))
+
+    def planning_state(self) -> Dict[str, torch.Tensor]:
+        """The state the last step's planning rollouts started from, new tensors ``qpos``, ``qvel``,
+        ``qacc_warmstart`` and ``counters`` (int32 {step, contact_stage}) with a leading [B] on a batched loop:
+        the predicted state of a predicting instance, the plant state of any other.  Asynchronous on the
+        current stream."""
+        lead = (self.n_instances,) if self.n_instances > 1 else ()
+        m = self.mbdpi.env.sys
+        out = dict(qpos=self.plan.empty(*lead, m.nq), qvel=self.plan.empty(*lead, m.nv),
+                   qacc_warmstart=self.plan.empty(*lead, m.nv),
+                   counters=torch.empty(*lead, 2, dtype=torch.int32, device=self.mbdpi.device))
+        self.plan.planning_state(out["qpos"], out["qvel"], out["qacc_warmstart"], out["counters"])
+        return out
+
     def step(self, n_diffuse: Optional[int] = None, env_step=True, initial: bool = False) -> None:
         """One control step (asynchronous on the current stream).  env_step: True = env step + shift
         + plan (the reference's main loop), False = plan only, 2 = shift + plan (state untouched).
@@ -646,13 +694,15 @@ class DeviceLoop:
             self._lims = list(counts)
         stepping = env_step is True or env_step == 1
         if self._rand:
-            # the env step (if any) runs at info["step"], the rollouts cover the Hsample+1 steps after it
+            # the env step (if any) runs at info["step"], the rollouts cover the Hsample+1 steps after it; a
+            # predicting instance's prediction steps and rollouts reach d steps further
+            ahead = [d if p else 0 for d, p in self._delay]
             horizon = self.mbdpi.args.Hsample + (2 if stepping else 1)
             if self._tasks_host is None:
-                self.plan.set_command(self.mbdpi.env.command_override(self._env_info[0], horizon))
+                self.plan.set_command(self.mbdpi.env.command_override(self._env_info[0], horizon + max(ahead)))
             else:
                 for b, info in enumerate(self._env_info):
-                    ov = self._envs[b].command_override(info, horizon)
+                    ov = self._envs[b].command_override(info, horizon + ahead[b])
                     key = _capi.task_set_command(self._tasks_host[b], ov)
                     if key != self._task_cmd[b]:      # upload only the instances whose command changed
                         self._upload_task(b)
@@ -688,7 +738,9 @@ class DeviceLoop:
 
     @property
     def action(self) -> torch.Tensor:
-        """``Y0[0]``: the action the next env step applies (device view; batched: [B,nu])."""
+        """``Y0[0]``: the action the next env step applies (device view; batched: [B,nu]).  With a delay it is
+        the action the next env step puts at the back of the instance's queue; the env step applies the
+        queue's front (``pending_actions()[..., 0, :]``)."""
         return self.buf["Y"][:, 0] if self.n_instances > 1 else self.buf["Y"][0]
 
     @property
@@ -859,6 +911,33 @@ def schedule_setting(spec, args: DialConfig) -> DialConfig:
     return dataclasses.replace(args, **{k: (int(v) if k.startswith("Ndiffuse") else v) for k, v in spec.items()})
 
 
+def delay_setting(spec):
+    """A delay spec -> (steps, predict) of ``dial_plan_set_instance_delay``: an int ``d`` (the action planned at
+    step t reaches the plant at step t + d, planned from the plant state) or ``{"steps": d, "predict": p}``
+    (``predict``, default False: plan from the state predicted through the d queued actions), d in 0..16.
+    Raises ValueError naming the bad key or value."""
+    dmax = _capi.DEFINES["DIAL_MAXDELAY"]
+
+    def steps(v):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= v <= dmax:
+            raise ValueError(f"steps must be an int in 0..{dmax}, got {v!r}")
+        return int(v)
+
+    if isinstance(spec, dict):
+        extra = sorted(set(spec) - {"steps", "predict"}, key=str)
+        if extra:
+            raise ValueError(f"unknown key {extra[0]!r} (a delay spec takes 'steps' and 'predict')")
+        if "steps" not in spec:
+            raise ValueError("a delay spec mapping needs steps, the delay in control steps")
+        p = spec.get("predict", False)
+        if not isinstance(p, (bool, np.bool_)):
+            raise ValueError(f"predict must be true or false, got {p!r}")
+        return steps(spec["steps"]), bool(p)
+    if isinstance(spec, bool) or not isinstance(spec, (int, np.integer)):
+        raise ValueError(f"a delay spec is an int (control steps) or a mapping of 'steps' and 'predict', got {spec!r}")
+    return steps(spec), False
+
+
 def load_setting(spec, key: str, K: int, nv: Optional[int] = None):
     """The ``risk``, ``adapt`` or ``prior`` entry ``key`` of an ``--ensemble`` file or an
     ``--instance-overrides`` mapping, checked for K members and nv dofs (``risk_setting``,
@@ -915,14 +994,15 @@ def load_ensemble(spec, env):
 
 
 def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                  schedule=None):
+                  schedule=None, delay=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
     ``ensemble``: K planning models shared by every instance (``DeviceLoop(..., ensemble=...)``), scored
     under ``risk`` (one risk spec or B of them, ``DeviceLoop(..., risk=...)``), adapting to the plant under
     ``adapt`` from the belief ``prior`` (``DeviceLoop(..., adapt=..., prior=...)``).  ``schedule``: B schedule
-    specs or None (``DeviceLoop(..., schedule=...)``); each instance runs its own Ndiffuse_init, then Ndiffuse."""
+    specs or None (``DeviceLoop(..., schedule=...)``); each instance runs its own Ndiffuse_init, then Ndiffuse.
+    ``delay``: one delay spec or B of them (``DeviceLoop(..., delay=...)``)."""
     mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
@@ -930,7 +1010,7 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
     loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior,
-                      schedule=schedule)
+                      schedule=schedule, delay=delay)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -951,6 +1031,13 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
     timestamp = time.strftime("%Y%m%d-%H%M%S")
     for b in range(B):
         save_run(dial_config.output_dir, [r[b] for r in rollout], [x[b] for x in infos], timestamp=f"{timestamp}_inst{b}")
+
+
+def _delay_specs(delay):
+    """(steps, predict), or a list of them, as delay specs for ``DeviceLoop(..., delay=...)``."""
+    if isinstance(delay, list):
+        return [{"steps": d, "predict": p} for d, p in delay]
+    return {"steps": delay[0], "predict": delay[1]}
 
 
 def _print_belief(loop) -> None:
@@ -991,6 +1078,11 @@ def main():
                              "weight the members by how well they predict each env step's qvel (S: one scale or one "
                              "per dof), from 'prior', K weights (default uniform); an --instance-overrides mapping "
                              "may carry its own 'adapt'")
+    parser.add_argument("--delay", type=str, default=None, metavar="STEPS[:predict]",
+                        help="control latency of every instance: the action planned at step t reaches the simulated "
+                             "robot at step t + STEPS (0..16); ':predict' plans from the state predicted STEPS steps "
+                             "ahead through the queued actions; an --instance-overrides mapping may carry its own "
+                             "'delay' (an int or {steps: d, predict: true})")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -1010,6 +1102,19 @@ def main():
         parser.error("--instances must be at least 1")
     if args.instances > 1 and args.eager:
         parser.error("--instances runs on the CUDA-graph loop; it excludes --eager")
+    delay = None
+    if args.delay is not None:
+        if args.eager:
+            parser.error("--delay runs on the CUDA-graph loop; it excludes --eager")
+        steps, sep, mode = args.delay.partition(":")
+        try:
+            if sep and mode != "predict":
+                raise ValueError(f"the suffix must be ':predict', got {args.delay!r}")
+            if not steps.strip().lstrip("-").isdigit():
+                raise ValueError(f"STEPS must be an int, got {steps!r}")
+            delay = delay_setting({"steps": int(steps), "predict": bool(sep)})
+        except ValueError as e:
+            parser.error(f"--delay: {e}")
     rng = drandom.PRNGKey(seed=dial_config.seed)
     env_config_type = dial_envs.get_config(dial_config.env_name)
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
@@ -1037,15 +1142,16 @@ def main():
         # DialConfig fields: the sampling schedule (SCHEDULE_FIELDS), or fields shared by the plan, which
         # schedule_setting rejects by name
         dial_fields = {f.name for f in dataclasses.fields(DialConfig)} - env_fields
-        known = env_fields | dial_fields | {"sys", "risk", "adapt"}
+        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay"}
         envs = []
         settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
         uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
         schedule = [None] * args.instances
+        delays = [delay] * args.instances
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt, delay "
                              f"or the sampling fields {', '.join(SCHEDULE_FIELDS)}, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
@@ -1057,6 +1163,12 @@ def main():
                     parser.error(f"--instance-overrides entry {b}: {e}")
                 schedule[b] = spec
             sys_ov = ov.pop("sys", None)
+            if ov.get("delay") is not None:
+                try:
+                    delays[b] = delay_setting(ov["delay"])
+                except ValueError as e:
+                    parser.error(f"--instance-overrides entry {b}: delay: {e}")
+            ov.pop("delay", None)
             for key in ("risk", "adapt"):
                 if ov.get(key) is not None:
                     if members is None:
@@ -1091,9 +1203,12 @@ def main():
             risk = [r or {"aggregate": "mean"} for r in settings["risk"]]
         if args.instance_overrides is not None and any(a is not None for a in settings["adapt"]):
             adapt = settings["adapt"]
+        if args.instance_overrides is not None and any(d is not None for d in delays):
+            delay = [d or (0, False) for d in delays]
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
                       ensemble=members, risk=risk, adapt=adapt, prior=prior,
-                      schedule=schedule if args.instance_overrides is not None and any(schedule) else None)
+                      schedule=schedule if args.instance_overrides is not None and any(schedule) else None,
+                      delay=None if delay is None else _delay_specs(delay))
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
@@ -1102,10 +1217,12 @@ def main():
     rng_exp, rng = drandom.split(rng)
     Nstep = args.n_steps or dial_config.n_steps
     rews, rollout, infos = [], [], []
+    if delay is not None and mbdpi.world_size != 1:
+        parser.error("--delay needs an unsharded plan (one process)")
     if mbdpi.world_size == 1 and not args.eager:
         # one CUDA graph per control step; the host launches it and logs
         loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk,
-                          adapt=adapt, prior=prior)
+                          adapt=adapt, prior=prior, delay=None if delay is None else _delay_specs(delay))
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):

@@ -157,6 +157,37 @@ HD const float* schedule_noise(const InstSchedule* S, int inst, int iter, const 
 // no limits: every instance runs every iteration)
 HD bool schedule_runs(const int32_t* lim, int inst, int iter) { return !lim || iter < lim[inst]; }
 
+// Instance b's control latency (dial_plan_set_instance_delay): d control steps, and whether it plans from
+// the state predicted through its queued actions.
+struct alignas(8) DelaySetting {
+  int32_t d;         // 0..DIAL_MAXDELAY
+  int32_t predict;   // 0 or 1
+};
+// The action queue of one instance is a ring of d slots of nu floats whose front is slot `head`.  Position
+// i of the queue (0: the front, applied next) is slot delay_slot(head, d, i).
+HD int delay_slot(int head, int d, int i) { const int s = head + i; return s >= d ? s - d : s; }
+// One control step of the queue, for the action elements a = a0, a0 + da, ... < nu (a CTA passes its
+// threads).  pop (a step with an env step): applied[a] = the front's element (y0[a] when d = 0), and y0[a]
+// takes the front's slot, which becomes the back.  Then, always: pending [DIAL_MAXDELAY][nu] = the queue in
+// application order, zero past d.  Returns the front slot after the step.  Each element is read and
+// written by one caller only, so callers that split the elements need no synchronisation.
+DEV int delay_queue_step(float* ring, int head, int d, int nu, const float* y0, float* applied, float* pending,
+                         bool pop, int a0, int da) {
+  const int h1 = pop && d > 0 ? delay_slot(head, d, 1) : head;
+  for (int a = a0; a < nu; a += da) {
+    if (pop) {
+      if (d == 0) {
+        applied[a] = y0[a];
+      } else {
+        applied[a] = ring[head * nu + a];
+        ring[head * nu + a] = y0[a];
+      }
+    }
+    for (int j = 0; j < DIAL_MAXDELAY; ++j) pending[j * nu + a] = j < d ? ring[delay_slot(h1, d, j) * nu + a] : 0.f;
+  }
+  return h1;
+}
+
 // arguments of one rollout launch
 struct RolloutArgs {
   int32_t nrows;        // sample rows rolled by this launch

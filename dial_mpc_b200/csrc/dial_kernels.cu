@@ -613,6 +613,37 @@ __global__ void __launch_bounds__(32) ens_belief_kernel(const float* __restrict_
   if (lane == 0) ens_belief_update(L + (size_t)b * K, w + (size_t)b * K, l, K, (double)adapt[b].forget);
 }
 
+// Control latency (dial_plan_set_instance_delay), one CTA per instance b: its queue's step
+// (delay_queue_step; pop in a step with an env step) from its action Y[b][0], the action its env step
+// applies (applied [B][nu]), its queue in application order (pending [B][DIAL_MAXDELAY][nu]) and its
+// prediction length pred_len[b] (d when it predicts, else 0) for the prediction launches.
+__global__ void __launch_bounds__(128) delay_queue_kernel(const DelaySetting* __restrict__ set, int32_t* __restrict__ head,
+                                                          float* __restrict__ ring, const float* __restrict__ Y, int n1,
+                                                          int nu, int pop, float* __restrict__ applied,
+                                                          float* __restrict__ pending, int32_t* __restrict__ pred_len) {
+  const int b = blockIdx.x;
+  const DelaySetting s = set[b];
+  const int h = head[b];
+  const size_t q = (size_t)b * DIAL_MAXDELAY * nu;
+  const int h1 = delay_queue_step(ring + q, h, s.d, nu, Y + (size_t)b * n1 * nu, applied + (size_t)b * nu, pending + q,
+                                  pop != 0, threadIdx.x, blockDim.x);
+  __syncthreads();   // every thread has read head[b]
+  if (threadIdx.x == 0) { head[b] = h1; pred_len[b] = s.predict && s.d > 0 ? s.d : 0; }
+}
+
+// dial_plan_set_instance_delay: instance b's queue refilled with d copies of Y[b][0], front at slot 0, and
+// its pending rows laid out (one CTA)
+__global__ void __launch_bounds__(128) delay_refill_kernel(int b, int d, int32_t* __restrict__ head, float* __restrict__ ring,
+                                                           const float* __restrict__ Y, int n1, int nu,
+                                                           float* __restrict__ pending) {
+  const size_t q = (size_t)b * DIAL_MAXDELAY * nu;
+  const float* y0 = Y + (size_t)b * n1 * nu;
+  for (int a = threadIdx.x; a < nu; a += blockDim.x)
+    for (int j = 0; j < d; ++j) ring[q + (size_t)j * nu + a] = y0[a];
+  delay_queue_step(ring + q, 0, d, nu, y0, nullptr, pending + q, false, threadIdx.x, blockDim.x);
+  if (threadIdx.x == 0) head[b] = 0;
+}
+
 // ---------------------------------------------------------------------------------
 // plan object
 // ---------------------------------------------------------------------------------
@@ -718,6 +749,23 @@ struct dial_plan {
   // call; the staging `h` mirrors what the device holds
   Staged<InstSchedule> sched;
   Staged<int32_t> lims;
+  // per-instance control latency (dial_plan_set_instance_delay): the settings [n_inst] (the staging mirrors
+  // the device), and, allocated with them, the queues' front slots [n_inst] and rings [n_inst][DIAL_MAXDELAY][nu],
+  // the applied actions [n_inst][nu], the queues in application order [n_inst][DIAL_MAXDELAY][nu], the
+  // prediction lengths [n_inst], the planning state (qpos, qvel, warm start, counters) and, on an ensemble
+  // plan, the planning models [n_inst] (a copy of member (b, 0)).  dl_max / dl_pred: the largest delay, and
+  // that of the predicting instances (the number of prediction launches), as set on the host.
+  Staged<DelaySetting> delay;
+  int32_t* dl_head = nullptr;
+  float* dl_ring = nullptr;
+  float* dl_applied = nullptr;
+  float* dl_pending = nullptr;
+  int32_t* dl_len = nullptr;
+  float *dl_qpos = nullptr, *dl_qvel = nullptr, *dl_warm = nullptr;
+  int32_t* dl_cnt = nullptr;
+  DevModel* dl_models = nullptr;
+  int dl_max = 0, dl_pred = 0;
+  int dl_pred_last = 0;   // dl_pred of the last dial_mpc_step (its graph's launch sequence)
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -987,6 +1035,9 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   p->models.release(); p->members.release(); p->risk.release();
   p->adapt.release(); p->belief_L.release(); p->belief_w.release(); p->sched.release(); p->lims.release();
   cudaFree(p->ens_rews); cudaFree(p->dEll); cudaFree(p->pred_us); cudaFree(p->pred_qd);
+  p->delay.release();
+  cudaFree(p->dl_head); cudaFree(p->dl_ring); cudaFree(p->dl_applied); cudaFree(p->dl_pending); cudaFree(p->dl_len);
+  cudaFree(p->dl_qpos); cudaFree(p->dl_qvel); cudaFree(p->dl_warm); cudaFree(p->dl_cnt); cudaFree(p->dl_models);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   cudaFree(p->weights2);
@@ -1100,7 +1151,12 @@ extern "C" int dial_plan_set_ensemble_model(dial_plan* p, int b, int k, const di
   if (int rc = need_ensemble(p, fn, 1)) return rc;
   if (int rc = need_instance(p, fn, b)) return rc;
   if (k < 0 || k >= p->n_ens) return fail(std::string(fn) + ": member " + std::to_string(k) + " out of range (0.." + std::to_string(p->n_ens - 1) + ")");
-  return set_model_slot(p, fn, p->members, (size_t)p->n_inst * p->n_ens, (size_t)b * p->n_ens + k, m, (cudaStream_t)stream);
+  const size_t slot = (size_t)b * p->n_ens + k;
+  if (int rc = set_model_slot(p, fn, p->members, (size_t)p->n_inst * p->n_ens, slot, m, (cudaStream_t)stream)) return rc;
+  // member (b, 0) is instance b's planning model for its prediction through a delay
+  if (k == 0 && p->dl_models)
+    CUDA_OK(cudaMemcpyAsync(p->dl_models + b, p->members.d + slot, sizeof(DevModel), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
 }
 
 extern "C" int dial_plan_set_ensemble_risk(dial_plan* p, int b, int mode, float alpha, void* stream) {
@@ -1263,6 +1319,105 @@ extern "C" int dial_plan_set_instance_iterations(dial_plan* p, const int32_t* n_
   }
   e = p->lims.put(0, [&](int32_t* L) { memcpy(L, n_iter, sizeof(int32_t) * p->n_inst); }, st);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
+// First dial_plan_set_instance_delay: the queues, the planning state and (ensemble plans) the planning models,
+// member (b, 0) of each instance as the member slots hold it, else the plan's model.
+static cudaError_t allocate_delay(dial_plan* p, cudaStream_t st) {
+  const size_t B = (size_t)p->n_inst, nu = p->hM.m.nu, nq = p->hM.m.nq, nv = p->hM.m.nv;
+  cudaError_t e = p->delay.allocate(B, 1, DelaySetting{0, 0});
+  auto dev = [&](auto*& ptr, size_t bytes) {
+    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ptr, 0, bytes, st);
+  };
+  dev(p->dl_head, B * sizeof(int32_t));
+  dev(p->dl_ring, B * DIAL_MAXDELAY * nu * sizeof(float));
+  dev(p->dl_applied, B * nu * sizeof(float));
+  dev(p->dl_pending, B * DIAL_MAXDELAY * nu * sizeof(float));
+  dev(p->dl_len, B * sizeof(int32_t));
+  dev(p->dl_qpos, B * nq * sizeof(float));
+  dev(p->dl_qvel, B * nv * sizeof(float));
+  dev(p->dl_warm, B * nv * sizeof(float));
+  dev(p->dl_cnt, B * 2 * sizeof(int32_t));
+  if (p->n_ens > 0 && e == cudaSuccess) {
+    e = cudaMalloc(&p->dl_models, B * sizeof(DevModel));
+    for (size_t b = 0; b < B && e == cudaSuccess; ++b)
+      e = p->members.d ? cudaMemcpyAsync(p->dl_models + b, p->members.d + b * p->n_ens, sizeof(DevModel), cudaMemcpyDeviceToDevice, st)
+                       : cudaMemcpy(p->dl_models + b, &p->hM, sizeof(DevModel), cudaMemcpyHostToDevice);
+  }
+  if (e != cudaSuccess) {
+    p->delay.release();
+    for (void* d : {(void*)p->dl_head, (void*)p->dl_ring, (void*)p->dl_applied, (void*)p->dl_pending, (void*)p->dl_len,
+                    (void*)p->dl_qpos, (void*)p->dl_qvel, (void*)p->dl_warm, (void*)p->dl_cnt, (void*)p->dl_models})
+      cudaFree(d);
+    p->dl_head = p->dl_len = p->dl_cnt = nullptr;
+    p->dl_ring = p->dl_applied = p->dl_pending = p->dl_qpos = p->dl_qvel = p->dl_warm = nullptr;
+    p->dl_models = nullptr;
+  }
+  return e;
+}
+
+extern "C" int dial_plan_set_instance_delay(dial_plan* p, int b, int steps, int predict, void* stream) {
+  static const char* fn = "dial_plan_set_instance_delay";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (int rc = need_instance(p, fn, b)) return rc;
+  const dial_plan_desc& c = p->hP.c;
+  if (c.Ntotal != c.Nsample || p->xch.on) return fail(std::string(fn) + ": sharded plans (Ntotal != Nsample) have no per-instance delay");
+  if (steps < 0 || steps > DIAL_MAXDELAY)
+    return fail(std::string(fn) + ": steps " + std::to_string(steps) + " out of range (0.." DIAL_STR(DIAL_MAXDELAY) ")");
+  if (predict != 0 && predict != 1) return fail(std::string(fn) + ": predict must be 0 or 1, got " + std::to_string(predict));
+  if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first (the queue is filled from the bound Y)");
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (!p->delay.d) {
+    // first call: the graphs captured so far apply Y[b][0] at once
+    if ((e = allocate_delay(p, st)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+    drop_graphs(p);
+  }
+  e = p->delay.put(b, [&](DelaySetting* s) { s->d = steps; s->predict = predict; }, st);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  const int n1 = c.Hnode + 1, nu = p->hM.m.nu;
+  delay_refill_kernel<<<1, 128, 0, st>>>(b, steps, p->dl_head, p->dl_ring, p->mpc.Y, n1, nu, p->dl_pending);
+  CUDA_OK(cudaGetLastError());
+  // the launch sequence depends on the largest delay and on the prediction length (staging = device)
+  int dmax = 0, dpred = 0;
+  for (int i = 0; i < p->n_inst; ++i) {
+    const DelaySetting& s = p->delay.h[i];
+    dmax = s.d > dmax ? s.d : dmax;
+    if (s.predict && s.d > dpred) dpred = s.d;
+  }
+  if (dmax != p->dl_max || dpred != p->dl_pred) drop_graphs(p);
+  p->dl_max = dmax; p->dl_pred = dpred;
+  return 0;
+}
+
+extern "C" int dial_plan_pending_actions(dial_plan* p, float* out, void* stream) {
+  static const char* fn = "dial_plan_pending_actions";
+  if (!p || !out) return fail(std::string(fn) + ": null argument");
+  const size_t n = (size_t)p->n_inst * DIAL_MAXDELAY * p->hM.m.nu * sizeof(float);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (p->dl_pending) CUDA_OK(cudaMemcpyAsync(out, p->dl_pending, n, cudaMemcpyDeviceToDevice, st));
+  else CUDA_OK(cudaMemsetAsync(out, 0, n, st));
+  return 0;
+}
+
+extern "C" int dial_plan_planning_state(dial_plan* p, float* qpos, float* qvel, float* warm, int32_t* counters, void* stream) {
+  static const char* fn = "dial_plan_planning_state";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
+  const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv;
+  // the last step planned from the predicted state when it predicted (then the other instances' rows hold
+  // their plant state, copied in that step)
+  const bool pred = p->dl_pred_last > 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const auto cp = [&](void* dst, const void* src, size_t bytes) {
+    return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
+  };
+  CUDA_OK(cp(qpos, pred ? p->dl_qpos : p->mpc.qpos, B * nq * sizeof(float)));
+  CUDA_OK(cp(qvel, pred ? p->dl_qvel : p->mpc.qvel, B * nv * sizeof(float)));
+  CUDA_OK(cp(warm, pred ? p->dl_warm : p->mpc.qacc_warmstart, B * nv * sizeof(float)));
+  CUDA_OK(cp(counters, pred ? p->dl_cnt : p->mpc.counters, B * 2 * sizeof(int32_t)));
   return 0;
 }
 
@@ -1532,12 +1687,25 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
   const bool batched = ni > 1;
   float* Y[2] = {B.Y, p->mpc_Y1};
   int cur = 0;
+  // control latency, once some instance was given a delay: the queues move in a step with an env step, which
+  // then applies the action each queue pops (dl_applied, one row of nu per instance) instead of Y[b][0]; while
+  // some instance predicts, the queue launch also lays out the pending actions in the other steps
+  const bool delay = p->delay.d != nullptr;
+  const int npred = delay ? p->dl_pred : 0;
+  if (delay && (env_step == 1 || npred > 0)) {
+    delay_queue_kernel<<<ni, 128, 0, st>>>(p->delay.d, p->dl_head, p->dl_ring, Y[cur], n1, nu, env_step == 1,
+                                           p->dl_applied, p->dl_pending, p->dl_len);
+    p->launches++;
+    CUDA_OK(cudaGetLastError());
+  }
+  const float* act = delay ? p->dl_applied : Y[cur];
+  const int act_n1 = delay ? 1 : n1;   // rows of nu floats between two instances' actions
   // ensemble adaptation, once some instance has turned it on: before the plant's env step, member (b, k)
   // makes the same env step on its own model, from instance b's state, counters and task with the action
-  // Y[b][0] (row b K + k, its CTA staging member slot b K + k); only the post-step qvel is kept
+  // the plant applies (row b K + k, its CTA staging member slot b K + k); only the post-step qvel is kept
   const bool adapt = env_step == 1 && p->pred_qd;
   if (adapt) {
-    ens_gather_kernel<<<ni, 128, 0, st>>>(Y[cur], K, n1, nu, p->pred_us);
+    ens_gather_kernel<<<ni, 128, 0, st>>>(act, K, act_n1, nu, p->pred_us);
     p->launches++;
     CUDA_OK(cudaGetLastError());
     RolloutArgs A; memset(&A, 0, sizeof(A));
@@ -1554,8 +1722,8 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     RolloutArgs A; memset(&A, 0, sizeof(A));
     A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart;
     A.counters_in = B.counters; A.counters_out = B.counters;
-    A.nrows = ni; A.H = 1; A.mode = 0; A.us = Y[cur]; A.rewss = B.reward;
-    if (batched) { A.rows_per_inst = 1; A.us_row = n1 * nu; }
+    A.nrows = ni; A.H = 1; A.mode = 0; A.us = act; A.rewss = B.reward;
+    if (batched) { A.rows_per_inst = 1; A.us_row = act_n1 * nu; }
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
     A.models = p->models.d;
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
@@ -1572,6 +1740,31 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     p->launches++;
     CUDA_OK(cudaGetLastError());
     cur ^= 1;
+  }
+  // The planning state: the plant state, or once some instance predicts, a copy of it in which each predicting
+  // instance b takes d_b env steps with its queued actions on its planning model (launch j: one row per
+  // instance, action pending[b][j], in place; an instance with pred_len[b] <= j exits at entry)
+  const float *qpos0 = B.qpos, *qvel0 = B.qvel, *warm0 = B.qacc_warmstart;
+  const int32_t* cnt0 = B.counters;
+  if (npred > 0) {
+    const size_t nq = p->hM.m.nq, nv = p->hM.m.nv;
+    CUDA_OK(cudaMemcpyAsync(p->dl_qpos, B.qpos, ni * nq * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(p->dl_qvel, B.qvel, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(p->dl_warm, B.qacc_warmstart, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(p->dl_cnt, B.counters, ni * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    for (int j = 0; j < npred; ++j) {
+      RolloutArgs A; memset(&A, 0, sizeof(A));
+      A.qpos0 = p->dl_qpos; A.qvel0 = p->dl_qvel; A.warm0 = p->dl_warm;
+      A.counters_in = p->dl_cnt; A.counters_out = p->dl_cnt;
+      A.nrows = ni; A.H = 1; A.mode = 0; A.rows_per_inst = 1;
+      A.us = p->dl_pending + (size_t)j * nu; A.us_row = DIAL_MAXDELAY * nu;
+      if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
+      A.models = p->n_ens > 0 ? p->dl_models : p->models.d;
+      A.iter_lim = p->dl_len; A.iter = j;
+      A.qpos_out = p->dl_qpos; A.qvel_out = p->dl_qvel; A.warm_out = p->dl_warm;
+      CUDA_OK(launch_rollout(p, A, 1, st));
+    }
+    qpos0 = p->dl_qpos; qvel0 = p->dl_qvel; warm0 = p->dl_warm; cnt0 = p->dl_cnt;
   }
   // The info-only bars (qbar, qdbar, xbar; dial_core.py:133-135) are computed for EVERY iteration,
   // like the reference's scan does (the caller sees those of the last one), on a side branch of
@@ -1592,7 +1785,7 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
     }
     if (bars && i >= 2) CUDA_OK(cudaStreamWaitEvent(st, p->ev_side[i & 1], 0));
     RolloutArgs A; memset(&A, 0, sizeof(A));
-    A.qpos0 = B.qpos; A.qvel0 = B.qvel; A.warm0 = B.qacc_warmstart; A.counters_in = B.counters;
+    A.qpos0 = qpos0; A.qvel0 = qvel0; A.warm0 = warm0; A.counters_in = cnt0;
     A.nrows = ni * K * (c.Nsample + 1); A.H = c.Hsample + 1; A.mode = 1;
     if (batched || p->n_ens > 0) A.rows_per_inst = K * (c.Nsample + 1);
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? K * (c.Nsample + 1) : 0; }
@@ -1666,6 +1859,7 @@ extern "C" int dial_mpc_step(dial_plan* p, int n_diffuse, int env_step, void* st
                   " diffusion iterations, its schedule has " + std::to_string(S.n_rows) + " rows");
   }
   cudaStream_t st = (cudaStream_t)stream;
+  p->dl_pred_last = p->delay.d ? p->dl_pred : 0;   // (a change of dl_pred drops the graphs)
   dial_plan::MpcGraph* g = nullptr;
   for (auto& e : p->mpc_graphs) if (e.n_diffuse == n_diffuse && e.env_step == env_step) g = &e;
   if (!g) {

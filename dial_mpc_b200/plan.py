@@ -162,6 +162,34 @@ class Plan:
         self._check(self.lib.dial_plan_set_instance_iterations(self.handle, a.ctypes.data_as(C.POINTER(C.c_int32)),
                                                                _stream()))
 
+    def set_instance_delay(self, b: int, steps: int, predict: bool = False) -> None:
+        """Instance b's control latency from the next ``mpc_step`` on: the action planned at step t reaches the
+        plant at step t + ``steps`` (0..16), and with ``predict`` the instance plans from the state predicted
+        through its queued actions.  Refills b's queue with ``steps`` copies of its current Y[0]; a stream-ordered
+        copy on the current stream (``dial_plan_set_instance_delay``)."""
+        self._check(self.lib.dial_plan_set_instance_delay(self.handle, int(b), int(steps), int(bool(predict)), _stream()))
+
+    def pending_actions(self, out: torch.Tensor) -> torch.Tensor:
+        """Copy each instance's queued actions in application order into ``out`` [n_inst * 16 * nu] elements,
+        rows past the instance's delay zero (``dial_plan_pending_actions``)."""
+        n = max(self.desc.n_inst, 1) * _capi.DEFINES["DIAL_MAXDELAY"] * self.nu
+        assert out.numel() == n, f"need {n} elements, got {tuple(out.shape)}"
+        self._check(self.lib.dial_plan_pending_actions(self.handle, _ptr(out), _stream()))
+        return out
+
+    def planning_state(self, qpos: Optional[torch.Tensor], qvel: Optional[torch.Tensor] = None,
+                       warm: Optional[torch.Tensor] = None, counters: Optional[torch.Tensor] = None) -> None:
+        """Copy the state the last planning rollouts started from (each output may be None; ``counters`` int32
+        [n_inst * 2]) (``dial_plan_planning_state``)."""
+        B = max(self.desc.n_inst, 1)
+        for t, n in ((qpos, B * self.nq), (qvel, B * self.nv), (warm, B * self.nv)):
+            assert t is None or t.numel() == n, f"need {n} elements, got {tuple(t.shape)}"
+        cnt = None
+        if counters is not None:
+            assert counters.is_cuda and counters.dtype == torch.int32 and counters.is_contiguous() and counters.numel() == 2 * B
+            cnt = C.c_void_p(counters.data_ptr())
+        self._check(self.lib.dial_plan_planning_state(self.handle, _ptr(qpos), _ptr(qvel), _ptr(warm), cnt, _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

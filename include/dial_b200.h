@@ -44,6 +44,7 @@ extern "C" {
 #define DIAL_MAXRANK 8  /* GPUs of one NVLink domain sharing the samples */
 #define DIAL_MAXENS 16  /* planning models (ensemble members) of one instance */
 #define DIAL_MAXDIFFUSE 64 /* diffusion iterations of one control step (dial_mpc_step) */
+#define DIAL_MAXDELAY 16   /* control steps of latency of one instance (dial_plan_set_instance_delay) */
 #define DIAL_IPC_HANDLE_BYTES 64
 
 /* environments (reward functors fused into the rollout kernel) */
@@ -493,6 +494,42 @@ int dial_plan_set_instance_schedule(dial_plan* plan, int b, float temp, int n_ro
  * allocates with the plan's model when no model was set), so a skipped instance's CTAs exit whole; an
  * instance's results do not depend on the launch shape. */
 int dial_plan_set_instance_iterations(dial_plan* plan, const int32_t* n_iter, void* stream);
+
+/* Per-instance control latency of dial_mpc_step.  Instance b holds a FIFO queue of d_b actions [nu]
+ * (d_b in 0..DIAL_MAXDELAY, 0 by default).  In a dial_mpc_step with env_step == 1 it pops the front a,
+ * pushes Y[b][0] to the back (d_b = 0: a = Y[b][0]), and the plant's env step applies a: the action
+ * planned at step t reaches the plant at step t + d_b.  ctrl and reward are those of that env step, and an
+ * adapting ensemble instance scores its members' predictions under a too.  With env_step 0 or 2 the queue
+ * does not move.
+ * An instance that predicts (predict = 1, d_b >= 1) plans from a predicted state: in every dial_mpc_step,
+ * after the env step and the shift, a copy of the plant's qpos, qvel, qacc_warmstart and counters takes d_b
+ * env steps on the instance's planning model (its model; member (b, 0) of an ensemble plan) with the queued
+ * actions in FIFO order, its task and counters advancing as the env step advances them.  Every rollout of
+ * the instance starts from that state, so its rews, bars and knots describe the plan from it.  Without an
+ * ensemble, the planning state recorded after step t equals, bit for bit, the plant state after step
+ * t + d_b.  The other instances plan from the plant state.
+ * The prediction is max d_b (over the predicting instances) rollout launches of one row per instance, each
+ * skipping the instances whose prediction is shorter, after one copy of the plant state; a small queue
+ * launch precedes the env step (and runs in steps without one while some instance predicts).  A plan on
+ * which no delay is ever set launches what it launched before.  Sharded plans are rejected. */
+
+/* Instance b's delay `steps` (0..DIAL_MAXDELAY) and `predict` (0 or 1).  Every call refills b's queue with
+ * `steps` copies of Y[b][0] as it stands when the call's stream-ordered work runs on `stream` (so the plan
+ * must be bound, dial_mpc_bind).  The first call allocates the queues and planning-state buffers and drops
+ * the captured graphs; a later call that changes the plan's largest delay, or the largest delay of a
+ * predicting instance, drops them too (the launch sequence changes); other calls keep them, and take effect
+ * at the next replay.  Fails for b out of range and for a bad argument, which the error names. */
+int dial_plan_set_instance_delay(dial_plan* plan, int b, int steps, int predict, void* stream);
+
+/* Each instance's queue in application order: out [dev][n_inst][DIAL_MAXDELAY][nu], row j < d_b the action
+ * the env step j + 1 steps from now applies, rows j >= d_b zero (all zero on a plan without delays).  A
+ * stream-ordered copy on `stream`. */
+int dial_plan_pending_actions(dial_plan* plan, float* out, void* stream);
+
+/* The state the last planning rollouts of dial_mpc_step started from: qpos [dev][n_inst][nq], qvel and warm
+ * [dev][n_inst][nv], counters [dev][n_inst][2] ({step, contact_stage}), each nullable; the predicted state of
+ * a predicting instance, the plant state of every other.  Stream-ordered copies on `stream`. */
+int dial_plan_planning_state(dial_plan* plan, float* qpos, float* qvel, float* warm, int32_t* counters, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops

@@ -16,8 +16,11 @@ feet ``FR FL RR RL``, else every pair's friction scaled so; a per-instance model
 (dial_plan_desc.n_ens) spread as ``--distinct-models`` spreads the instances (member k: base mass
 +3 kg * k / K, friction 1 - 0.5 k / K), bound through ``dial_plan_set_ensemble_model``, and scores each
 sample by the ``--risk`` measure of its member rewards (mean, worst or cvar:ALPHA; default mean).
+``--delays FILE.yaml``: a YAML list of one delay spec per instance (``DeviceLoop(..., delay=...)``: an int or
+``{steps: d, predict: true}``), so that the step also moves the action queues and, for predicting instances,
+runs the prediction launches (use ``--env-step 1`` for the queues to move).
 ``--profile-kernels``: instead of the timing, run the steps without graph capture under torch.profiler and
-print the mean device time per launch of the rollout, update and ensemble reduction kernels."""
+print the mean device time per launch of the rollout, update, ensemble reduction and delay queue kernels."""
 import argparse
 import copy
 import json
@@ -80,6 +83,9 @@ def main():
     ap.add_argument("--schedules", default=None, metavar="FILE.yaml",
                     help="a YAML list of one schedule spec per instance (null: the config's; DeviceLoop(..., "
                          "schedule=...)); each instance then runs its own Ndiffuse")
+    ap.add_argument("--delays", default=None, metavar="FILE.yaml",
+                    help="a YAML list of one delay spec per instance (an int or {steps: d, predict: true}; "
+                         "DeviceLoop(..., delay=...))")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
@@ -95,7 +101,7 @@ def main():
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, schedule_setting
+    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, delay_setting, schedule_setting
 
     B, b = args.instances, BASELINE[args.config]
     cfg = dial_config(args.config, world=1)
@@ -143,12 +149,24 @@ def main():
             n_diffuse = [schedule_setting(s or {}, cfg).Ndiffuse for s in schedule]
         except ValueError as e:
             ap.error(f"--schedules {args.schedules}: {e}")
+    delay, n_pred = None, 0
+    if args.delays is not None:
+        import yaml
+        delay = yaml.safe_load(open(args.delays))
+        if not isinstance(delay, list) or len(delay) != B:
+            ap.error(f"--delays must hold a list of {B} delay specs (one per instance)")
+        try:
+            settings = [delay_setting(0 if s is None else s) for s in delay]
+        except ValueError as e:
+            ap.error(f"--delays {args.delays}: {e}")
+        delay = [{"steps": d, "predict": p} for d, p in settings]
+        n_pred = max([d for d, p in settings if p] or [0])
     if B == 1:
         loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt,
-                          schedule=schedule)
+                          schedule=schedule, delay=delay)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
-                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule)
+                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule, delay=delay)
     es = args.env_step
     # without --schedules every step runs the config's Ndiffuse on every instance, as before
     nd = None if schedule is not None else cfg.Ndiffuse
@@ -168,18 +186,21 @@ def main():
                 continue
             if "rollout_kernel" in ev.name:
                 rollouts.append((ev.time_range.start, ev.time_range.elapsed_us()))
-            for key in ("update_kernel", "ensemble_reduce_kernel", "trajbar", "ens_gather_kernel", "ens_belief_kernel"):
+            for key in ("update_kernel", "ensemble_reduce_kernel", "trajbar", "ens_gather_kernel", "ens_belief_kernel",
+                        "delay_queue_kernel"):
                 if key in ev.name:
                     n, tot = acc.get(key, (0, 0.0))
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
-        # the rollout launches of one step in order: [member prediction, env step (env_step 1)], the planner's
-        per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) + ["plan"] * max(n_diffuse)
+        # the rollout launches of one step in order: [member prediction, env step (env_step 1)], [the delay
+        # prediction steps], the planner's
+        per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) + \
+            ["delay prediction"] * n_pred + ["plan"] * max(n_diffuse)
         for i, (_, us) in enumerate(sorted(rollouts)):
             key = f"rollout_kernel ({per_step[i % len(per_step)]})"
             n, tot = acc.get(key, (0, 0.0))
             acc[key] = (n + 1, tot + us)
         print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
-                              risk=args.risk, adapt=args.adapt, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              risk=args.risk, adapt=args.adapt, delays=args.delays, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
                               launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
         return
     evs = []
@@ -196,7 +217,7 @@ def main():
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
                           distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
-                          schedules=args.schedules, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
+                          schedules=args.schedules, delays=args.delays, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
                           value=sum(n_diffuse) * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
 
