@@ -3200,7 +3200,9 @@ DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, flo
     float r_yaw = -dy * dy;
     const float r_contact = part0, pen = part1;   // per-contact terms: reward_partials
     rew = r_pos + r_upright + 0.3f * r_yaw + 0.1f * r_contact - 0.1f * pen + 10.f;
-    int ns = (int)floorf((float)(step + 1) * c.dt / T.jump_dt);
+    // IEEE division: -use_fast_math would make it a * (1 / b), whose floor differs from the host's at boundaries
+    // of jump_dt that are not powers of two (the host, the C port and the reference divide in fp32)
+    int ns = (int)floorf(__fdiv_rn((float)(step + 1) * c.dt, T.jump_dt));
     stage = ns < T.n_stage - 1 ? ns : T.n_stage - 1;
   }
   return rew;

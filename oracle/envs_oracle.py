@@ -308,8 +308,15 @@ class Go2SeqJumpOracle(Go2WalkOracle):
                 penalty[:, i] &= ~cond
         pen = penalty.sum(-1)
         rew = r_pos + r_upright + 0.3 * r_yaw + 0.1 * r_contact - 0.1 * pen + 10.0
-        new_stage = np.minimum(np.floor((s.step + 1) * self.dt / self.jump_dt), n - 1).astype(np.int64)
-        return rew, new_stage
+        return rew, self.next_stage(s.step)
+
+    def next_stage(self, step):
+        """Stage after the env step whose info["step"] is `step`: the reference computes the quotient in
+        JAX fp32 (unitree_go2_env.py:508-515), and an fp64 one floors differently at boundaries such as
+        step + 1 = 15 for jump_dt = 0.3 (fp32 0.99999994 -> stage 0)."""
+        f = np.float32
+        q = (np.asarray(step) + 1).astype(f) * f(self.dt) / f(self.jump_dt)
+        return np.minimum(np.floor(q), self.contact_targets.shape[0] - 1).astype(np.int64)
 
 
 class H1WalkOracle(OracleEnv):
