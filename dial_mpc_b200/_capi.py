@@ -262,6 +262,10 @@ def _bind(path: str) -> C.CDLL:
     lib.dial_plan_pending_actions.restype = C.c_int
     lib.dial_plan_planning_state.argtypes = [V, P, P, P, P, V]
     lib.dial_plan_planning_state.restype = C.c_int
+    lib.dial_plan_set_instance_observation.argtypes = [V, I, I, P, P, C.POINTER(C.c_uint32), V]
+    lib.dial_plan_set_instance_observation.restype = C.c_int
+    lib.dial_plan_observed_state.argtypes = [V, P, P, P, P, P, V]
+    lib.dial_plan_observed_state.restype = C.c_int
     for fn in ("dial_rollout", "dial_env_step", "dial_env_step_kin", "dial_plan_set_command", "dial_plan_set_stages", "dial_pipeline_init", "dial_reverse_rollout",
                "dial_reverse_update", "dial_reverse_update_x", "dial_reverse_update_fused", "dial_reverse_trajbar",
                "dial_reverse_trajectories", "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status"):
@@ -300,4 +304,4 @@ EXPORTS = ["dial_abi_version", "dial_last_error", "dial_sizeof", "dial_plan_crea
            "dial_plan_set_ensemble_risk", "dial_plan_member_rewards", "dial_plan_set_ensemble_adapt",
            "dial_plan_set_ensemble_belief", "dial_plan_ensemble_belief", "dial_plan_set_instance_schedule",
            "dial_plan_set_instance_iterations", "dial_plan_set_instance_delay", "dial_plan_pending_actions",
-           "dial_plan_planning_state"]
+           "dial_plan_planning_state", "dial_plan_set_instance_observation", "dial_plan_observed_state"]

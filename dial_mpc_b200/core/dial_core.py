@@ -315,7 +315,7 @@ class DeviceLoop:
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
                  compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                 schedule=None, delay=None):
+                 schedule=None, delay=None, observe=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -362,7 +362,14 @@ class DeviceLoop:
         None (``delay_setting``: an int d, or ``{"steps": d, "predict": True}``).  The action planned at step t
         reaches the plant at step t + d; a predicting instance plans from the plant state predicted d steps
         ahead through its queued actions on its planning model (``set_delay``, ``pending_actions``,
-        ``planning_state``)."""
+        ``planning_state``).
+
+        ``observe``: each instance's view of its plant, one observe spec for every instance or a list of B specs
+        or None (``observe_setting``: ``{"delay": k, "qpos": S, "qvel": S, "seed": s}``).  Instance b's
+        rollouts start from the plant record min(k, records - 1) env steps old plus Gaussian noise drawn once
+        per env step; a predicting instance (its delay spec's ``predict``) first takes the actions applied since
+        that record and its queued ones.  The plant, its reward and adaptation keep the plant state
+        (``set_observation``, ``observed_state``, ``planning_state``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -434,11 +441,20 @@ class DeviceLoop:
             delay = self._per_instance("delay", delay, f"one delay spec or a list of {B}",
                                        lambda s: isinstance(s, (list, tuple)))
             delay = [None if spec is None else delay_setting(spec) for spec in delay]
+        if observe is not None:
+            if mbdpi.world_size != 1:
+                raise ValueError("observe= needs an unsharded plan (world_size 1)")
+            observe = self._per_instance("observe", observe, f"one observe spec or a list of {B}",
+                                         lambda s: isinstance(s, (list, tuple)))
+            observe = [None if spec is None else observe_setting(spec, m) for spec in observe]
+            if rand[0] and any(o is not None and o[0] > 0 for o in observe):
+                raise ValueError(self._RAND_OBSERVE)
         # each instance's DialConfig, whether it has a table of its own, and the iteration limits last
         # uploaded (None: no limits, every instance runs every iteration of a step)
         self._cfg, self._own, self._lims = [a] * B, [False] * B, None
-        # each instance's (steps, predict) as last set
+        # each instance's (steps, predict) as last set, and its observation setting (None: none)
         self._delay = [(0, False)] * B
+        self._observe = [None] * B
         ps = [s.pipeline_state for s in states]
         per = (lambda t: t[0]) if B == 1 else torch.stack   # one instance: the buffers keep their plain shapes
         counters = [[int(s.info.get("step", 0)), int(s.info.get("contact_stage", 0))] for s in states]
@@ -501,6 +517,9 @@ class DeviceLoop:
         for b, d in enumerate(delay or ()):
             if d is not None and d != (0, False):   # a loop without delays keeps the plan's launches
                 self.set_delay(b, {"steps": d[0], "predict": d[1]})
+        for b, o in enumerate(observe or ()):
+            if o is not None and self._observing(o):   # nor does a loop without observations
+                self._set_observation(b, o)
 
     @staticmethod
     def _model(env_or_sys):
@@ -654,6 +673,51 @@ class DeviceLoop:
         self.plan.set_instance_delay(b, steps, predict)
         self._delay[b] = (steps, predict)
 
+    _RAND_OBSERVE = ("an observation delay needs a loop without randomize_tasks: its rollouts would start before "
+                     "the current command window (noise alone is allowed)")
+
+    @staticmethod
+    def _observing(setting) -> bool:
+        return setting[0] > 0 or bool(setting[1].any()) or bool(setting[2].any())
+
+    def _set_observation(self, b: int, setting) -> None:
+        self.plan.set_instance_observation(b, *setting)
+        self._observe[b] = setting if self._observing(setting) else None
+
+    def set_observation(self, b: int, spec) -> None:
+        """Instance b plans from an observation of its plant from the next ``step`` on (an observe spec,
+        ``observe_setting``), or from its plant state again (None).  Resets its history: the next step seeds it
+        from the plant, and its noise restarts from the spec's seed.  A stream-ordered copy on the current
+        stream.  The first observation of a loop, and a call that changes the number of prediction launches
+        (max(k + d) over the predicting instances), make the next steps capture their graphs again; other calls
+        keep them."""
+        b = self._instance(b)
+        if spec is None:
+            if self._observe[b] is not None:
+                nv = self.mbdpi.env.sys.nv
+                self._set_observation(b, (0, np.zeros(nv, np.float32), np.zeros(nv, np.float32), np.zeros(2, np.uint32)))
+            return
+        setting = observe_setting(spec, self.mbdpi.env.sys)
+        if self._rand and setting[0] > 0:
+            raise ValueError(self._RAND_OBSERVE)
+        self._set_observation(b, setting)
+
+    def observed_state(self) -> Dict[str, torch.Tensor]:
+        """The observation the last step planned from, before any prediction: new tensors ``qpos``, ``qvel``,
+        ``qacc_warmstart``, ``counters`` (int32 {step, contact_stage}) and ``age`` (int32, how many env steps
+        old the observed record is), with a leading [B] on a batched loop; the plant state at age 0 for an
+        instance without an observation.  Asynchronous on the current stream."""
+        lead = (self.n_instances,) if self.n_instances > 1 else ()
+        m = self.mbdpi.env.sys
+        i32 = dict(dtype=torch.int32, device=self.mbdpi.device)
+        out = dict(qpos=self.plan.empty(*lead, m.nq), qvel=self.plan.empty(*lead, m.nv),
+                   qacc_warmstart=self.plan.empty(*lead, m.nv), counters=torch.empty(*lead, 2, **i32),
+                   age=torch.empty(*lead, **i32) if lead else torch.empty(1, **i32))
+        self.plan.observed_state(out["qpos"], out["qvel"], out["qacc_warmstart"], out["counters"], out["age"])
+        if not lead:
+            out["age"] = out["age"][0]
+        return out
+
     def pending_actions(self) -> torch.Tensor:
         """Each instance's queued actions in the order the next env steps apply them, a new tensor [B, 16, nu]
         ([16, nu] for one instance; rows past the instance's delay are zero).  Asynchronous on the current
@@ -664,8 +728,8 @@ class DeviceLoop:
     def planning_state(self) -> Dict[str, torch.Tensor]:
         """The state the last step's planning rollouts started from, new tensors ``qpos``, ``qvel``,
         ``qacc_warmstart`` and ``counters`` (int32 {step, contact_stage}) with a leading [B] on a batched loop:
-        the predicted state of a predicting instance, the plant state of any other.  Asynchronous on the
-        current stream."""
+        the predicted state of a predicting instance, the observation of an observing one, the plant state of
+        any other.  Asynchronous on the current stream."""
         lead = (self.n_instances,) if self.n_instances > 1 else ()
         m = self.mbdpi.env.sys
         out = dict(qpos=self.plan.empty(*lead, m.nq), qvel=self.plan.empty(*lead, m.nv),
@@ -722,7 +786,8 @@ class DeviceLoop:
         """Overwrite the planning state (deploy: the state comes from the robot / simulator).  ``step``
         sets ``info["step"]`` only, like the reference's ``update_mjx_state`` (dial_plan.py:149-155):
         a seq-jump ``contact_stage`` is whatever the bound state carries.  Batched loops: [B,...]
-        arrays and ``step`` an int or [B]."""
+        arrays and ``step`` an int or [B].  Each observing instance starts its history again from the new
+        state, and its noise from its seed, as ``set_observation`` does."""
         self.buf["qpos"].copy_(self.plan.f32(qpos))
         self.buf["qvel"].copy_(self.plan.f32(qvel))
         if qacc_warmstart is not None:
@@ -735,6 +800,10 @@ class DeviceLoop:
         elif step is not None:
             self.buf["counters"][0] = int(step)
             self._env_info[0]["step"] = int(step)
+        # the observing instances start their history again from the new state (and their noise from the seed)
+        for b, setting in enumerate(self._observe):
+            if setting is not None:
+                self.plan.set_instance_observation(b, *setting)
 
     @property
     def action(self) -> torch.Tensor:
@@ -938,6 +1007,67 @@ def delay_setting(spec):
     return steps(spec), False
 
 
+OBSERVE_KEYS = ("delay", "qpos", "qvel", "seed")
+
+
+def observe_setting(spec, sys):
+    """An observe spec -> (delay, qpos_std [nv], qvel_std [nv], key) of ``dial_plan_set_instance_observation``
+    for the model of ``sys`` (a ``System``, an env or a ``CompiledModel``).  The spec maps any of ``delay`` (the
+    observation delay in control steps, 0..16, default 0), ``qpos`` and ``qvel`` (noise standard deviations,
+    default 0: one number for every dof, a list of nv, or ``{joint_name: value}`` resolved as
+    ``System.tree_replace`` resolves a dof field by joint name; a free joint takes one number or 6, 3 position
+    and 3 rotation) and ``seed`` (the noise key is ``PRNGKey(seed)``, default 0: instances with other
+    standard deviations see the same draws, scaled).  Raises ValueError naming the bad key or value."""
+    model = getattr(getattr(sys, "sys", sys), "model", getattr(sys, "sys", sys))
+    nv = model.nv
+    dmax = _capi.DEFINES["DIAL_MAXDELAY"]
+    if not isinstance(spec, dict):
+        raise ValueError(f"an observe spec is a mapping of {', '.join(OBSERVE_KEYS)}, got {spec!r}")
+    extra = sorted(set(spec) - set(OBSERVE_KEYS), key=str)
+    if extra:
+        raise ValueError(f"unknown key {extra[0]!r} (an observe spec takes {', '.join(map(repr, OBSERVE_KEYS))})")
+
+    def count(name, v, hi=None):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 0 or (hi is not None and v > hi):
+            raise ValueError(f"{name} must be an int in 0..{hi}, got {v!r}" if hi is not None else
+                             f"{name} must be an int >= 0, got {v!r}")
+        return int(v)
+
+    def std(name, v):
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)) or \
+                not math.isfinite(v) or v < 0:
+            raise ValueError(f"{name} must be a finite number >= 0, got {v!r}")
+        return float(v)
+
+    def stds(name, S):
+        out = np.zeros(nv, np.float32)
+        if isinstance(S, dict):
+            for joint, v in S.items():
+                try:
+                    rows = model._entries("joint", joint, name)
+                except KeyError:
+                    raise ValueError(f"{name}: unknown joint {joint!r} (known: {model.names.get('joint', [])})") from None
+                n = len(range(nv)[rows]) if isinstance(rows, slice) else 1
+                vals = v if isinstance(v, (list, tuple, np.ndarray)) else [v] * n
+                if len(vals) != n:
+                    raise ValueError(f"{name}: joint {joint!r} has {n} dofs: give one number or {n}, got {list(vals)!r}")
+                out[rows] = [std(f"{name}: {joint}", x) for x in vals]
+            return out
+        if isinstance(S, (list, tuple, np.ndarray)):
+            if len(S) != nv:
+                raise ValueError(f"{name} must be one number, a list of nv = {nv} or a mapping of joint names, "
+                                 f"got a list of {len(S)}")
+            out[:] = [std(f"{name}[{i}]", x) for i, x in enumerate(S)]
+            return out
+        out[:] = std(name, S)
+        return out
+
+    delay = count("delay", spec.get("delay", 0), dmax)
+    q, v = stds("qpos", spec.get("qpos", 0.0)), stds("qvel", spec.get("qvel", 0.0))
+    key = drandom.PRNGKey(count("seed", spec.get("seed", 0), 0xFFFFFFFF))
+    return delay, q, v, np.asarray(key, np.uint32)
+
+
 def load_setting(spec, key: str, K: int, nv: Optional[int] = None):
     """The ``risk``, ``adapt`` or ``prior`` entry ``key`` of an ``--ensemble`` file or an
     ``--instance-overrides`` mapping, checked for K members and nv dofs (``risk_setting``,
@@ -994,7 +1124,7 @@ def load_ensemble(spec, env):
 
 
 def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                  schedule=None, delay=None):
+                  schedule=None, delay=None, observe=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
@@ -1002,7 +1132,8 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
     under ``risk`` (one risk spec or B of them, ``DeviceLoop(..., risk=...)``), adapting to the plant under
     ``adapt`` from the belief ``prior`` (``DeviceLoop(..., adapt=..., prior=...)``).  ``schedule``: B schedule
     specs or None (``DeviceLoop(..., schedule=...)``); each instance runs its own Ndiffuse_init, then Ndiffuse.
-    ``delay``: one delay spec or B of them (``DeviceLoop(..., delay=...)``)."""
+    ``delay``: one delay spec or B of them (``DeviceLoop(..., delay=...)``).  ``observe``: one observe spec or B
+    of them (``DeviceLoop(..., observe=...)``)."""
     mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
@@ -1010,7 +1141,7 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
     loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior,
-                      schedule=schedule, delay=delay)
+                      schedule=schedule, delay=delay, observe=observe)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -1083,6 +1214,12 @@ def main():
                              "robot at step t + STEPS (0..16); ':predict' plans from the state predicted STEPS steps "
                              "ahead through the queued actions; an --instance-overrides mapping may carry its own "
                              "'delay' (an int or {steps: d, predict: true})")
+    parser.add_argument("--observe", type=str, default=None, metavar="SPEC",
+                        help="every instance plans from an observation of its simulated robot: a YAML flow mapping "
+                             "such as '{delay: 2, qpos: 0.01, qvel: 0.1, seed: 0}', the record 'delay' control "
+                             "steps old (0..16) with Gaussian noise of standard deviation 'qpos' / 'qvel' (one number, "
+                             "nv numbers or a mapping of joint names); an --instance-overrides mapping may carry its "
+                             "own 'observe'")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -1115,10 +1252,25 @@ def main():
             delay = delay_setting({"steps": int(steps), "predict": bool(sep)})
         except ValueError as e:
             parser.error(f"--delay: {e}")
+    observe = None
+    if args.observe is not None:
+        if args.eager:
+            parser.error("--observe runs on the CUDA-graph loop; it excludes --eager")
+        try:
+            observe = yaml.safe_load(args.observe)
+        except yaml.YAMLError as e:
+            parser.error(f"--observe: not a YAML mapping: {e}")
     rng = drandom.PRNGKey(seed=dial_config.seed)
     env_config_type = dial_envs.get_config(dial_config.env_name)
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
     env = dial_envs.get_environment(dial_config.env_name, config=env_config)
+    if observe is not None:
+        try:
+            observe_setting(observe, env.sys)
+            if observe.get("delay", 0) > 0 and getattr(env_config, "randomize_tasks", False):
+                raise ValueError(DeviceLoop._RAND_OBSERVE)
+        except ValueError as e:
+            parser.error(f"--observe: {e}")
     envs = None
     members, plant, risk, adapt, prior = None, None, None, None, None
     if args.ensemble is not None:
@@ -1142,16 +1294,17 @@ def main():
         # DialConfig fields: the sampling schedule (SCHEDULE_FIELDS), or fields shared by the plan, which
         # schedule_setting rejects by name
         dial_fields = {f.name for f in dataclasses.fields(DialConfig)} - env_fields
-        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay"}
+        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay", "observe"}
         envs = []
         settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
         uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
         schedule = [None] * args.instances
         delays = [delay] * args.instances
+        observes = [observe] * args.instances
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt, delay "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt, delay, observe "
                              f"or the sampling fields {', '.join(SCHEDULE_FIELDS)}, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
@@ -1169,6 +1322,15 @@ def main():
                 except ValueError as e:
                     parser.error(f"--instance-overrides entry {b}: delay: {e}")
             ov.pop("delay", None)
+            if ov.get("observe") is not None:
+                try:
+                    observe_setting(ov["observe"], env.sys)
+                    if ov["observe"].get("delay", 0) > 0 and getattr(env_config, "randomize_tasks", False):
+                        raise ValueError(DeviceLoop._RAND_OBSERVE)
+                except ValueError as e:
+                    parser.error(f"--instance-overrides entry {b}: observe: {e}")
+                observes[b] = ov["observe"]
+            ov.pop("observe", None)
             for key in ("risk", "adapt"):
                 if ov.get(key) is not None:
                     if members is None:
@@ -1205,10 +1367,12 @@ def main():
             adapt = settings["adapt"]
         if args.instance_overrides is not None and any(d is not None for d in delays):
             delay = [d or (0, False) for d in delays]
+        if args.instance_overrides is not None and any(o is not None for o in observes):
+            observe = observes
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
                       ensemble=members, risk=risk, adapt=adapt, prior=prior,
                       schedule=schedule if args.instance_overrides is not None and any(schedule) else None,
-                      delay=None if delay is None else _delay_specs(delay))
+                      delay=None if delay is None else _delay_specs(delay), observe=observe)
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
@@ -1219,10 +1383,13 @@ def main():
     rews, rollout, infos = [], [], []
     if delay is not None and mbdpi.world_size != 1:
         parser.error("--delay needs an unsharded plan (one process)")
+    if observe is not None and mbdpi.world_size != 1:
+        parser.error("--observe needs an unsharded plan (one process)")
     if mbdpi.world_size == 1 and not args.eager:
         # one CUDA graph per control step; the host launches it and logs
         loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk,
-                          adapt=adapt, prior=prior, delay=None if delay is None else _delay_specs(delay))
+                          adapt=adapt, prior=prior, delay=None if delay is None else _delay_specs(delay),
+                          observe=observe)
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):

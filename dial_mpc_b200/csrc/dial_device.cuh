@@ -749,6 +749,145 @@ DEV float jax_normal_legacy(uint32_t k0, uint32_t k1, uint32_t i, uint32_t n) {
 }
 
 // ---------------------------------------------------------------------------------
+// per-instance observation (dial_plan_set_instance_observation)
+// ---------------------------------------------------------------------------------
+// Instance b's observation setting (dial_plan_set_instance_observation): the observation delay k in control
+// steps, whether the instance observes (k > 0 or some sigma > 0; else it plans from its plant state), the key
+// a reset restarts its noise from, and the noise standard deviations: sigma[i] on qpos dof i (tangent space),
+// sigma[nv + i] on qvel dof i.
+struct alignas(8) ObsSetting {
+  int32_t k;
+  int32_t on;
+  uint32_t key[2];
+  float sigma[2 * DIAL_MAXV];
+};
+#define DIAL_OBSRING (DIAL_MAXDELAY + 1)   // plant records of one instance: ages 0..DIAL_MAXDELAY
+// An instance's ring of plant records: the slot of the newest, the records since the reset (counting the
+// seed, saturating at DIAL_OBSRING; 0: the next observe step seeds), the running noise key and the key of
+// the last draw.
+struct alignas(8) ObsRing {
+  int32_t head, count;
+  uint32_t key[2], sub[2];
+};
+// One instance's slices of the buffers an observe step reads and writes: the plant state and the action its
+// last env step applied (null: none), the ring's records [DIAL_OBSRING][*], the observation, the planning
+// state the prediction starts from, the prediction's actions [DIAL_MAXDELAY][nu] and the pending actions of
+// the delay queue [DIAL_MAXDELAY][nu] (null: no queue).
+struct ObsView {
+  const float *qpos, *qvel, *warm, *act;
+  const int32_t* cnt;
+  float *rq, *rv, *rw, *ra;
+  int32_t* rc;
+  float *oq, *ov, *ow;
+  int32_t* oc;
+  float *pq, *pv, *pw;
+  int32_t* pc;
+  float* seq;
+  const float* pending;
+};
+// The ring after one observe step: an observing instance pushes a record in a step with an env step, and
+// seeds one after a reset; each new record draws its noise key, (key, sub) = split(key).
+DEV bool observe_pushes(const ObsSetting& s, const ObsRing& r, bool env_step) { return s.on && (r.count == 0 || env_step); }
+DEV ObsRing observe_advance(const ObsSetting& s, ObsRing r, bool env_step) {
+  if (!observe_pushes(s, r, env_step)) return r;
+  r.head = r.count == 0 ? 0 : (r.head + 1 == DIAL_OBSRING ? 0 : r.head + 1);
+  r.count = r.count < DIAL_OBSRING ? r.count + 1 : DIAL_OBSRING;
+  uint32_t n0, n1, s0, s1;
+  split_rng(r.key[0], r.key[1], n0, n1);
+  split_key(r.key[0], r.key[1], s0, s1);
+  r.key[0] = n0; r.key[1] = n1; r.sub[0] = s0; r.sub[1] = s1;
+  return r;
+}
+// The age of the record an instance observes: min(k, count - 1), the oldest record while the ring fills.
+DEV int observe_age(const ObsSetting& s, const ObsRing& r) {
+  if (!s.on) return 0;
+  return s.k < r.count - 1 ? s.k : r.count - 1;
+}
+// Stage 1 of an observe step, for the elements a = a0, a0 + da, ... (a CTA passes its threads): when the step
+// pushes (observe_pushes), the new record (slot r1.head, r1 = observe_advance(...)) takes the plant state, its
+// counters and the applied action (zero without one).  Each element is read and written by one caller only.
+DEV void observe_record(bool push, const ObsRing& r1, const ObsView& V, int nq, int nv, int nu, int a0, int da) {
+  if (!push) return;
+  const int h = r1.head;
+  for (int i = a0; i < nq; i += da) V.rq[h * nq + i] = V.qpos[i];
+  for (int i = a0; i < nv; i += da) { V.rv[h * nv + i] = V.qvel[i]; V.rw[h * nv + i] = V.warm[i]; }
+  for (int i = a0; i < nu; i += da) V.ra[h * nu + i] = V.act ? V.act[i] : 0.f;
+  if (a0 == 0) { V.rc[2 * h] = V.cnt[0]; V.rc[2 * h + 1] = V.cnt[1]; }
+}
+// x + sigma eps, and x itself, bit for bit, where sigma is 0
+DEV float observe_noisy(float x, float sigma, float eps) { return sigma == 0.f ? x : fmaf(sigma, eps, x); }
+// q composed with the rotation w (body frame) as physics_step integrates a free joint's orientation:
+// qnormalize(q * axisangle(w / |w|, |w|))
+DEV Q4 observe_rotate(Q4 q, V3 w) {
+  const float nrm = sqrtf(dot(w, w));
+  const V3 ax = w * (1.f / (nrm + 1e-6f * (nrm == 0.f ? 1.f : 0.f)));
+  return qnormalize(qmul(q, axisangle(ax, nrm)));
+}
+// Stage 2 of an observe step (after stage 1 of every element), for the elements a0, a0 + da, ...: the
+// observation (the record `age` pushes back plus the noise of the newest record's draw; the plant state of an
+// instance that does not observe) into V.o* and V.p*, and the prediction's actions: `age` history rows (the
+// actions applied since the observed record, oldest first), then the d pending rows, then zero rows.  The
+// prediction length is age + d (the caller applies the predict flag).
+DEV void observe_emit(const ObsSetting& s, const ObsRing& r1, const dial_model_desc& m, int d, const ObsView& V,
+                      int a0, int da) {
+  const int nq = m.nq, nv = m.nv, nu = m.nu;
+  const int age = observe_age(s, r1);
+  const int h = s.on ? (r1.head - age < 0 ? r1.head - age + DIAL_OBSRING : r1.head - age) : 0;
+  const float* q = s.on ? V.rq + h * nq : V.qpos;
+  const float* v = s.on ? V.rv + h * nv : V.qvel;
+  const float* w = s.on ? V.rw + h * nv : V.warm;
+  const int32_t* c = s.on ? V.rc + 2 * h : V.cnt;
+  const uint32_t k0 = r1.sub[0], k1 = r1.sub[1];
+  const uint32_t n = 2u * (uint32_t)nv;
+  const float* sg = s.sigma;
+  for (int j = a0; j < m.njnt; j += da) {
+    const int qa = m.jnt_qposadr[j], dd = m.jnt_dofadr[j], t = m.jnt_type[j];
+    int qr = -1, dr = -1;   // quaternion address and its three rotation dofs (free and ball joints)
+    if (t == JNT_FREE) {
+      for (int i = 0; i < 3; ++i) {
+        const float x = !s.on ? q[qa + i] : observe_noisy(q[qa + i], sg[dd + i],
+                                                          sg[dd + i] == 0.f ? 0.f : jax_normal_legacy(k0, k1, dd + i, n));
+        V.oq[qa + i] = x; V.pq[qa + i] = x;
+      }
+      qr = qa + 3; dr = dd + 3;
+    } else if (t == JNT_BALL) {
+      qr = qa; dr = dd;
+    } else {
+      const float x = !s.on || sg[dd] == 0.f ? q[qa] : observe_noisy(q[qa], sg[dd], jax_normal_legacy(k0, k1, dd, n));
+      V.oq[qa] = x; V.pq[qa] = x;
+    }
+    if (qr >= 0) {
+      Q4 o = ldq(q + qr);
+      if (s.on && (sg[dr] != 0.f || sg[dr + 1] != 0.f || sg[dr + 2] != 0.f)) {
+        V3 e = v3(0.f, 0.f, 0.f);
+        if (sg[dr] != 0.f) e.x = sg[dr] * jax_normal_legacy(k0, k1, dr, n);
+        if (sg[dr + 1] != 0.f) e.y = sg[dr + 1] * jax_normal_legacy(k0, k1, dr + 1, n);
+        if (sg[dr + 2] != 0.f) e.z = sg[dr + 2] * jax_normal_legacy(k0, k1, dr + 2, n);
+        o = observe_rotate(o, e);
+      }
+      stq(V.oq + qr, o); stq(V.pq + qr, o);
+    }
+  }
+  for (int i = a0; i < nv; i += da) {
+    const float x = !s.on || sg[nv + i] == 0.f ? v[i] : observe_noisy(v[i], sg[nv + i], jax_normal_legacy(k0, k1, nv + i, n));
+    V.ov[i] = x; V.pv[i] = x;
+    V.ow[i] = w[i]; V.pw[i] = w[i];
+  }
+  if (a0 == 0) { V.oc[0] = c[0]; V.oc[1] = c[1]; V.pc[0] = c[0]; V.pc[1] = c[1]; }
+  for (int a = a0; a < nu; a += da)
+    for (int j = 0; j < DIAL_MAXDELAY; ++j) {
+      float u = 0.f;
+      if (j < age) {
+        const int back = age - 1 - j, sl = r1.head - back;   // the record j + 1 steps after the observed one
+        u = V.ra[(sl < 0 ? sl + DIAL_OBSRING : sl) * nu + a];
+      } else if (j < age + d && V.pending) {
+        u = V.pending[(j - age) * nu + a];
+      }
+      V.seq[j * nu + a] = u;
+    }
+}
+
+// ---------------------------------------------------------------------------------
 // per-warp context
 // ---------------------------------------------------------------------------------
 // "Compact chain coordinates": the mass matrix M and the Newton Hessian H = M + J^T D J of

@@ -13,6 +13,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <float.h>
+#include <cmath>
 #include <memory>
 #include <string>
 #include <vector>
@@ -644,6 +645,65 @@ __global__ void __launch_bounds__(128) delay_refill_kernel(int b, int d, int32_t
   if (threadIdx.x == 0) head[b] = 0;
 }
 
+// The buffers of the observation (dial_plan_set_instance_observation), instance-major: the rings [B], their
+// records [B][DIAL_OBSRING][*], the observation [B][*] and its age [B], the prediction's actions
+// [B][DIAL_MAXDELAY][nu] and lengths [B].
+struct ObsBuffers {
+  ObsRing* ring;
+  float *rq, *rv, *rw, *ra;
+  int32_t* rc;
+  float *oq, *ov, *ow;
+  int32_t *oc, *age;
+  float* seq;
+  int32_t* len;
+};
+
+// Observation, one CTA per instance b, after the plant's env step and the shift: its ring's step (a record
+// pushed in a step with an env step, seeded after a reset; observe_advance / observe_record), its observation
+// (observe_emit) into the observed state and the planning state (pq.. [B][*]), the prediction's actions and
+// the prediction length (age + d_b when b predicts through its delay setting `dset`, else 0).  `act`: the
+// actions the env step applied, one row of act_row floats per instance.
+__global__ void __launch_bounds__(128) observe_kernel(const DevModel* __restrict__ M, const ObsSetting* __restrict__ set,
+                                                      ObsBuffers O, const DelaySetting* __restrict__ dset,
+                                                      const float* __restrict__ pending, int env_step,
+                                                      const float* __restrict__ qpos, const float* __restrict__ qvel,
+                                                      const float* __restrict__ warm, const int32_t* __restrict__ cnt,
+                                                      const float* __restrict__ act, int act_row, float* __restrict__ pq,
+                                                      float* __restrict__ pv, float* __restrict__ pw, int32_t* __restrict__ pc) {
+  const int b = blockIdx.x;
+  const dial_model_desc& m = M->m;
+  const size_t nq = m.nq, nv = m.nv, nu = m.nu, R = DIAL_OBSRING;
+  const ObsSetting& s = set[b];
+  const ObsRing r = O.ring[b];
+  const DelaySetting ds = dset ? dset[b] : DelaySetting{0, 0};
+  const ObsRing r1 = observe_advance(s, r, env_step != 0);
+  ObsView V;
+  V.qpos = qpos + b * nq; V.qvel = qvel + b * nv; V.warm = warm + b * nv; V.cnt = cnt + 2 * b;
+  V.act = env_step ? act + b * act_row : nullptr;
+  V.rq = O.rq + b * R * nq; V.rv = O.rv + b * R * nv; V.rw = O.rw + b * R * nv; V.ra = O.ra + b * R * nu;
+  V.rc = O.rc + b * R * 2;
+  V.oq = O.oq + b * nq; V.ov = O.ov + b * nv; V.ow = O.ow + b * nv; V.oc = O.oc + 2 * b;
+  V.pq = pq + b * nq; V.pv = pv + b * nv; V.pw = pw + b * nv; V.pc = pc + 2 * b;
+  V.seq = O.seq + b * DIAL_MAXDELAY * nu;
+  V.pending = pending ? pending + b * DIAL_MAXDELAY * nu : nullptr;
+  observe_record(observe_pushes(s, r, env_step != 0), r1, V, (int)nq, (int)nv, (int)nu, threadIdx.x, blockDim.x);
+  __syncthreads();   // the new record is complete, and every thread has read ring[b]
+  observe_emit(s, r1, m, ds.d, V, threadIdx.x, blockDim.x);
+  if (threadIdx.x == 0) {
+    const int age = observe_age(s, r1);
+    O.ring[b] = r1; O.age[b] = age; O.len[b] = ds.predict ? age + ds.d : 0;
+  }
+}
+
+// dial_plan_set_instance_observation: instance b's ring reset (the next observe step seeds it), its noise
+// key that of its setting
+__global__ void observe_reset_kernel(int b, const ObsSetting* __restrict__ set, ObsRing* __restrict__ ring) {
+  ObsRing r;
+  r.head = 0; r.count = 0;
+  r.key[0] = set[b].key[0]; r.key[1] = set[b].key[1]; r.sub[0] = 0u; r.sub[1] = 0u;
+  ring[b] = r;
+}
+
 // ---------------------------------------------------------------------------------
 // plan object
 // ---------------------------------------------------------------------------------
@@ -752,8 +812,9 @@ struct dial_plan {
   // per-instance control latency (dial_plan_set_instance_delay): the settings [n_inst] (the staging mirrors
   // the device), and, allocated with them, the queues' front slots [n_inst] and rings [n_inst][DIAL_MAXDELAY][nu],
   // the applied actions [n_inst][nu], the queues in application order [n_inst][DIAL_MAXDELAY][nu], the
-  // prediction lengths [n_inst], the planning state (qpos, qvel, warm start, counters) and, on an ensemble
-  // plan, the planning models [n_inst] (a copy of member (b, 0)).  dl_max / dl_pred: the largest delay, and
+  // prediction lengths [n_inst], and the planning state (qpos, qvel, warm start, counters) and, on an ensemble
+  // plan, the planning models [n_inst] (a copy of member (b, 0)), which dial_plan_set_instance_observation
+  // allocates instead when it runs first.  dl_max / dl_pred: the largest delay, and
   // that of the predicting instances (the number of prediction launches), as set on the host.
   Staged<DelaySetting> delay;
   int32_t* dl_head = nullptr;
@@ -766,6 +827,15 @@ struct dial_plan {
   DevModel* dl_models = nullptr;
   int dl_max = 0, dl_pred = 0;
   int dl_pred_last = 0;   // dl_pred of the last dial_mpc_step (its graph's launch sequence)
+  // per-instance observation (dial_plan_set_instance_observation): the settings [n_inst] (the staging mirrors
+  // the device) and, allocated with them by the first call, the rings and observations (ObsBuffers; the
+  // planning state above is allocated by whichever of the two setters runs first).  ob_pred: the number of
+  // prediction launches while the observe launch runs, max(k_b + d_b) over the predicting instances, as set
+  // on the host; ob_last: the last dial_mpc_step ran the observe launch.
+  Staged<ObsSetting> obs;
+  ObsBuffers ob{};
+  int ob_pred = 0;
+  bool ob_last = false;
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -1038,6 +1108,11 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   p->delay.release();
   cudaFree(p->dl_head); cudaFree(p->dl_ring); cudaFree(p->dl_applied); cudaFree(p->dl_pending); cudaFree(p->dl_len);
   cudaFree(p->dl_qpos); cudaFree(p->dl_qvel); cudaFree(p->dl_warm); cudaFree(p->dl_cnt); cudaFree(p->dl_models);
+  p->obs.release();
+  for (void* d : {(void*)p->ob.ring, (void*)p->ob.rq, (void*)p->ob.rv, (void*)p->ob.rw, (void*)p->ob.ra, (void*)p->ob.rc,
+                  (void*)p->ob.oq, (void*)p->ob.ov, (void*)p->ob.ow, (void*)p->ob.oc, (void*)p->ob.age, (void*)p->ob.seq,
+                  (void*)p->ob.len})
+    cudaFree(d);
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   cudaFree(p->weights2);
@@ -1322,20 +1397,17 @@ extern "C" int dial_plan_set_instance_iterations(dial_plan* p, const int32_t* n_
   return 0;
 }
 
-// First dial_plan_set_instance_delay: the queues, the planning state and (ensemble plans) the planning models,
-// member (b, 0) of each instance as the member slots hold it, else the plan's model.
-static cudaError_t allocate_delay(dial_plan* p, cudaStream_t st) {
-  const size_t B = (size_t)p->n_inst, nu = p->hM.m.nu, nq = p->hM.m.nq, nv = p->hM.m.nv;
-  cudaError_t e = p->delay.allocate(B, 1, DelaySetting{0, 0});
+// The planning state (qpos, qvel, warm start, counters) and, on an ensemble plan, the planning models (member
+// (b, 0) of each instance as the member slots hold it, else the plan's model), allocated by the first
+// dial_plan_set_instance_delay or dial_plan_set_instance_observation.
+static cudaError_t allocate_planning(dial_plan* p, cudaStream_t st) {
+  if (p->dl_qpos) return cudaSuccess;
+  const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv;
+  cudaError_t e = cudaSuccess;
   auto dev = [&](auto*& ptr, size_t bytes) {
     if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes);
     if (e == cudaSuccess) e = cudaMemsetAsync(ptr, 0, bytes, st);
   };
-  dev(p->dl_head, B * sizeof(int32_t));
-  dev(p->dl_ring, B * DIAL_MAXDELAY * nu * sizeof(float));
-  dev(p->dl_applied, B * nu * sizeof(float));
-  dev(p->dl_pending, B * DIAL_MAXDELAY * nu * sizeof(float));
-  dev(p->dl_len, B * sizeof(int32_t));
   dev(p->dl_qpos, B * nq * sizeof(float));
   dev(p->dl_qvel, B * nv * sizeof(float));
   dev(p->dl_warm, B * nv * sizeof(float));
@@ -1347,15 +1419,85 @@ static cudaError_t allocate_delay(dial_plan* p, cudaStream_t st) {
                        : cudaMemcpy(p->dl_models + b, &p->hM, sizeof(DevModel), cudaMemcpyHostToDevice);
   }
   if (e != cudaSuccess) {
-    p->delay.release();
-    for (void* d : {(void*)p->dl_head, (void*)p->dl_ring, (void*)p->dl_applied, (void*)p->dl_pending, (void*)p->dl_len,
-                    (void*)p->dl_qpos, (void*)p->dl_qvel, (void*)p->dl_warm, (void*)p->dl_cnt, (void*)p->dl_models})
-      cudaFree(d);
-    p->dl_head = p->dl_len = p->dl_cnt = nullptr;
-    p->dl_ring = p->dl_applied = p->dl_pending = p->dl_qpos = p->dl_qvel = p->dl_warm = nullptr;
+    for (void* d : {(void*)p->dl_qpos, (void*)p->dl_qvel, (void*)p->dl_warm, (void*)p->dl_cnt, (void*)p->dl_models}) cudaFree(d);
+    p->dl_qpos = p->dl_qvel = p->dl_warm = nullptr;
+    p->dl_cnt = nullptr;
     p->dl_models = nullptr;
   }
   return e;
+}
+
+// First dial_plan_set_instance_delay: the queues (and the planning state, if not yet allocated).
+static cudaError_t allocate_delay(dial_plan* p, cudaStream_t st) {
+  const size_t B = (size_t)p->n_inst, nu = p->hM.m.nu;
+  cudaError_t e = allocate_planning(p, st);
+  if (e == cudaSuccess) e = p->delay.allocate(B, 1, DelaySetting{0, 0});
+  auto dev = [&](auto*& ptr, size_t bytes) {
+    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ptr, 0, bytes, st);
+  };
+  dev(p->dl_head, B * sizeof(int32_t));
+  dev(p->dl_ring, B * DIAL_MAXDELAY * nu * sizeof(float));
+  dev(p->dl_applied, B * nu * sizeof(float));
+  dev(p->dl_pending, B * DIAL_MAXDELAY * nu * sizeof(float));
+  dev(p->dl_len, B * sizeof(int32_t));
+  if (e != cudaSuccess) {
+    p->delay.release();
+    for (void* d : {(void*)p->dl_head, (void*)p->dl_ring, (void*)p->dl_applied, (void*)p->dl_pending, (void*)p->dl_len})
+      cudaFree(d);
+    p->dl_head = p->dl_len = nullptr;
+    p->dl_ring = p->dl_applied = p->dl_pending = nullptr;
+  }
+  return e;
+}
+
+// First dial_plan_set_instance_observation: the settings, rings and observations (and the planning state, if
+// not yet allocated).  Every ring starts empty.
+static cudaError_t allocate_observation(dial_plan* p, cudaStream_t st) {
+  const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv, nu = p->hM.m.nu, R = DIAL_OBSRING;
+  cudaError_t e = allocate_planning(p, st);
+  ObsSetting off;
+  memset(&off, 0, sizeof(off));
+  if (e == cudaSuccess) e = p->obs.allocate(B, 1, off);
+  ObsBuffers& O = p->ob;
+  auto dev = [&](auto*& ptr, size_t bytes) {
+    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ptr, 0, bytes, st);
+  };
+  dev(O.ring, B * sizeof(ObsRing));
+  dev(O.rq, B * R * nq * sizeof(float));
+  dev(O.rv, B * R * nv * sizeof(float));
+  dev(O.rw, B * R * nv * sizeof(float));
+  dev(O.ra, B * R * nu * sizeof(float));
+  dev(O.rc, B * R * 2 * sizeof(int32_t));
+  dev(O.oq, B * nq * sizeof(float));
+  dev(O.ov, B * nv * sizeof(float));
+  dev(O.ow, B * nv * sizeof(float));
+  dev(O.oc, B * 2 * sizeof(int32_t));
+  dev(O.age, B * sizeof(int32_t));
+  dev(O.seq, B * DIAL_MAXDELAY * nu * sizeof(float));
+  dev(O.len, B * sizeof(int32_t));
+  if (e != cudaSuccess) {
+    p->obs.release();
+    for (void* d : {(void*)O.ring, (void*)O.rq, (void*)O.rv, (void*)O.rw, (void*)O.ra, (void*)O.rc, (void*)O.oq,
+                    (void*)O.ov, (void*)O.ow, (void*)O.oc, (void*)O.age, (void*)O.seq, (void*)O.len})
+      cudaFree(d);
+    O = ObsBuffers{};
+  }
+  return e;
+}
+
+// The number of prediction launches of the current settings: max(k_b + d_b) over the predicting instances
+// while the observe launch runs (k_b of an observing instance, else 0), max(d_b) over them without it
+// (staging = device).
+static int prediction_launches(const dial_plan* p) {
+  int n = 0;
+  for (int b = 0; p->delay.d && b < p->n_inst; ++b) {
+    const DelaySetting& s = p->delay.h[b];
+    const int k = p->obs.d && p->obs.h[b].on ? p->obs.h[b].k : 0;
+    if (s.predict && s.d + k > n) n = s.d + k;
+  }
+  return n;
 }
 
 extern "C" int dial_plan_set_instance_delay(dial_plan* p, int b, int steps, int predict, void* stream) {
@@ -1367,6 +1509,9 @@ extern "C" int dial_plan_set_instance_delay(dial_plan* p, int b, int steps, int 
   if (steps < 0 || steps > DIAL_MAXDELAY)
     return fail(std::string(fn) + ": steps " + std::to_string(steps) + " out of range (0.." DIAL_STR(DIAL_MAXDELAY) ")");
   if (predict != 0 && predict != 1) return fail(std::string(fn) + ": predict must be 0 or 1, got " + std::to_string(predict));
+  if (p->obs.d && steps + p->obs.h[b].k > DIAL_MAXDELAY)
+    return fail(std::string(fn) + ": steps " + std::to_string(steps) + " plus instance " + std::to_string(b) +
+                "'s observation delay " + std::to_string(p->obs.h[b].k) + " exceeds " DIAL_STR(DIAL_MAXDELAY));
   if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first (the queue is filled from the bound Y)");
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaSuccess;
@@ -1389,6 +1534,81 @@ extern "C" int dial_plan_set_instance_delay(dial_plan* p, int b, int steps, int 
   }
   if (dmax != p->dl_max || dpred != p->dl_pred) drop_graphs(p);
   p->dl_max = dmax; p->dl_pred = dpred;
+  if (p->obs.d) {   // with the observe launch, the prediction's length also counts the observation delays
+    const int n = prediction_launches(p);
+    if (n != p->ob_pred) drop_graphs(p);
+    p->ob_pred = n;
+  }
+  return 0;
+}
+
+extern "C" int dial_plan_set_instance_observation(dial_plan* p, int b, int delay, const float* qpos_std,
+                                                  const float* qvel_std, const uint32_t key[2], void* stream) {
+  static const char* fn = "dial_plan_set_instance_observation";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (int rc = need_instance(p, fn, b)) return rc;
+  if (delay < 0 || delay > DIAL_MAXDELAY)
+    return fail(std::string(fn) + ": delay " + std::to_string(delay) + " out of range (0.." DIAL_STR(DIAL_MAXDELAY) ")");
+  const int d = p->delay.d ? p->delay.h[b].d : 0;
+  if (delay + d > DIAL_MAXDELAY)
+    return fail(std::string(fn) + ": delay " + std::to_string(delay) + " plus instance " + std::to_string(b) +
+                "'s action delay " + std::to_string(d) + " exceeds " DIAL_STR(DIAL_MAXDELAY));
+  const int nv = p->hM.m.nv;
+  bool noisy = false;
+  for (int w = 0; w < 2; ++w) {
+    const float* sd = w == 0 ? qpos_std : qvel_std;
+    for (int i = 0; sd && i < nv; ++i) {
+      if (!(sd[i] >= 0.f) || !std::isfinite(sd[i]))
+        return fail(std::string(fn) + ": " + (w == 0 ? "qpos_std[" : "qvel_std[") + std::to_string(i) + "] = " +
+                    std::to_string(sd[i]) + " must be finite and >= 0");
+      noisy |= sd[i] != 0.f;
+    }
+  }
+  const dial_plan_desc& c = p->hP.c;
+  if (c.Ntotal != c.Nsample || p->xch.on) return fail(std::string(fn) + ": sharded plans (Ntotal != Nsample) have no per-instance observation");
+  if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (!p->obs.d) {
+    // first call: the graphs captured so far plan from the plant state
+    if ((e = allocate_observation(p, st)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+    drop_graphs(p);
+  }
+  e = p->obs.put(b, [&](ObsSetting* s) {
+    s->k = delay; s->on = delay > 0 || noisy;
+    s->key[0] = key ? key[0] : 0u; s->key[1] = key ? key[1] : 0u;
+    for (int i = 0; i < 2 * DIAL_MAXV; ++i) s->sigma[i] = 0.f;
+    for (int i = 0; i < nv; ++i) { s->sigma[i] = qpos_std ? qpos_std[i] : 0.f; s->sigma[nv + i] = qvel_std ? qvel_std[i] : 0.f; }
+  }, st);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  observe_reset_kernel<<<1, 1, 0, st>>>(b, p->obs.d, p->ob.ring);
+  CUDA_OK(cudaGetLastError());
+  const int n = prediction_launches(p);
+  if (n != p->ob_pred) drop_graphs(p);
+  p->ob_pred = n;
+  return 0;
+}
+
+extern "C" int dial_plan_observed_state(dial_plan* p, float* qpos, float* qvel, float* warm, int32_t* counters,
+                                        int32_t* age, void* stream) {
+  static const char* fn = "dial_plan_observed_state";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
+  const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv;
+  // the observation of the last step when it ran the observe launch, else the plant state at age 0
+  const bool ob = p->ob_last;
+  cudaStream_t st = (cudaStream_t)stream;
+  const auto cp = [&](void* dst, const void* src, size_t bytes) {
+    return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
+  };
+  CUDA_OK(cp(qpos, ob ? p->ob.oq : p->mpc.qpos, B * nq * sizeof(float)));
+  CUDA_OK(cp(qvel, ob ? p->ob.ov : p->mpc.qvel, B * nv * sizeof(float)));
+  CUDA_OK(cp(warm, ob ? p->ob.ow : p->mpc.qacc_warmstart, B * nv * sizeof(float)));
+  CUDA_OK(cp(counters, ob ? p->ob.oc : p->mpc.counters, B * 2 * sizeof(int32_t)));
+  if (age) {
+    if (ob) CUDA_OK(cp(age, p->ob.age, B * sizeof(int32_t)));
+    else CUDA_OK(cudaMemsetAsync(age, 0, B * sizeof(int32_t), st));
+  }
   return 0;
 }
 
@@ -1409,7 +1629,7 @@ extern "C" int dial_plan_planning_state(dial_plan* p, float* qpos, float* qvel, 
   const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv;
   // the last step planned from the predicted state when it predicted (then the other instances' rows hold
   // their plant state, copied in that step)
-  const bool pred = p->dl_pred_last > 0;
+  const bool pred = p->dl_pred_last > 0 || p->ob_last;
   cudaStream_t st = (cudaStream_t)stream;
   const auto cp = [&](void* dst, const void* src, size_t bytes) {
     return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
@@ -1691,8 +1911,11 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
   // then applies the action each queue pops (dl_applied, one row of nu per instance) instead of Y[b][0]; while
   // some instance predicts, the queue launch also lays out the pending actions in the other steps
   const bool delay = p->delay.d != nullptr;
-  const int npred = delay ? p->dl_pred : 0;
-  if (delay && (env_step == 1 || npred > 0)) {
+  // observation, once some instance was given a setting: the observe launch after the env step and the shift
+  // writes every instance's planning state, and the prediction runs max(k_b + d_b) launches
+  const bool obs = p->obs.d != nullptr;
+  const int npred = obs ? p->ob_pred : delay ? p->dl_pred : 0;
+  if (delay && (env_step == 1 || p->dl_pred > 0)) {
     delay_queue_kernel<<<ni, 128, 0, st>>>(p->delay.d, p->dl_head, p->dl_ring, Y[cur], n1, nu, env_step == 1,
                                            p->dl_applied, p->dl_pending, p->dl_len);
     p->launches++;
@@ -1744,28 +1967,37 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
   // The planning state: the plant state, or once some instance predicts, a copy of it in which each predicting
   // instance b takes d_b env steps with its queued actions on its planning model (launch j: one row per
   // instance, action pending[b][j], in place; an instance with pred_len[b] <= j exits at entry)
+  // With the observe launch, the copy is its observation instead (the plant state of an instance that does not
+  // observe), and a predicting instance b takes age_b + d_b env steps: the actions applied since the observed
+  // record, then its queue (launch j: action seq[b][j]; pred_len[b] = age_b + d_b).
   const float *qpos0 = B.qpos, *qvel0 = B.qvel, *warm0 = B.qacc_warmstart;
   const int32_t* cnt0 = B.counters;
-  if (npred > 0) {
+  if (obs) {
+    observe_kernel<<<ni, 128, 0, st>>>(p->dM, p->obs.d, p->ob, delay ? p->delay.d : nullptr, delay ? p->dl_pending : nullptr,
+                                       env_step == 1, B.qpos, B.qvel, B.qacc_warmstart, B.counters, act, act_n1 * nu,
+                                       p->dl_qpos, p->dl_qvel, p->dl_warm, p->dl_cnt);
+    p->launches++;
+    CUDA_OK(cudaGetLastError());
+  } else if (npred > 0) {
     const size_t nq = p->hM.m.nq, nv = p->hM.m.nv;
     CUDA_OK(cudaMemcpyAsync(p->dl_qpos, B.qpos, ni * nq * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CUDA_OK(cudaMemcpyAsync(p->dl_qvel, B.qvel, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CUDA_OK(cudaMemcpyAsync(p->dl_warm, B.qacc_warmstart, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CUDA_OK(cudaMemcpyAsync(p->dl_cnt, B.counters, ni * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-    for (int j = 0; j < npred; ++j) {
-      RolloutArgs A; memset(&A, 0, sizeof(A));
-      A.qpos0 = p->dl_qpos; A.qvel0 = p->dl_qvel; A.warm0 = p->dl_warm;
-      A.counters_in = p->dl_cnt; A.counters_out = p->dl_cnt;
-      A.nrows = ni; A.H = 1; A.mode = 0; A.rows_per_inst = 1;
-      A.us = p->dl_pending + (size_t)j * nu; A.us_row = DIAL_MAXDELAY * nu;
-      if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
-      A.models = p->n_ens > 0 ? p->dl_models : p->models.d;
-      A.iter_lim = p->dl_len; A.iter = j;
-      A.qpos_out = p->dl_qpos; A.qvel_out = p->dl_qvel; A.warm_out = p->dl_warm;
-      CUDA_OK(launch_rollout(p, A, 1, st));
-    }
-    qpos0 = p->dl_qpos; qvel0 = p->dl_qvel; warm0 = p->dl_warm; cnt0 = p->dl_cnt;
   }
+  for (int j = 0; j < npred; ++j) {
+    RolloutArgs A; memset(&A, 0, sizeof(A));
+    A.qpos0 = p->dl_qpos; A.qvel0 = p->dl_qvel; A.warm0 = p->dl_warm;
+    A.counters_in = p->dl_cnt; A.counters_out = p->dl_cnt;
+    A.nrows = ni; A.H = 1; A.mode = 0; A.rows_per_inst = 1;
+    A.us = (obs ? p->ob.seq : p->dl_pending) + (size_t)j * nu; A.us_row = DIAL_MAXDELAY * nu;
+    if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
+    A.models = p->n_ens > 0 ? p->dl_models : p->models.d;
+    A.iter_lim = obs ? p->ob.len : p->dl_len; A.iter = j;
+    A.qpos_out = p->dl_qpos; A.qvel_out = p->dl_qvel; A.warm_out = p->dl_warm;
+    CUDA_OK(launch_rollout(p, A, 1, st));
+  }
+  if (obs || npred > 0) { qpos0 = p->dl_qpos; qvel0 = p->dl_qvel; warm0 = p->dl_warm; cnt0 = p->dl_cnt; }
   // The info-only bars (qbar, qdbar, xbar; dial_core.py:133-135) are computed for EVERY iteration,
   // like the reference's scan does (the caller sees those of the last one), on a side branch of
   // the graph: the bars of iteration i read trajectory buffer i&1 and weights buffer i&1 while
@@ -1860,6 +2092,7 @@ extern "C" int dial_mpc_step(dial_plan* p, int n_diffuse, int env_step, void* st
   }
   cudaStream_t st = (cudaStream_t)stream;
   p->dl_pred_last = p->delay.d ? p->dl_pred : 0;   // (a change of dl_pred drops the graphs)
+  p->ob_last = p->obs.d != nullptr;                 // (the first observation setting drops them)
   dial_plan::MpcGraph* g = nullptr;
   for (auto& e : p->mpc_graphs) if (e.n_diffuse == n_diffuse && e.env_step == env_step) g = &e;
   if (!g) {

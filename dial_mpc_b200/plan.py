@@ -190,6 +190,39 @@ class Plan:
             cnt = C.c_void_p(counters.data_ptr())
         self._check(self.lib.dial_plan_planning_state(self.handle, _ptr(qpos), _ptr(qvel), _ptr(warm), cnt, _stream()))
 
+    def set_instance_observation(self, b: int, delay: int, qpos_std=None, qvel_std=None, key=None) -> None:
+        """Instance b plans from an observation of its plant from the next ``mpc_step`` on: the record ``delay``
+        (0..16) env steps old, with Gaussian noise of standard deviations ``qpos_std`` [nv] (tangent space) and
+        ``qvel_std`` [nv] (None: zero) drawn from ``key`` (uint32 [2], None: {0, 0}).  Resets b's history; a
+        stream-ordered copy on the current stream (``dial_plan_set_instance_observation``)."""
+        arrs = []
+        for a in (qpos_std, qvel_std):
+            if a is None:
+                arrs.append(None)
+                continue
+            a = np.ascontiguousarray(a, dtype=np.float32)
+            assert a.shape == (self.nv,), f"need {self.nv} standard deviations, got shape {a.shape}"
+            arrs.append(a)
+        ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
+        self._check(self.lib.dial_plan_set_instance_observation(self.handle, int(b), int(delay), ptr[0], ptr[1],
+                                                                _key(key), _stream()))
+
+    def observed_state(self, qpos: Optional[torch.Tensor], qvel: Optional[torch.Tensor] = None,
+                       warm: Optional[torch.Tensor] = None, counters: Optional[torch.Tensor] = None,
+                       age: Optional[torch.Tensor] = None) -> None:
+        """Copy the observation of the last ``mpc_step``, before the prediction (each output may be None;
+        ``counters`` int32 [n_inst * 2], ``age`` int32 [n_inst]) (``dial_plan_observed_state``)."""
+        B = max(self.desc.n_inst, 1)
+        for t, n in ((qpos, B * self.nq), (qvel, B * self.nv), (warm, B * self.nv)):
+            assert t is None or t.numel() == n, f"need {n} elements, got {tuple(t.shape)}"
+        ints = []
+        for t, n in ((counters, 2 * B), (age, B)):
+            if t is not None:
+                assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n
+            ints.append(None if t is None else C.c_void_p(t.data_ptr()))
+        self._check(self.lib.dial_plan_observed_state(self.handle, _ptr(qpos), _ptr(qvel), _ptr(warm), ints[0], ints[1],
+                                                      _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

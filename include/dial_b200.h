@@ -531,6 +531,51 @@ int dial_plan_pending_actions(dial_plan* plan, float* out, void* stream);
  * a predicting instance, the plant state of every other.  Stream-ordered copies on `stream`. */
 int dial_plan_planning_state(dial_plan* plan, float* qpos, float* qvel, float* warm, int32_t* counters, void* stream);
 
+/* Per-instance observation of dial_mpc_step: instance b may plan from a noisy, late estimate of its plant
+ * state instead of the state itself.  Its setting is an observation delay k_b in control steps, noise
+ * standard deviations sigma_q[nv] (on qpos, in tangent space) and sigma_v[nv] (on qvel), and a noise key.
+ * An instance observes while k_b > 0 or some sigma > 0; the plant, ctrl, reward and adaptation's belief
+ * update keep the plant state.
+ * History: each observing instance keeps a ring of plant records (qpos, qvel, qacc_warmstart, counters and
+ * the action the env step applied: the front of its delay queue, else Y[b][0]).  A dial_mpc_step with
+ * env_step == 1 pushes the post-step record.  A setting resets the ring; the next dial_mpc_step then seeds
+ * it from the plant state.  With c_b records since the reset (the seed counted), the observed record is the
+ * one age_b = min(k_b, c_b - 1) pushes back: the first k_b steps observe the oldest record there is.
+ * Noise: each pushed or seeded record draws (key_b, sub) = split(key_b), eps = normal(sub, 2 nv) (JAX's
+ * legacy Threefry sampler), and the observation is the observed record with hinge and slide qpos + sigma_q
+ * eps[:nv], free-joint positions + sigma eps, a free (or ball) joint's quaternion
+ * qnormalize(q * axisangle(w / |w|, |w|)) with w = sigma_rot eps in the body frame (physics_step's
+ * composition), qvel + sigma_v eps[nv:], and the record's qacc_warmstart and counters.  A dof whose sigma
+ * is 0 is copied bit for bit (a quaternion whose three sigma are 0 stays unnormalised); steps without an env
+ * step reuse the last draw.
+ * Planning: the instance's rollouts start from its observation.  One that predicts (its delay setting's
+ * predict = 1) first takes age_b + d_b env steps on its planning model: the age_b actions applied since the
+ * observed record, oldest first, then its d_b queued actions.  Without noise and without an ensemble its
+ * planning state after step t equals the plant state after step t + d_b, bit for bit.
+ * Launches: once some instance was given a setting, one observe launch runs after the env step and the
+ * shift in every dial_mpc_step, in place of the copy of the plant state, followed by max(k_b + d_b) (over the
+ * predicting instances) prediction launches of one row per instance.  A plan on which no observation is
+ * ever set launches what it launched before.  k_b + d_b <= DIAL_MAXDELAY, checked by whichever of the two
+ * setters runs second.  Sharded plans are rejected. */
+
+/* Instance b's observation setting: `delay` (0..DIAL_MAXDELAY), qpos_std and qvel_std [host][nv] (each
+ * nullable: zero), key [host][2] (nullable: {0, 0}).  A delay of 0 with every sigma 0 removes the setting:
+ * the instance plans from its plant state again.  Every call resets b's ring and restarts its noise from
+ * `key`, stream-ordered on `stream` (so the plan must be bound, dial_mpc_bind).  The first call allocates the
+ * rings and drops the captured graphs; a later call that changes the number of prediction launches drops them
+ * too; other calls keep them, and take effect at the next replay.  Fails for b out of range, a delay out of
+ * range or one whose sum with b's action delay exceeds DIAL_MAXDELAY, a negative or non-finite sigma, and
+ * sharded or unbound plans; the error names the bad argument. */
+int dial_plan_set_instance_observation(dial_plan* plan, int b, int delay, const float* qpos_std,
+                                       const float* qvel_std, const uint32_t key[2], void* stream);
+
+/* The observation of the last dial_mpc_step, before the prediction: qpos [dev][n_inst][nq], qvel and warm
+ * [dev][n_inst][nv], counters [dev][n_inst][2], age [dev][n_inst] (int32, the observed record's age), each
+ * nullable; the plant state at age 0 for an instance that does not observe, and for every instance before
+ * the first step after the first setting.  Stream-ordered copies on `stream`. */
+int dial_plan_observed_state(dial_plan* plan, float* qpos, float* qvel, float* warm, int32_t* counters,
+                             int32_t* age, void* stream);
+
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops
  * previously captured graphs. */

@@ -19,8 +19,14 @@ sample by the ``--risk`` measure of its member rewards (mean, worst or cvar:ALPH
 ``--delays FILE.yaml``: a YAML list of one delay spec per instance (``DeviceLoop(..., delay=...)``: an int or
 ``{steps: d, predict: true}``), so that the step also moves the action queues and, for predicting instances,
 runs the prediction launches (use ``--env-step 1`` for the queues to move).
+``--observe SPEC_OR_FILE``: each instance plans from an observation of its plant (``DeviceLoop(..., observe=...)``):
+a YAML flow mapping applied to every instance (``'{delay: 2, qpos: 0.01, qvel: 0.1}'``) or a YAML file holding
+one such mapping or a list of one per instance (null: none), so that the step also runs the observe launch and,
+for instances predicting through ``--delays``, max(k + d) prediction launches (use ``--env-step 1`` for the
+rings to move).
 ``--profile-kernels``: instead of the timing, run the steps without graph capture under torch.profiler and
-print the mean device time per launch of the rollout, update, ensemble reduction and delay queue kernels."""
+print the mean device time per launch of the rollout, update, ensemble reduction, delay queue and observe
+kernels."""
 import argparse
 import copy
 import json
@@ -86,6 +92,9 @@ def main():
     ap.add_argument("--delays", default=None, metavar="FILE.yaml",
                     help="a YAML list of one delay spec per instance (an int or {steps: d, predict: true}; "
                          "DeviceLoop(..., delay=...))")
+    ap.add_argument("--observe", default=None, metavar="SPEC_OR_FILE",
+                    help="an observe spec for every instance (a YAML flow mapping such as '{delay: 2, qpos: 0.01}') or "
+                         "a YAML file with one spec or a list of one per instance (DeviceLoop(..., observe=...))")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
@@ -101,7 +110,7 @@ def main():
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, delay_setting, schedule_setting
+    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, delay_setting, observe_setting, schedule_setting
 
     B, b = args.instances, BASELINE[args.config]
     cfg = dial_config(args.config, world=1)
@@ -149,7 +158,7 @@ def main():
             n_diffuse = [schedule_setting(s or {}, cfg).Ndiffuse for s in schedule]
         except ValueError as e:
             ap.error(f"--schedules {args.schedules}: {e}")
-    delay, n_pred = None, 0
+    delay, n_pred, settings = None, 0, [(0, False)] * B
     if args.delays is not None:
         import yaml
         delay = yaml.safe_load(open(args.delays))
@@ -161,12 +170,25 @@ def main():
             ap.error(f"--delays {args.delays}: {e}")
         delay = [{"steps": d, "predict": p} for d, p in settings]
         n_pred = max([d for d, p in settings if p] or [0])
+    observe = None
+    if args.observe is not None:
+        import yaml
+        try:
+            observe = yaml.safe_load(open(args.observe) if os.path.isfile(args.observe) else args.observe)
+            if isinstance(observe, list) and len(observe) != B:
+                raise ValueError(f"a list of observe specs needs {B} entries (one per instance), got {len(observe)}")
+            specs = observe if isinstance(observe, list) else [observe] * B
+            ks = [0 if o is None else observe_setting(o, env.sys)[0] for o in specs]
+        except (ValueError, yaml.YAMLError) as e:
+            ap.error(f"--observe {args.observe}: {e}")
+        # with the observe launch the prediction also runs through each predicting instance's observation delay
+        n_pred = max([d + k for (d, p), k in zip(settings, ks) if p] or [0])
     if B == 1:
         loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt,
-                          schedule=schedule, delay=delay)
+                          schedule=schedule, delay=delay, observe=observe)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
-                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule, delay=delay)
+                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule, delay=delay, observe=observe)
     es = args.env_step
     # without --schedules every step runs the config's Ndiffuse on every instance, as before
     nd = None if schedule is not None else cfg.Ndiffuse
@@ -187,7 +209,7 @@ def main():
             if "rollout_kernel" in ev.name:
                 rollouts.append((ev.time_range.start, ev.time_range.elapsed_us()))
             for key in ("update_kernel", "ensemble_reduce_kernel", "trajbar", "ens_gather_kernel", "ens_belief_kernel",
-                        "delay_queue_kernel"):
+                        "delay_queue_kernel", "observe_kernel"):
                 if key in ev.name:
                     n, tot = acc.get(key, (0, 0.0))
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
@@ -200,7 +222,7 @@ def main():
             n, tot = acc.get(key, (0, 0.0))
             acc[key] = (n + 1, tot + us)
         print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
-                              risk=args.risk, adapt=args.adapt, delays=args.delays, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              risk=args.risk, adapt=args.adapt, delays=args.delays, observe=args.observe, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
                               launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
         return
     evs = []
@@ -217,7 +239,7 @@ def main():
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
                           distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
-                          schedules=args.schedules, delays=args.delays, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
+                          schedules=args.schedules, delays=args.delays, observe=args.observe, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
                           value=sum(n_diffuse) * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
 
