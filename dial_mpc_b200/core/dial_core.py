@@ -666,8 +666,8 @@ class DeviceLoop:
         """Instance b's control latency from the next ``step`` on (a delay spec, ``delay_setting``).  Refills its
         queue with d copies of its current ``Y[0]``: until then the plant applies the plan it holds.  A
         stream-ordered copy on the current stream.  The first delay of a loop, and a call that changes the
-        largest delay or the largest delay of a predicting instance, make the next steps capture their graphs
-        again; other calls keep them."""
+        number of prediction launches or whether any instance predicts through its delay, change the launch
+        sequence: the next steps capture their graphs again.  Other calls keep them."""
         b = self._instance(b)
         steps, predict = delay_setting(spec)
         self.plan.set_instance_delay(b, steps, predict)
@@ -689,8 +689,8 @@ class DeviceLoop:
         ``observe_setting``), or from its plant state again (None).  Resets its history: the next step seeds it
         from the plant, and its noise restarts from the spec's seed.  A stream-ordered copy on the current
         stream.  The first observation of a loop, and a call that changes the number of prediction launches
-        (max(k + d) over the predicting instances), make the next steps capture their graphs again; other calls
-        keep them."""
+        (max(k + d) over the predicting instances), change the launch sequence: the next steps capture their
+        graphs again.  Other calls keep them."""
         b = self._instance(b)
         if spec is None:
             if self._observe[b] is not None:

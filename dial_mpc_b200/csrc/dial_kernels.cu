@@ -709,7 +709,7 @@ __global__ void observe_reset_kernel(int b, const ObsSetting* __restrict__ set, 
 // ---------------------------------------------------------------------------------
 // A per-instance setting the captured graphs read between replays: the device array of n slots of `width`
 // elements, its pinned host staging and, per slot, the event of the last copy out of the staging slot.
-// `d` stays null until allocate(): the launches tell an unset setting by it.
+// `d` stays null until allocate(): the plan's launch key (launch_key) tells an unset setting by it.
 template <class T> struct Staged {
   T* d = nullptr;
   T* h = nullptr;
@@ -745,6 +745,22 @@ template <class T> struct Staged {
     ev.clear();
     cudaFree(d); cudaFreeHost(h);
     d = nullptr; h = nullptr;
+  }
+};
+
+// The host-side facts mpc_enqueue branches on or bakes into a capture, all derived from the plan's settings
+// (launch_key): which optional buffers are allocated (an allocation lasts as long as the plan), whether some
+// instance predicts through its action delay, and the number of prediction launches.  A captured
+// control-step graph replays what mpc_enqueue enqueues under the key it was captured with.
+struct LaunchKey {
+  bool models = false, members = false, sched = false, lims = false, adapt = false, delay = false, obs = false;
+  bool predicts = false;   // some instance predicts through a delay d_b > 0: the queue launch also runs without an env step
+  int npred = 0;           // prediction launches
+  // the planner's rollouts start from the planning state, not the plant state
+  bool planning() const { return obs || npred > 0; }
+  bool operator!=(const LaunchKey& o) const {
+    return models != o.models || members != o.members || sched != o.sched || lims != o.lims || adapt != o.adapt ||
+           delay != o.delay || obs != o.obs || predicts != o.predicts || npred != o.npred;
   }
 };
 
@@ -785,6 +801,9 @@ struct dial_plan {
   uint32_t* mpc_key = nullptr;  // sampling key of the current reverse_once
   struct MpcGraph { int n_diffuse, env_step, seen; cudaGraphExec_t exec; int64_t launches; };
   std::vector<MpcGraph> mpc_graphs;
+  // the launch key of the current settings, refreshed by every setter that changes one; and that of the last
+  // dial_mpc_step, under which every graph in mpc_graphs was captured
+  LaunchKey key, ran;
   // per-instance models (dial_plan_set_instance_model): [n_inst] slots read by dial_mpc_step, allocated by
   // the first call
   Staged<DevModel> models;
@@ -809,33 +828,43 @@ struct dial_plan {
   // call; the staging `h` mirrors what the device holds
   Staged<InstSchedule> sched;
   Staged<int32_t> lims;
+  // the planning state the planner's rollouts start from once some instance predicts or observes (qpos, qvel,
+  // warm start, counters [n_inst][*]) and, on an ensemble plan, the planning models [n_inst] (a copy of member
+  // (b, 0)); allocated by whichever of dial_plan_set_instance_delay and _observation runs first
+  struct PlanningState {
+    float *qpos = nullptr, *qvel = nullptr, *warm = nullptr;
+    int32_t* cnt = nullptr;
+    DevModel* models = nullptr;
+  } planning;
   // per-instance control latency (dial_plan_set_instance_delay): the settings [n_inst] (the staging mirrors
-  // the device), and, allocated with them, the queues' front slots [n_inst] and rings [n_inst][DIAL_MAXDELAY][nu],
-  // the applied actions [n_inst][nu], the queues in application order [n_inst][DIAL_MAXDELAY][nu], the
-  // prediction lengths [n_inst], and the planning state (qpos, qvel, warm start, counters) and, on an ensemble
-  // plan, the planning models [n_inst] (a copy of member (b, 0)), which dial_plan_set_instance_observation
-  // allocates instead when it runs first.  dl_max / dl_pred: the largest delay, and
-  // that of the predicting instances (the number of prediction launches), as set on the host.
+  // the device), and, allocated with them, the queues
   Staged<DelaySetting> delay;
-  int32_t* dl_head = nullptr;
-  float* dl_ring = nullptr;
-  float* dl_applied = nullptr;
-  float* dl_pending = nullptr;
-  int32_t* dl_len = nullptr;
-  float *dl_qpos = nullptr, *dl_qvel = nullptr, *dl_warm = nullptr;
-  int32_t* dl_cnt = nullptr;
-  DevModel* dl_models = nullptr;
-  int dl_max = 0, dl_pred = 0;
-  int dl_pred_last = 0;   // dl_pred of the last dial_mpc_step (its graph's launch sequence)
+  // the queues: front slots [n_inst] and rings [n_inst][DIAL_MAXDELAY][nu], the applied actions [n_inst][nu],
+  // the queues in application order [n_inst][DIAL_MAXDELAY][nu] and the prediction lengths [n_inst]
+  struct DelayQueue {
+    int32_t* head = nullptr;
+    float *ring = nullptr, *applied = nullptr, *pending = nullptr;
+    int32_t* len = nullptr;
+  } queue;
   // per-instance observation (dial_plan_set_instance_observation): the settings [n_inst] (the staging mirrors
-  // the device) and, allocated with them by the first call, the rings and observations (ObsBuffers; the
-  // planning state above is allocated by whichever of the two setters runs first).  ob_pred: the number of
-  // prediction launches while the observe launch runs, max(k_b + d_b) over the predicting instances, as set
-  // on the host; ob_last: the last dial_mpc_step ran the observe launch.
+  // the device) and, allocated with them by the first call, the rings and observations
   Staged<ObsSetting> obs;
   ObsBuffers ob{};
-  int ob_pred = 0;
-  bool ob_last = false;
+  // the plan's device buffers that cudaMalloc allocated, by the address of the pointer holding each (own)
+  std::vector<void**> owned;
+  // cudaMalloc `bytes` into `ptr`, which the plan owns from then on (free_since, dial_plan_destroy); with
+  // `zero`, also cleared stream-ordered on `st`.  Does nothing once `e` holds an error, so a group of calls
+  // checks it once.
+  template <class T> cudaError_t own(cudaError_t& e, T*& ptr, size_t bytes, bool zero = false, cudaStream_t st = nullptr) {
+    void** slot = reinterpret_cast<void**>(&ptr);
+    if (e == cudaSuccess && (e = cudaMalloc(slot, bytes)) == cudaSuccess) owned.push_back(slot);
+    if (e == cudaSuccess && zero) e = cudaMemsetAsync(ptr, 0, bytes, st);
+    return e;
+  }
+  // frees the buffers owned since owned.size() was `mark`, and nulls their pointers
+  void free_since(size_t mark) {
+    for (; owned.size() > mark; owned.pop_back()) { cudaFree(*owned.back()); *owned.back() = nullptr; }
+  }
   // multi-GPU exchange over NVLink peer memory (dial_exchange_*): one cudaMalloc per rank, mapped
   // into every peer with CUDA IPC.  Word offsets inside the block are the same on every rank.
   struct Exchange {
@@ -859,6 +888,24 @@ struct dial_plan {
 static void drop_graphs(dial_plan* p) {
   for (auto& g : p->mpc_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   p->mpc_graphs.clear();
+}
+
+// The launch key of the plan's current settings (the staging mirrors the device).  The prediction runs
+// max(k_b + d_b) launches over the predicting instances, k_b the observation delay of an observing instance
+// while the observe launch runs, else 0.
+static LaunchKey launch_key(const dial_plan* p) {
+  LaunchKey k;
+  k.models = p->models.d != nullptr; k.members = p->members.d != nullptr;
+  k.sched = p->sched.d != nullptr; k.lims = p->lims.d != nullptr; k.adapt = p->pred_qd != nullptr;
+  k.delay = p->delay.d != nullptr; k.obs = p->obs.d != nullptr;
+  for (int b = 0; k.delay && b < p->n_inst; ++b) {
+    const DelaySetting& s = p->delay.h[b];
+    const int n = s.d + (k.obs && p->obs.h[b].on ? p->obs.h[b].k : 0);
+    if (!s.predict) continue;
+    k.predicts |= s.d > 0;
+    k.npred = n > k.npred ? n : k.npred;
+  }
+  return k;
 }
 
 static void fill_xch(const dial_plan* p, RolloutArgs& A) {
@@ -1038,21 +1085,21 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     dial_plan_destroy(p);
     return (dial_plan*)nullptr;
   };
-  cudaError_t e;
-  if ((e = cudaMalloc(&p->dM, sizeof(DevModel))) != cudaSuccess) return bad(e, "cudaMalloc(model)");
-  if ((e = cudaMalloc(&p->dP, sizeof(DevPlan))) != cudaSuccess) return bad(e, "cudaMalloc(plan)");
+  cudaError_t e = cudaSuccess;
+  if (p->own(e, p->dM, sizeof(DevModel)) != cudaSuccess) return bad(e, "cudaMalloc(model)");
+  if (p->own(e, p->dP, sizeof(DevPlan)) != cudaSuccess) return bad(e, "cudaMalloc(plan)");
   if ((e = cudaMemcpy(p->dM, &p->hM, sizeof(DevModel), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(model)");
   if ((e = cudaMemcpy(p->dP, &p->hP, sizeof(DevPlan), cudaMemcpyHostToDevice)) != cudaSuccess) return bad(e, "cudaMemcpy(plan)");
   const size_t B = (size_t)p->n_inst, H = (size_t)c.Hsample + 1;
   const size_t rows = B * (p->n_ens > 1 ? (size_t)p->n_ens : 1) * ((size_t)c.Nsample + 1);   // every member's trajectories
   const dial_model_desc& m = *model;
   for (int b = 0; b < 2; ++b) {
-    if ((e = cudaMalloc(&p->traj_q[b], rows * H * m.nq * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_q)");
-    if ((e = cudaMalloc(&p->traj_qd[b], rows * H * m.nv * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_qd)");
-    if ((e = cudaMalloc(&p->traj_x[b], rows * H * 3 * (m.nbody - 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(traj_x)");
+    if (p->own(e, p->traj_q[b], rows * H * m.nq * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(traj_q)");
+    if (p->own(e, p->traj_qd[b], rows * H * m.nv * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(traj_qd)");
+    if (p->own(e, p->traj_x[b], rows * H * 3 * (m.nbody - 1) * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(traj_x)");
   }
   if (p->n_ens > 1) {
-    if ((e = cudaMalloc(&p->ens_rews, rows * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(ens_rews)");
+    if (p->own(e, p->ens_rews, rows * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(ens_rews)");
     // every instance starts at the mean, no instance adapts, every belief starts uniform
     const size_t K = p->n_ens;
     const double L0 = log(1.0 / p->n_ens);
@@ -1060,11 +1107,11 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     if ((e = p->adapt.allocate(B, 1, EnsAdapt{})) != cudaSuccess) return bad(e, "allocate(adapt)");
     if ((e = p->belief_L.allocate(B, K, L0)) != cudaSuccess) return bad(e, "allocate(belief)");
     if ((e = p->belief_w.allocate(B, K, (float)exp(L0))) != cudaSuccess) return bad(e, "allocate(belief)");
-    if ((e = cudaMalloc(&p->dEll, B * K * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
+    if (p->own(e, p->dEll, B * K * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(belief)");
     if ((e = cudaMemset(p->dEll, 0, B * K * sizeof(float))) != cudaSuccess) return bad(e, "cudaMemset(belief)");
   }
-  if ((e = cudaMalloc(&p->weights, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
-  if ((e = cudaMalloc(&p->weights2, B * ((size_t)c.Ntotal + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
+  if (p->own(e, p->weights, B * ((size_t)c.Ntotal + 1) * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(weights)");
+  if (p->own(e, p->weights2, B * ((size_t)c.Ntotal + 1) * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(weights2)");
   if ((e = cudaStreamCreateWithFlags(&p->side, cudaStreamNonBlocking)) != cudaSuccess) return bad(e, "cudaStreamCreate(side)");
   for (int i = 0; i < 2; ++i) {
     if ((e = cudaEventCreateWithFlags(&p->ev_main[i], cudaEventDisableTiming)) != cudaSuccess) return bad(e, "cudaEventCreate");
@@ -1077,46 +1124,34 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     int gu = (c.Ntotal + 1 + slots * 8 - 1) / (slots * 8);
     p->upd_grid = gu < 1 ? 1 : (gu > p->ybar_grid ? p->ybar_grid : gu);
   }
-  if ((e = cudaMalloc(&p->partial, B * p->ybar_grid * (ne + 1) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(partial)");
-  if ((e = cudaMalloc(&p->tb_partial, B * TB_CHUNKS * H * (m.nq + m.nv + 3 * (m.nbody - 1)) * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(tb_partial)");
-  if ((e = cudaMalloc(&p->counter, B * sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMalloc(counter)");
+  if (p->own(e, p->partial, B * p->ybar_grid * (ne + 1) * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(partial)");
+  if (p->own(e, p->tb_partial, B * TB_CHUNKS * H * (m.nq + m.nv + 3 * (m.nbody - 1)) * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(tb_partial)");
+  if (p->own(e, p->counter, B * sizeof(unsigned int)) != cudaSuccess) return bad(e, "cudaMalloc(counter)");
   if ((e = cudaMemset(p->counter, 0, B * sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMemset(counter)");
-  if ((e = cudaMalloc(&p->row_counter, sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMalloc(row_counter)");
+  if (p->own(e, p->row_counter, sizeof(unsigned int)) != cudaSuccess) return bad(e, "cudaMalloc(row_counter)");
   if (getenv("DIAL_DEBUG_COUNTERS")) {
-    if ((e = cudaMalloc(&p->dbg, 8 * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(dbg)");
+    if (p->own(e, p->dbg, 8 * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(dbg)");
     cudaMemset(p->dbg, 0, 8 * sizeof(float));
   }
-  if ((e = cudaMalloc(&p->zeros, DIAL_MAXV * sizeof(float))) != cudaSuccess) return bad(e, "cudaMalloc(zeros)");
+  if (p->own(e, p->zeros, DIAL_MAXV * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(zeros)");
   if ((e = cudaMemset(p->zeros, 0, DIAL_MAXV * sizeof(float))) != cudaSuccess) return bad(e, "cudaMemset(zeros)");
   return p;
 }
 
 extern "C" void dial_plan_destroy(dial_plan* p) {
   if (!p) return;
-  cudaFree(p->dM); cudaFree(p->dP);
-  for (int b = 0; b < 2; ++b) { cudaFree(p->traj_q[b]); cudaFree(p->traj_qd[b]); cudaFree(p->traj_x[b]); }
   drop_graphs(p);
   for (int r = 0; r < DIAL_MAXRANK; ++r) {
     if (!p->xch.base[r]) continue;
     if (r == p->xch.rank) cudaFree(p->xch.base[r]); else cudaIpcCloseMemHandle(p->xch.base[r]);
   }
   cudaFree(p->xch.bars_partial);
-  cudaFree(p->mpc_Msh); cudaFree(p->mpc_Y1); cudaFree(p->mpc_key);
   p->models.release(); p->members.release(); p->risk.release();
   p->adapt.release(); p->belief_L.release(); p->belief_w.release(); p->sched.release(); p->lims.release();
-  cudaFree(p->ens_rews); cudaFree(p->dEll); cudaFree(p->pred_us); cudaFree(p->pred_qd);
-  p->delay.release();
-  cudaFree(p->dl_head); cudaFree(p->dl_ring); cudaFree(p->dl_applied); cudaFree(p->dl_pending); cudaFree(p->dl_len);
-  cudaFree(p->dl_qpos); cudaFree(p->dl_qvel); cudaFree(p->dl_warm); cudaFree(p->dl_cnt); cudaFree(p->dl_models);
-  p->obs.release();
-  for (void* d : {(void*)p->ob.ring, (void*)p->ob.rq, (void*)p->ob.rv, (void*)p->ob.rw, (void*)p->ob.ra, (void*)p->ob.rc,
-                  (void*)p->ob.oq, (void*)p->ob.ov, (void*)p->ob.ow, (void*)p->ob.oc, (void*)p->ob.age, (void*)p->ob.seq,
-                  (void*)p->ob.len})
-    cudaFree(d);
+  p->delay.release(); p->obs.release();
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
-  cudaFree(p->weights2);
-  cudaFree(p->weights); cudaFree(p->partial); cudaFree(p->tb_partial); cudaFree(p->counter); cudaFree(p->row_counter); cudaFree(p->zeros); cudaFree(p->dbg);
+  p->free_since(0);
   delete p;
 }
 
@@ -1190,8 +1225,8 @@ static int need_instance(const dial_plan* p, const char* fn, int b) {
 }
 
 // Derive `m`, check it against the plan's model and copy it into slot `slot` of the model slots `a` [n],
-// allocating them on first use with every slot holding the plan's own model and dropping the captured
-// graphs then.  `fn` names the public call in errors.
+// allocating them on first use with every slot holding the plan's own model.  `fn` names the public call
+// in errors.
 static int set_model_slot(dial_plan* p, const char* fn, Staged<DevModel>& a, size_t n, size_t slot,
                           const dial_model_desc* m, cudaStream_t st) {
   std::unique_ptr<DevModel> D(new (std::nothrow) DevModel());
@@ -1202,12 +1237,9 @@ static int set_model_slot(dial_plan* p, const char* fn, Staged<DevModel>& a, siz
     return fail(std::string(fn) + ": field '" + diff + "' differs from the plan's model "
                 "(an instance's model may differ in floats other than timestep, jnt_range and actuator_ctrlrange only)");
   cudaError_t e = cudaSuccess;
-  if (!a.d) {
-    // first call: the graphs captured so far launch without these slots
-    if ((e = a.allocate(n, 1, p->hM)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
-    drop_graphs(p);
-  }
+  if (!a.d && (e = a.allocate(n, 1, p->hM)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   e = a.put(slot, [&](DevModel* h) { *h = *D; }, st);
+  p->key = launch_key(p);
   CUDA_OK(e);
   return 0;
 }
@@ -1229,8 +1261,8 @@ extern "C" int dial_plan_set_ensemble_model(dial_plan* p, int b, int k, const di
   const size_t slot = (size_t)b * p->n_ens + k;
   if (int rc = set_model_slot(p, fn, p->members, (size_t)p->n_inst * p->n_ens, slot, m, (cudaStream_t)stream)) return rc;
   // member (b, 0) is instance b's planning model for its prediction through a delay
-  if (k == 0 && p->dl_models)
-    CUDA_OK(cudaMemcpyAsync(p->dl_models + b, p->members.d + slot, sizeof(DevModel), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  if (k == 0 && p->planning.models)
+    CUDA_OK(cudaMemcpyAsync(p->planning.models + b, p->members.d + slot, sizeof(DevModel), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return 0;
 }
 
@@ -1276,17 +1308,13 @@ extern "C" int dial_plan_set_ensemble_adapt(dial_plan* p, int b, int on, float f
   }
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaSuccess;
-  if (on && !p->pred_qd) {
-    // first instance to adapt: the prediction workspaces; the graphs captured so far hold no adaptation
-    // launches and are recaptured on their next use
-    const size_t rows = (size_t)p->n_inst * K;
-    if ((e = cudaMalloc(&p->pred_us, rows * p->hM.m.nu * sizeof(float))) == cudaSuccess)
-      e = cudaMalloc(&p->pred_qd, rows * nv * sizeof(float));
-    if (e != cudaSuccess) {
-      cudaFree(p->pred_us); cudaFree(p->pred_qd); p->pred_us = p->pred_qd = nullptr;
+  if (on && !p->pred_qd) {   // first instance to adapt: the prediction workspaces
+    const size_t rows = (size_t)p->n_inst * K, mark = p->owned.size();
+    p->own(e, p->pred_us, rows * p->hM.m.nu * sizeof(float));
+    if (p->own(e, p->pred_qd, rows * nv * sizeof(float)) != cudaSuccess) {
+      p->free_since(mark);
       return fail(std::string(fn) + ": " + cudaGetErrorString(e));
     }
-    drop_graphs(p);
   }
   e = p->adapt.put(b, [&](EnsAdapt* a) {   // off: the staged forget, prune and sigma are kept
     a->on = on;
@@ -1295,6 +1323,7 @@ extern "C" int dial_plan_set_ensemble_adapt(dial_plan* p, int b, int on, float f
       for (int j = 0; j < DIAL_MAXV; ++j) a->sigma[j] = j < nv ? sigma[j] : 1.f;
     }
   }, st);
+  p->key = launch_key(p);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   return 0;
 }
@@ -1358,11 +1387,8 @@ extern "C" int dial_plan_set_instance_schedule(dial_plan* p, int b, float temp, 
   }
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaSuccess;
-  if (!p->sched.d) {
-    // first call: the graphs captured so far launch without the schedules
-    if ((e = p->sched.allocate(p->n_inst, 1, InstSchedule{})) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
-    drop_graphs(p);
-  }
+  if (!p->sched.d && (e = p->sched.allocate(p->n_inst, 1, InstSchedule{})) != cudaSuccess)
+    return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   e = p->sched.put(b, [&](InstSchedule* S) {
     memset(S, 0, sizeof(*S));
     if (!noise) return;
@@ -1370,6 +1396,7 @@ extern "C" int dial_plan_set_instance_schedule(dial_plan* p, int b, float temp, 
     for (int r = 0; r < n_rows; ++r)
       for (int k = 0; k < n1; ++k) S->noise[r][k] = noise[r * n1 + k];
   }, st);
+  p->key = launch_key(p);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   return 0;
 }
@@ -1390,64 +1417,44 @@ extern "C" int dial_plan_set_instance_iterations(dial_plan* p, const int32_t* n_
     if (!M.d) e = M.allocate((size_t)p->n_inst * (p->n_ens > 0 ? p->n_ens : 1), 1, p->hM);
     if (e == cudaSuccess) e = p->lims.allocate(1, p->n_inst, DIAL_MAXDIFFUSE);
     if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
-    drop_graphs(p);
   }
   e = p->lims.put(0, [&](int32_t* L) { memcpy(L, n_iter, sizeof(int32_t) * p->n_inst); }, st);
+  p->key = launch_key(p);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   return 0;
 }
 
 // The planning state (qpos, qvel, warm start, counters) and, on an ensemble plan, the planning models (member
 // (b, 0) of each instance as the member slots hold it, else the plan's model), allocated by the first
-// dial_plan_set_instance_delay or dial_plan_set_instance_observation.
+// dial_plan_set_instance_delay or dial_plan_set_instance_observation; on failure the caller frees what it owns.
 static cudaError_t allocate_planning(dial_plan* p, cudaStream_t st) {
-  if (p->dl_qpos) return cudaSuccess;
+  dial_plan::PlanningState& P = p->planning;
+  if (P.qpos) return cudaSuccess;
   const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv;
   cudaError_t e = cudaSuccess;
-  auto dev = [&](auto*& ptr, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ptr, 0, bytes, st);
-  };
-  dev(p->dl_qpos, B * nq * sizeof(float));
-  dev(p->dl_qvel, B * nv * sizeof(float));
-  dev(p->dl_warm, B * nv * sizeof(float));
-  dev(p->dl_cnt, B * 2 * sizeof(int32_t));
-  if (p->n_ens > 0 && e == cudaSuccess) {
-    e = cudaMalloc(&p->dl_models, B * sizeof(DevModel));
-    for (size_t b = 0; b < B && e == cudaSuccess; ++b)
-      e = p->members.d ? cudaMemcpyAsync(p->dl_models + b, p->members.d + b * p->n_ens, sizeof(DevModel), cudaMemcpyDeviceToDevice, st)
-                       : cudaMemcpy(p->dl_models + b, &p->hM, sizeof(DevModel), cudaMemcpyHostToDevice);
-  }
-  if (e != cudaSuccess) {
-    for (void* d : {(void*)p->dl_qpos, (void*)p->dl_qvel, (void*)p->dl_warm, (void*)p->dl_cnt, (void*)p->dl_models}) cudaFree(d);
-    p->dl_qpos = p->dl_qvel = p->dl_warm = nullptr;
-    p->dl_cnt = nullptr;
-    p->dl_models = nullptr;
-  }
+  p->own(e, P.qpos, B * nq * sizeof(float), true, st);
+  p->own(e, P.qvel, B * nv * sizeof(float), true, st);
+  p->own(e, P.warm, B * nv * sizeof(float), true, st);
+  p->own(e, P.cnt, B * 2 * sizeof(int32_t), true, st);
+  if (p->n_ens > 0) p->own(e, P.models, B * sizeof(DevModel));
+  for (size_t b = 0; P.models && b < B && e == cudaSuccess; ++b)
+    e = p->members.d ? cudaMemcpyAsync(P.models + b, p->members.d + b * p->n_ens, sizeof(DevModel), cudaMemcpyDeviceToDevice, st)
+                     : cudaMemcpy(P.models + b, &p->hM, sizeof(DevModel), cudaMemcpyHostToDevice);
   return e;
 }
 
-// First dial_plan_set_instance_delay: the queues (and the planning state, if not yet allocated).
+// First dial_plan_set_instance_delay: the settings and queues (and the planning state, if not yet allocated).
 static cudaError_t allocate_delay(dial_plan* p, cudaStream_t st) {
-  const size_t B = (size_t)p->n_inst, nu = p->hM.m.nu;
+  const size_t B = (size_t)p->n_inst, nu = p->hM.m.nu, mark = p->owned.size();
+  dial_plan::DelayQueue& Q = p->queue;
   cudaError_t e = allocate_planning(p, st);
   if (e == cudaSuccess) e = p->delay.allocate(B, 1, DelaySetting{0, 0});
-  auto dev = [&](auto*& ptr, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ptr, 0, bytes, st);
-  };
-  dev(p->dl_head, B * sizeof(int32_t));
-  dev(p->dl_ring, B * DIAL_MAXDELAY * nu * sizeof(float));
-  dev(p->dl_applied, B * nu * sizeof(float));
-  dev(p->dl_pending, B * DIAL_MAXDELAY * nu * sizeof(float));
-  dev(p->dl_len, B * sizeof(int32_t));
-  if (e != cudaSuccess) {
-    p->delay.release();
-    for (void* d : {(void*)p->dl_head, (void*)p->dl_ring, (void*)p->dl_applied, (void*)p->dl_pending, (void*)p->dl_len})
-      cudaFree(d);
-    p->dl_head = p->dl_len = nullptr;
-    p->dl_ring = p->dl_applied = p->dl_pending = nullptr;
-  }
+  p->own(e, Q.head, B * sizeof(int32_t), true, st);
+  p->own(e, Q.ring, B * DIAL_MAXDELAY * nu * sizeof(float), true, st);
+  p->own(e, Q.applied, B * nu * sizeof(float), true, st);
+  p->own(e, Q.pending, B * DIAL_MAXDELAY * nu * sizeof(float), true, st);
+  p->own(e, Q.len, B * sizeof(int32_t), true, st);
+  if (e != cudaSuccess) { p->delay.release(); p->free_since(mark); }
   return e;
 }
 
@@ -1455,49 +1462,27 @@ static cudaError_t allocate_delay(dial_plan* p, cudaStream_t st) {
 // not yet allocated).  Every ring starts empty.
 static cudaError_t allocate_observation(dial_plan* p, cudaStream_t st) {
   const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv, nu = p->hM.m.nu, R = DIAL_OBSRING;
+  const size_t mark = p->owned.size();
   cudaError_t e = allocate_planning(p, st);
   ObsSetting off;
   memset(&off, 0, sizeof(off));
   if (e == cudaSuccess) e = p->obs.allocate(B, 1, off);
   ObsBuffers& O = p->ob;
-  auto dev = [&](auto*& ptr, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ptr, 0, bytes, st);
-  };
-  dev(O.ring, B * sizeof(ObsRing));
-  dev(O.rq, B * R * nq * sizeof(float));
-  dev(O.rv, B * R * nv * sizeof(float));
-  dev(O.rw, B * R * nv * sizeof(float));
-  dev(O.ra, B * R * nu * sizeof(float));
-  dev(O.rc, B * R * 2 * sizeof(int32_t));
-  dev(O.oq, B * nq * sizeof(float));
-  dev(O.ov, B * nv * sizeof(float));
-  dev(O.ow, B * nv * sizeof(float));
-  dev(O.oc, B * 2 * sizeof(int32_t));
-  dev(O.age, B * sizeof(int32_t));
-  dev(O.seq, B * DIAL_MAXDELAY * nu * sizeof(float));
-  dev(O.len, B * sizeof(int32_t));
-  if (e != cudaSuccess) {
-    p->obs.release();
-    for (void* d : {(void*)O.ring, (void*)O.rq, (void*)O.rv, (void*)O.rw, (void*)O.ra, (void*)O.rc, (void*)O.oq,
-                    (void*)O.ov, (void*)O.ow, (void*)O.oc, (void*)O.age, (void*)O.seq, (void*)O.len})
-      cudaFree(d);
-    O = ObsBuffers{};
-  }
+  p->own(e, O.ring, B * sizeof(ObsRing), true, st);
+  p->own(e, O.rq, B * R * nq * sizeof(float), true, st);
+  p->own(e, O.rv, B * R * nv * sizeof(float), true, st);
+  p->own(e, O.rw, B * R * nv * sizeof(float), true, st);
+  p->own(e, O.ra, B * R * nu * sizeof(float), true, st);
+  p->own(e, O.rc, B * R * 2 * sizeof(int32_t), true, st);
+  p->own(e, O.oq, B * nq * sizeof(float), true, st);
+  p->own(e, O.ov, B * nv * sizeof(float), true, st);
+  p->own(e, O.ow, B * nv * sizeof(float), true, st);
+  p->own(e, O.oc, B * 2 * sizeof(int32_t), true, st);
+  p->own(e, O.age, B * sizeof(int32_t), true, st);
+  p->own(e, O.seq, B * DIAL_MAXDELAY * nu * sizeof(float), true, st);
+  p->own(e, O.len, B * sizeof(int32_t), true, st);
+  if (e != cudaSuccess) { p->obs.release(); p->free_since(mark); }
   return e;
-}
-
-// The number of prediction launches of the current settings: max(k_b + d_b) over the predicting instances
-// while the observe launch runs (k_b of an observing instance, else 0), max(d_b) over them without it
-// (staging = device).
-static int prediction_launches(const dial_plan* p) {
-  int n = 0;
-  for (int b = 0; p->delay.d && b < p->n_inst; ++b) {
-    const DelaySetting& s = p->delay.h[b];
-    const int k = p->obs.d && p->obs.h[b].on ? p->obs.h[b].k : 0;
-    if (s.predict && s.d + k > n) n = s.d + k;
-  }
-  return n;
 }
 
 extern "C" int dial_plan_set_instance_delay(dial_plan* p, int b, int steps, int predict, void* stream) {
@@ -1515,30 +1500,13 @@ extern "C" int dial_plan_set_instance_delay(dial_plan* p, int b, int steps, int 
   if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first (the queue is filled from the bound Y)");
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaSuccess;
-  if (!p->delay.d) {
-    // first call: the graphs captured so far apply Y[b][0] at once
-    if ((e = allocate_delay(p, st)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
-    drop_graphs(p);
-  }
+  if (!p->delay.d && (e = allocate_delay(p, st)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   e = p->delay.put(b, [&](DelaySetting* s) { s->d = steps; s->predict = predict; }, st);
+  p->key = launch_key(p);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   const int n1 = c.Hnode + 1, nu = p->hM.m.nu;
-  delay_refill_kernel<<<1, 128, 0, st>>>(b, steps, p->dl_head, p->dl_ring, p->mpc.Y, n1, nu, p->dl_pending);
+  delay_refill_kernel<<<1, 128, 0, st>>>(b, steps, p->queue.head, p->queue.ring, p->mpc.Y, n1, nu, p->queue.pending);
   CUDA_OK(cudaGetLastError());
-  // the launch sequence depends on the largest delay and on the prediction length (staging = device)
-  int dmax = 0, dpred = 0;
-  for (int i = 0; i < p->n_inst; ++i) {
-    const DelaySetting& s = p->delay.h[i];
-    dmax = s.d > dmax ? s.d : dmax;
-    if (s.predict && s.d > dpred) dpred = s.d;
-  }
-  if (dmax != p->dl_max || dpred != p->dl_pred) drop_graphs(p);
-  p->dl_max = dmax; p->dl_pred = dpred;
-  if (p->obs.d) {   // with the observe launch, the prediction's length also counts the observation delays
-    const int n = prediction_launches(p);
-    if (n != p->ob_pred) drop_graphs(p);
-    p->ob_pred = n;
-  }
   return 0;
 }
 
@@ -1569,23 +1537,17 @@ extern "C" int dial_plan_set_instance_observation(dial_plan* p, int b, int delay
   if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaSuccess;
-  if (!p->obs.d) {
-    // first call: the graphs captured so far plan from the plant state
-    if ((e = allocate_observation(p, st)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
-    drop_graphs(p);
-  }
+  if (!p->obs.d && (e = allocate_observation(p, st)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   e = p->obs.put(b, [&](ObsSetting* s) {
     s->k = delay; s->on = delay > 0 || noisy;
     s->key[0] = key ? key[0] : 0u; s->key[1] = key ? key[1] : 0u;
     for (int i = 0; i < 2 * DIAL_MAXV; ++i) s->sigma[i] = 0.f;
     for (int i = 0; i < nv; ++i) { s->sigma[i] = qpos_std ? qpos_std[i] : 0.f; s->sigma[nv + i] = qvel_std ? qvel_std[i] : 0.f; }
   }, st);
+  p->key = launch_key(p);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   observe_reset_kernel<<<1, 1, 0, st>>>(b, p->obs.d, p->ob.ring);
   CUDA_OK(cudaGetLastError());
-  const int n = prediction_launches(p);
-  if (n != p->ob_pred) drop_graphs(p);
-  p->ob_pred = n;
   return 0;
 }
 
@@ -1596,7 +1558,7 @@ extern "C" int dial_plan_observed_state(dial_plan* p, float* qpos, float* qvel, 
   if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
   const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv;
   // the observation of the last step when it ran the observe launch, else the plant state at age 0
-  const bool ob = p->ob_last;
+  const bool ob = p->ran.obs;
   cudaStream_t st = (cudaStream_t)stream;
   const auto cp = [&](void* dst, const void* src, size_t bytes) {
     return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
@@ -1617,7 +1579,7 @@ extern "C" int dial_plan_pending_actions(dial_plan* p, float* out, void* stream)
   if (!p || !out) return fail(std::string(fn) + ": null argument");
   const size_t n = (size_t)p->n_inst * DIAL_MAXDELAY * p->hM.m.nu * sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
-  if (p->dl_pending) CUDA_OK(cudaMemcpyAsync(out, p->dl_pending, n, cudaMemcpyDeviceToDevice, st));
+  if (p->queue.pending) CUDA_OK(cudaMemcpyAsync(out, p->queue.pending, n, cudaMemcpyDeviceToDevice, st));
   else CUDA_OK(cudaMemsetAsync(out, 0, n, st));
   return 0;
 }
@@ -1627,17 +1589,18 @@ extern "C" int dial_plan_planning_state(dial_plan* p, float* qpos, float* qvel, 
   if (!p) return fail(std::string(fn) + ": null plan");
   if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
   const size_t B = (size_t)p->n_inst, nq = p->hM.m.nq, nv = p->hM.m.nv;
-  // the last step planned from the predicted state when it predicted (then the other instances' rows hold
-  // their plant state, copied in that step)
-  const bool pred = p->dl_pred_last > 0 || p->ob_last;
+  // the last step planned from the planning state when it predicted or observed (then the other instances'
+  // rows hold their plant state, copied in that step)
+  const bool pred = p->ran.planning();
   cudaStream_t st = (cudaStream_t)stream;
   const auto cp = [&](void* dst, const void* src, size_t bytes) {
     return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
   };
-  CUDA_OK(cp(qpos, pred ? p->dl_qpos : p->mpc.qpos, B * nq * sizeof(float)));
-  CUDA_OK(cp(qvel, pred ? p->dl_qvel : p->mpc.qvel, B * nv * sizeof(float)));
-  CUDA_OK(cp(warm, pred ? p->dl_warm : p->mpc.qacc_warmstart, B * nv * sizeof(float)));
-  CUDA_OK(cp(counters, pred ? p->dl_cnt : p->mpc.counters, B * 2 * sizeof(int32_t)));
+  const dial_plan::PlanningState& P = p->planning;
+  CUDA_OK(cp(qpos, pred ? P.qpos : p->mpc.qpos, B * nq * sizeof(float)));
+  CUDA_OK(cp(qvel, pred ? P.qvel : p->mpc.qvel, B * nv * sizeof(float)));
+  CUDA_OK(cp(warm, pred ? P.warm : p->mpc.qacc_warmstart, B * nv * sizeof(float)));
+  CUDA_OK(cp(counters, pred ? P.cnt : p->mpc.counters, B * 2 * sizeof(int32_t)));
   return 0;
 }
 
@@ -1888,9 +1851,10 @@ extern "C" int dial_mpc_bind(dial_plan* p, const dial_mpc_buffers* b, const floa
   if (p->n_inst > 1 && b->rews_all) return fail("dial_mpc_bind: rews_all must be NULL on a batched plan");
   const int n1 = c.Hnode + 1, nu = p->hM.m.nu;
   drop_graphs(p);
-  if (!p->mpc_Msh) CUDA_OK(cudaMalloc(&p->mpc_Msh, DIAL_MAXNODE * DIAL_MAXNODE * sizeof(float)));
-  if (!p->mpc_Y1) CUDA_OK(cudaMalloc(&p->mpc_Y1, (size_t)p->n_inst * DIAL_MAXNODE * DIAL_MAXU * sizeof(float)));
-  if (!p->mpc_key) CUDA_OK(cudaMalloc(&p->mpc_key, 2 * sizeof(uint32_t)));
+  cudaError_t e = cudaSuccess;
+  if (!p->mpc_Msh) CUDA_OK(p->own(e, p->mpc_Msh, DIAL_MAXNODE * DIAL_MAXNODE * sizeof(float)));
+  if (!p->mpc_Y1) CUDA_OK(p->own(e, p->mpc_Y1, (size_t)p->n_inst * DIAL_MAXNODE * DIAL_MAXU * sizeof(float)));
+  if (!p->mpc_key) CUDA_OK(p->own(e, p->mpc_key, 2 * sizeof(uint32_t)));
   CUDA_OK(cudaMemcpy(p->mpc_Msh, M_shift, (size_t)n1 * n1 * sizeof(float), cudaMemcpyHostToDevice));
   (void)nu;
   p->mpc = *b;
@@ -1898,35 +1862,32 @@ extern "C" int dial_mpc_bind(dial_plan* p, const dial_mpc_buffers* b, const floa
   return 0;
 }
 
-// enqueue one MPC step on `st` (eagerly or into a capture)
-static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t st) {
+// enqueue one MPC step on `st` (eagerly or into a capture), the launch sequence of the plan's key `k`
+static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_step, cudaStream_t st) {
   const dial_plan_desc& c = p->hP.c;
   const dial_mpc_buffers& B = p->mpc;
   const int n1 = c.Hnode + 1, nu = p->hM.m.nu, ni = p->n_inst;
   const int K = p->n_ens > 1 ? p->n_ens : 1;   // rollout rows per sample
   const bool batched = ni > 1;
+  const dial_plan::DelayQueue& Q = p->queue;
+  const dial_plan::PlanningState& P = p->planning;
   float* Y[2] = {B.Y, p->mpc_Y1};
   int cur = 0;
   // control latency, once some instance was given a delay: the queues move in a step with an env step, which
-  // then applies the action each queue pops (dl_applied, one row of nu per instance) instead of Y[b][0]; while
+  // then applies the action each queue pops (Q.applied, one row of nu per instance) instead of Y[b][0]; while
   // some instance predicts, the queue launch also lays out the pending actions in the other steps
-  const bool delay = p->delay.d != nullptr;
-  // observation, once some instance was given a setting: the observe launch after the env step and the shift
-  // writes every instance's planning state, and the prediction runs max(k_b + d_b) launches
-  const bool obs = p->obs.d != nullptr;
-  const int npred = obs ? p->ob_pred : delay ? p->dl_pred : 0;
-  if (delay && (env_step == 1 || p->dl_pred > 0)) {
-    delay_queue_kernel<<<ni, 128, 0, st>>>(p->delay.d, p->dl_head, p->dl_ring, Y[cur], n1, nu, env_step == 1,
-                                           p->dl_applied, p->dl_pending, p->dl_len);
+  if (k.delay && (env_step == 1 || k.predicts)) {
+    delay_queue_kernel<<<ni, 128, 0, st>>>(p->delay.d, Q.head, Q.ring, Y[cur], n1, nu, env_step == 1,
+                                           Q.applied, Q.pending, Q.len);
     p->launches++;
     CUDA_OK(cudaGetLastError());
   }
-  const float* act = delay ? p->dl_applied : Y[cur];
-  const int act_n1 = delay ? 1 : n1;   // rows of nu floats between two instances' actions
+  const float* act = k.delay ? Q.applied : Y[cur];
+  const int act_n1 = k.delay ? 1 : n1;   // rows of nu floats between two instances' actions
   // ensemble adaptation, once some instance has turned it on: before the plant's env step, member (b, k)
   // makes the same env step on its own model, from instance b's state, counters and task with the action
   // the plant applies (row b K + k, its CTA staging member slot b K + k); only the post-step qvel is kept
-  const bool adapt = env_step == 1 && p->pred_qd;
+  const bool adapt = env_step == 1 && k.adapt;
   if (adapt) {
     ens_gather_kernel<<<ni, 128, 0, st>>>(act, K, act_n1, nu, p->pred_us);
     p->launches++;
@@ -1967,37 +1928,37 @@ static int mpc_enqueue(dial_plan* p, int n_diffuse, int env_step, cudaStream_t s
   // The planning state: the plant state, or once some instance predicts, a copy of it in which each predicting
   // instance b takes d_b env steps with its queued actions on its planning model (launch j: one row per
   // instance, action pending[b][j], in place; an instance with pred_len[b] <= j exits at entry)
-  // With the observe launch, the copy is its observation instead (the plant state of an instance that does not
-  // observe), and a predicting instance b takes age_b + d_b env steps: the actions applied since the observed
-  // record, then its queue (launch j: action seq[b][j]; pred_len[b] = age_b + d_b).
+  // With the observe launch (once some instance was given an observation setting), the copy is its observation
+  // instead (the plant state of an instance that does not observe), and a predicting instance b takes
+  // age_b + d_b env steps: the actions applied since the observed record, then its queue (launch j: action
+  // seq[b][j]; pred_len[b] = age_b + d_b).
   const float *qpos0 = B.qpos, *qvel0 = B.qvel, *warm0 = B.qacc_warmstart;
   const int32_t* cnt0 = B.counters;
-  if (obs) {
-    observe_kernel<<<ni, 128, 0, st>>>(p->dM, p->obs.d, p->ob, delay ? p->delay.d : nullptr, delay ? p->dl_pending : nullptr,
-                                       env_step == 1, B.qpos, B.qvel, B.qacc_warmstart, B.counters, act, act_n1 * nu,
-                                       p->dl_qpos, p->dl_qvel, p->dl_warm, p->dl_cnt);
+  if (k.obs) {
+    observe_kernel<<<ni, 128, 0, st>>>(p->dM, p->obs.d, p->ob, p->delay.d, Q.pending, env_step == 1, B.qpos, B.qvel,
+                                       B.qacc_warmstart, B.counters, act, act_n1 * nu, P.qpos, P.qvel, P.warm, P.cnt);
     p->launches++;
     CUDA_OK(cudaGetLastError());
-  } else if (npred > 0) {
+  } else if (k.npred > 0) {
     const size_t nq = p->hM.m.nq, nv = p->hM.m.nv;
-    CUDA_OK(cudaMemcpyAsync(p->dl_qpos, B.qpos, ni * nq * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(p->dl_qvel, B.qvel, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(p->dl_warm, B.qacc_warmstart, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(p->dl_cnt, B.counters, ni * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(P.qpos, B.qpos, ni * nq * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(P.qvel, B.qvel, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(P.warm, B.qacc_warmstart, ni * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(P.cnt, B.counters, ni * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   }
-  for (int j = 0; j < npred; ++j) {
+  for (int j = 0; j < k.npred; ++j) {
     RolloutArgs A; memset(&A, 0, sizeof(A));
-    A.qpos0 = p->dl_qpos; A.qvel0 = p->dl_qvel; A.warm0 = p->dl_warm;
-    A.counters_in = p->dl_cnt; A.counters_out = p->dl_cnt;
+    A.qpos0 = P.qpos; A.qvel0 = P.qvel; A.warm0 = P.warm;
+    A.counters_in = P.cnt; A.counters_out = P.cnt;
     A.nrows = ni; A.H = 1; A.mode = 0; A.rows_per_inst = 1;
-    A.us = (obs ? p->ob.seq : p->dl_pending) + (size_t)j * nu; A.us_row = DIAL_MAXDELAY * nu;
+    A.us = (k.obs ? p->ob.seq : Q.pending) + (size_t)j * nu; A.us_row = DIAL_MAXDELAY * nu;
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
-    A.models = p->n_ens > 0 ? p->dl_models : p->models.d;
-    A.iter_lim = obs ? p->ob.len : p->dl_len; A.iter = j;
-    A.qpos_out = p->dl_qpos; A.qvel_out = p->dl_qvel; A.warm_out = p->dl_warm;
+    A.models = p->n_ens > 0 ? P.models : p->models.d;
+    A.iter_lim = k.obs ? p->ob.len : Q.len; A.iter = j;
+    A.qpos_out = P.qpos; A.qvel_out = P.qvel; A.warm_out = P.warm;
     CUDA_OK(launch_rollout(p, A, 1, st));
   }
-  if (obs || npred > 0) { qpos0 = p->dl_qpos; qvel0 = p->dl_qvel; warm0 = p->dl_warm; cnt0 = p->dl_cnt; }
+  if (k.planning()) { qpos0 = P.qpos; qvel0 = P.qvel; warm0 = P.warm; cnt0 = P.cnt; }
   // The info-only bars (qbar, qdbar, xbar; dial_core.py:133-135) are computed for EVERY iteration,
   // like the reference's scan does (the caller sees those of the last one), on a side branch of
   // the graph: the bars of iteration i read trajectory buffer i&1 and weights buffer i&1 while
@@ -2091,24 +2052,26 @@ extern "C" int dial_mpc_step(dial_plan* p, int n_diffuse, int env_step, void* st
                   " diffusion iterations, its schedule has " + std::to_string(S.n_rows) + " rows");
   }
   cudaStream_t st = (cudaStream_t)stream;
-  p->dl_pred_last = p->delay.d ? p->dl_pred : 0;   // (a change of dl_pred drops the graphs)
-  p->ob_last = p->obs.d != nullptr;                 // (the first observation setting drops them)
+  // the cached graphs replay the launch sequence of the last step's key: when the settings changed it, the next
+  // use of each shape runs eagerly and the one after captures it again
+  if (p->key != p->ran) drop_graphs(p);
+  p->ran = p->key;
   dial_plan::MpcGraph* g = nullptr;
   for (auto& e : p->mpc_graphs) if (e.n_diffuse == n_diffuse && e.env_step == env_step) g = &e;
   if (!g) {
     // first use of this shape: run it eagerly (also configures the kernels' shared-memory limits)
     p->mpc_graphs.push_back({n_diffuse, env_step, 1, nullptr, 0});
-    return mpc_enqueue(p, n_diffuse, env_step, st);
+    return mpc_enqueue(p, p->ran, n_diffuse, env_step, st);
   }
   if (!g->exec) {
-    if (getenv("DIAL_NO_GRAPH")) return mpc_enqueue(p, n_diffuse, env_step, st);
+    if (getenv("DIAL_NO_GRAPH")) return mpc_enqueue(p, p->ran, n_diffuse, env_step, st);
     // second use: capture the same sequence into a graph, then replay it from now on
     cudaStream_t cs;
     CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
     const int64_t l0 = p->launches;
     cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) { cudaStreamDestroy(cs); CUDA_OK(e); }
-    int rc = mpc_enqueue(p, n_diffuse, env_step, cs);
+    int rc = mpc_enqueue(p, p->ran, n_diffuse, env_step, cs);
     cudaGraph_t graph = nullptr;
     e = cudaStreamEndCapture(cs, &graph);
     cudaStreamDestroy(cs);

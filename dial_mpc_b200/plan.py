@@ -116,7 +116,8 @@ class Plan:
         """Instance b adapts its belief over its members to the plant at every env step (``on``), with
         ``forget`` in (0, 1], ``prune`` in [0, 1/K) and ``sigma`` [nv] > 0; or stops (the belief is kept).
         A stream-ordered copy on the current stream; the first call that turns adaptation on in a plan
-        makes the next steps capture their graphs again (``dial_plan_set_ensemble_adapt``)."""
+        changes the launch sequence, so the next steps capture their graphs again; later calls keep them
+        (``dial_plan_set_ensemble_adapt``)."""
         s = None
         if sigma is not None:
             a = np.ascontiguousarray(sigma, dtype=np.float32).ravel()
@@ -145,7 +146,8 @@ class Plan:
         """Instance b's sampling schedule from the next ``mpc_step`` on: softmax temperature ``temp`` and
         noise rows ``noise`` [n_rows, Hnode+1] (fp32, n_rows in 1..64); ``noise=None`` returns it to the
         plan's temp_sample and the bound noise.  A stream-ordered copy on the current stream; the first
-        call on a plan makes the next steps capture their graphs again (``dial_plan_set_instance_schedule``)."""
+        call on a plan changes the launch sequence, so the next steps capture their graphs again; later calls
+        keep them (``dial_plan_set_instance_schedule``)."""
         if noise is None:
             self._check(self.lib.dial_plan_set_instance_schedule(self.handle, int(b), float(temp), 0, None, _stream()))
             return

@@ -323,7 +323,10 @@ int dial_exchange_status(dial_plan* plan, uint32_t out[6]);
  * counters, rng and control knots stay in HBM (caller-owned `dial_mpc_buffers`), the key
  * splitting / shift / counter bookkeeping between kernels runs as tiny glue kernels, and
  * `dial_mpc_step` only replays the graph (captured on the second use of an
- * (n_diffuse, env_step) shape; the first use runs eagerly).  Results equal the eager
+ * (n_diffuse, env_step) shape; the first use runs eagerly).  The graphs are captured again when the
+ * launch sequence changes: a feature's first setting, or a change in the number of prediction launches or
+ * in whether any instance predicts through its delay; other settings take effect at the next replay.
+ * Results equal the eager
  * `dial_env_step` + `dial_reverse_*` sequence.  Sharded plans (Ntotal > Nsample) need a connected
  * exchange: every rank replays the same graph, the env step runs redundantly on every rank. */
 typedef struct dial_mpc_buffers { /* all [dev], caller-owned, fixed while bound */
@@ -515,10 +518,11 @@ int dial_plan_set_instance_iterations(dial_plan* plan, const int32_t* n_iter, vo
 
 /* Instance b's delay `steps` (0..DIAL_MAXDELAY) and `predict` (0 or 1).  Every call refills b's queue with
  * `steps` copies of Y[b][0] as it stands when the call's stream-ordered work runs on `stream` (so the plan
- * must be bound, dial_mpc_bind).  The first call allocates the queues and planning-state buffers and drops
- * the captured graphs; a later call that changes the plan's largest delay, or the largest delay of a
- * predicting instance, drops them too (the launch sequence changes); other calls keep them, and take effect
- * at the next replay.  Fails for b out of range and for a bad argument, which the error names. */
+ * must be bound, dial_mpc_bind).  The first call allocates the queues and planning-state buffers.  The
+ * graphs are captured again when the launch sequence changes: at the first call, and at a call that changes
+ * the number of prediction launches or whether any instance predicts through its delay; other calls keep
+ * them, and take effect at the next replay.  Fails for b out of range and for a bad argument, which the
+ * error names. */
 int dial_plan_set_instance_delay(dial_plan* plan, int b, int steps, int predict, void* stream);
 
 /* Each instance's queue in application order: out [dev][n_inst][DIAL_MAXDELAY][nu], row j < d_b the action
@@ -562,8 +566,8 @@ int dial_plan_planning_state(dial_plan* plan, float* qpos, float* qvel, float* w
  * nullable: zero), key [host][2] (nullable: {0, 0}).  A delay of 0 with every sigma 0 removes the setting:
  * the instance plans from its plant state again.  Every call resets b's ring and restarts its noise from
  * `key`, stream-ordered on `stream` (so the plan must be bound, dial_mpc_bind).  The first call allocates the
- * rings and drops the captured graphs; a later call that changes the number of prediction launches drops them
- * too; other calls keep them, and take effect at the next replay.  Fails for b out of range, a delay out of
+ * rings; it and a later call that changes the number of prediction launches make the graphs be captured
+ * again; other calls keep them, and take effect at the next replay.  Fails for b out of range, a delay out of
  * range or one whose sum with b's action delay exceeds DIAL_MAXDELAY, a negative or non-finite sigma, and
  * sharded or unbound plans; the error names the bad argument. */
 int dial_plan_set_instance_observation(dial_plan* plan, int b, int delay, const float* qpos_std,
