@@ -315,7 +315,7 @@ class DeviceLoop:
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
                  compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                 schedule=None, delay=None, observe=None):
+                 schedule=None, delay=None, observe=None, pushes=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -369,7 +369,13 @@ class DeviceLoop:
         rollouts start from the plant record min(k, records - 1) env steps old plus Gaussian noise drawn once
         per env step; a predicting instance (its delay spec's ``predict``) first takes the actions applied since
         that record and its queued ones.  The plant, its reward and adaptation keep the plant state
-        (``set_observation``, ``observed_state``, ``planning_state``)."""
+        (``set_observation``, ``observed_state``, ``planning_state``).
+
+        ``pushes``: each instance's pushes, one push spec for every instance or a list of B specs or None
+        (``push_setting``: a list of ``{"step": s, "steps": n, "body": name, "pos": p, "force": f, "torque": t}``).
+        After each env step whose post-step counter lies in [s, s + n), the plant's qvel takes the impulse of
+        the force at the point p of the body and of the torque, held over that env step.  The planner is not
+        told; the trigger moves with the counter (``set_state(step=...)``) (``set_pushes``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -449,6 +455,14 @@ class DeviceLoop:
             observe = [None if spec is None else observe_setting(spec, m) for spec in observe]
             if rand[0] and any(o is not None and o[0] > 0 for o in observe):
                 raise ValueError(self._RAND_OBSERVE)
+        if pushes is not None:
+            if mbdpi.world_size != 1:
+                raise ValueError("pushes= needs an unsharded plan (world_size 1)")
+            # a list of B lists (or Nones) is per instance; a list of mappings is one spec for every instance
+            pushes = self._per_instance("pushes", pushes, f"one push spec or a list of {B}",
+                                        lambda s: isinstance(s, (list, tuple)) and len(s) > 0 and
+                                        all(x is None or isinstance(x, (list, tuple)) for x in s))
+            pushes = [push_setting(spec, m) for spec in pushes]
         # each instance's DialConfig, whether it has a table of its own, and the iteration limits last
         # uploaded (None: no limits, every instance runs every iteration of a step)
         self._cfg, self._own, self._lims = [a] * B, [False] * B, None
@@ -520,6 +534,9 @@ class DeviceLoop:
         for b, o in enumerate(observe or ()):
             if o is not None and self._observing(o):   # nor does a loop without observations
                 self._set_observation(b, o)
+        for b, table in enumerate(pushes or ()):
+            if table:                                   # nor does a loop without pushes
+                self.plan.set_instance_pushes(b, table)
 
     @staticmethod
     def _model(env_or_sys):
@@ -701,6 +718,12 @@ class DeviceLoop:
         if self._rand and setting[0] > 0:
             raise ValueError(self._RAND_OBSERVE)
         self._set_observation(b, setting)
+
+    def set_pushes(self, b: int, spec) -> None:
+        """Instance b's push table from the next ``step`` on (a push spec, ``push_setting``; None or [] clears
+        it).  A stream-ordered copy on the current stream.  The first table of a loop changes the launch sequence:
+        the next steps capture their graphs again.  Later calls keep them."""
+        self.plan.set_instance_pushes(self._instance(b), push_setting(spec, self.mbdpi.env.sys))
 
     def observed_state(self) -> Dict[str, torch.Tensor]:
         """The observation the last step planned from, before any prediction: new tensors ``qpos``, ``qvel``,
@@ -1068,6 +1091,63 @@ def observe_setting(spec, sys):
     return delay, q, v, np.asarray(key, np.uint32)
 
 
+PUSH_KEYS = ("step", "steps", "body", "pos", "force", "torque")
+
+
+def push_setting(spec, sys) -> list:
+    """A push spec -> the push table of ``dial_plan_set_instance_pushes`` (a list of ``_capi.dial_push``) for the
+    model of ``sys`` (a ``System``, an env or a ``CompiledModel``).  The spec is a list of at most 16 mappings of
+    ``step`` (the first post-step counter ``info["step"]`` the push fires at, >= 1), ``steps`` (the env steps it
+    fires in, >= 1, default 1), ``body`` (a body name other than the world), ``pos`` (the point of application
+    in the body's frame, default its origin), ``force`` [N] and ``torque`` [N m] (world frame, default zero).
+    After each env step it fires in, the plant's qvel takes the impulse of the force and torque held over that
+    step.  An empty list (or None) is no pushes.  Raises ValueError naming the entry and the bad key or value."""
+    model = getattr(getattr(sys, "sys", sys), "model", getattr(sys, "sys", sys))
+    pmax = _capi.DEFINES["DIAL_MAXPUSH"]
+    if spec is None:
+        return []
+    if not isinstance(spec, (list, tuple)):
+        raise ValueError(f"a push spec is a list of mappings of {', '.join(PUSH_KEYS)}, got {spec!r}")
+    if len(spec) > pmax:
+        raise ValueError(f"a push spec has at most {pmax} entries, got {len(spec)}")
+    bodies = model.names.get("body", [])
+    out = []
+    for i, e in enumerate(spec):
+        at = f"push {i}: "
+        if not isinstance(e, dict):
+            raise ValueError(f"{at}an entry is a mapping of {', '.join(PUSH_KEYS)}, got {e!r}")
+        extra = sorted(set(e) - set(PUSH_KEYS), key=str)
+        if extra:
+            raise ValueError(f"{at}unknown key {extra[0]!r} (an entry takes {', '.join(map(repr, PUSH_KEYS))})")
+
+        def count(name, v):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= 0x7FFFFFFF:
+                raise ValueError(f"{at}{name} must be an int >= 1, got {v!r}")
+            return int(v)
+
+        def vec(name, v):
+            ok = isinstance(v, (list, tuple, np.ndarray)) and len(v) == 3 and all(
+                not isinstance(x, bool) and isinstance(x, (int, float, np.integer, np.floating)) and
+                math.isfinite(x) and abs(float(x)) <= float(np.finfo(np.float32).max) for x in v)
+            if not ok:
+                raise ValueError(f"{at}{name} must be a list of 3 finite numbers, got {v!r}")
+            return [float(x) for x in v]
+
+        if "step" not in e:
+            raise ValueError(f"{at}needs step, the post-step counter it fires at")
+        if "body" not in e:
+            raise ValueError(f"{at}needs body, the name of the body pushed")
+        body = e["body"]
+        if not isinstance(body, str) or body not in bodies[1:]:
+            raise ValueError(f"{at}unknown body {body!r} (known: {bodies[1:]})")
+        p = _capi.dial_push()
+        p.step, p.n_steps, p.body = count("step", e["step"]), count("steps", e.get("steps", 1)), bodies.index(body)
+        for name in ("pos", "force", "torque"):
+            getattr(p, name)[:] = vec(name, e.get(name, [0.0, 0.0, 0.0]))
+        out.append(p)
+    return out
+
+
 def load_setting(spec, key: str, K: int, nv: Optional[int] = None):
     """The ``risk``, ``adapt`` or ``prior`` entry ``key`` of an ``--ensemble`` file or an
     ``--instance-overrides`` mapping, checked for K members and nv dofs (``risk_setting``,
@@ -1124,7 +1204,7 @@ def load_ensemble(spec, env):
 
 
 def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                  schedule=None, delay=None, observe=None):
+                  schedule=None, delay=None, observe=None, pushes=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
@@ -1133,7 +1213,8 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
     ``adapt`` from the belief ``prior`` (``DeviceLoop(..., adapt=..., prior=...)``).  ``schedule``: B schedule
     specs or None (``DeviceLoop(..., schedule=...)``); each instance runs its own Ndiffuse_init, then Ndiffuse.
     ``delay``: one delay spec or B of them (``DeviceLoop(..., delay=...)``).  ``observe``: one observe spec or B
-    of them (``DeviceLoop(..., observe=...)``)."""
+    of them (``DeviceLoop(..., observe=...)``).  ``pushes``: one push spec or B of them
+    (``DeviceLoop(..., pushes=...)``)."""
     mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
@@ -1141,7 +1222,7 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
     loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior,
-                      schedule=schedule, delay=delay, observe=observe)
+                      schedule=schedule, delay=delay, observe=observe, pushes=pushes)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -1220,6 +1301,12 @@ def main():
                              "steps old (0..16) with Gaussian noise of standard deviation 'qpos' / 'qvel' (one number, "
                              "nv numbers or a mapping of joint names); an --instance-overrides mapping may carry its "
                              "own 'observe'")
+    parser.add_argument("--push", type=str, default=None, metavar="SPEC",
+                        help="push every instance's simulated robot: a YAML flow list such as "
+                             "'[{step: 50, body: base, force: [60, 0, 0], steps: 5}]'; after each env step whose "
+                             "counter lies in [step, step + steps) the robot takes the impulse of 'force' [N] at 'pos' "
+                             "(body frame, default the body's origin) and 'torque' [N m] (world frame) held over that "
+                             "step; the planner is not told; an --instance-overrides mapping may carry its own 'push'")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -1260,6 +1347,14 @@ def main():
             observe = yaml.safe_load(args.observe)
         except yaml.YAMLError as e:
             parser.error(f"--observe: not a YAML mapping: {e}")
+    push = None
+    if args.push is not None:
+        if args.eager:
+            parser.error("--push runs on the CUDA-graph loop; it excludes --eager")
+        try:
+            push = yaml.safe_load(args.push)
+        except yaml.YAMLError as e:
+            parser.error(f"--push: not a YAML list: {e}")
     rng = drandom.PRNGKey(seed=dial_config.seed)
     env_config_type = dial_envs.get_config(dial_config.env_name)
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
@@ -1271,6 +1366,11 @@ def main():
                 raise ValueError(DeviceLoop._RAND_OBSERVE)
         except ValueError as e:
             parser.error(f"--observe: {e}")
+    if push is not None:
+        try:
+            push_setting(push, env.sys)
+        except ValueError as e:
+            parser.error(f"--push: {e}")
     envs = None
     members, plant, risk, adapt, prior = None, None, None, None, None
     if args.ensemble is not None:
@@ -1294,17 +1394,18 @@ def main():
         # DialConfig fields: the sampling schedule (SCHEDULE_FIELDS), or fields shared by the plan, which
         # schedule_setting rejects by name
         dial_fields = {f.name for f in dataclasses.fields(DialConfig)} - env_fields
-        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay", "observe"}
+        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay", "observe", "push"}
         envs = []
         settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
         uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
         schedule = [None] * args.instances
         delays = [delay] * args.instances
         observes = [observe] * args.instances
+        pushes = [push] * args.instances
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt, delay, observe "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt, delay, observe, push "
                              f"or the sampling fields {', '.join(SCHEDULE_FIELDS)}, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
@@ -1331,6 +1432,13 @@ def main():
                     parser.error(f"--instance-overrides entry {b}: observe: {e}")
                 observes[b] = ov["observe"]
             ov.pop("observe", None)
+            if ov.get("push") is not None:
+                try:
+                    push_setting(ov["push"], env.sys)
+                except ValueError as e:
+                    parser.error(f"--instance-overrides entry {b}: push: {e}")
+                pushes[b] = ov["push"]
+            ov.pop("push", None)
             for key in ("risk", "adapt"):
                 if ov.get(key) is not None:
                     if members is None:
@@ -1369,10 +1477,12 @@ def main():
             delay = [d or (0, False) for d in delays]
         if args.instance_overrides is not None and any(o is not None for o in observes):
             observe = observes
+        if args.instance_overrides is not None and any(q is not None for q in pushes):
+            push = pushes
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
                       ensemble=members, risk=risk, adapt=adapt, prior=prior,
                       schedule=schedule if args.instance_overrides is not None and any(schedule) else None,
-                      delay=None if delay is None else _delay_specs(delay), observe=observe)
+                      delay=None if delay is None else _delay_specs(delay), observe=observe, pushes=push)
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
@@ -1385,11 +1495,13 @@ def main():
         parser.error("--delay needs an unsharded plan (one process)")
     if observe is not None and mbdpi.world_size != 1:
         parser.error("--observe needs an unsharded plan (one process)")
+    if push is not None and mbdpi.world_size != 1:
+        parser.error("--push needs an unsharded plan (one process)")
     if mbdpi.world_size == 1 and not args.eager:
         # one CUDA graph per control step; the host launches it and logs
         loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk,
                           adapt=adapt, prior=prior, delay=None if delay is None else _delay_specs(delay),
-                          observe=observe)
+                          observe=observe, pushes=push)
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):

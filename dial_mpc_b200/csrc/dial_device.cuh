@@ -888,6 +888,267 @@ DEV void observe_emit(const ObsSetting& s, const ObsRing& r1, const dial_model_d
 }
 
 // ---------------------------------------------------------------------------------
+// per-instance pushes (dial_plan_set_instance_pushes)
+// ---------------------------------------------------------------------------------
+// This is a separate, plain fp64 restatement of the kinematics, the COM-frame inertias and motion axes and the
+// CRB mass matrix, not a reuse of physics_step's sections: those are fused and tuned for the rollout kernel's
+// instruction stream, and sharing them would put this feature into rollout_kernel.  It runs only in an env step
+// at which some push fires, on one warp per instance (push_kernel), so its cost does not matter.
+//
+// Instance b's push table: its n entries (dial_push, include/dial_b200.h).
+struct alignas(16) PushTable {
+  int32_t n;
+  int32_t pad[3];
+  dial_push e[DIAL_MAXPUSH];
+};
+// entry e fires after the env step whose post-step counter is `step`: step in [e.step, e.step + n_steps)
+HD bool push_fires(const dial_push& e, int step) { return step >= e.step && step - e.step < e.n_steps; }
+HD bool push_any(const PushTable& T, int step) {
+  for (int i = 0; i < T.n; ++i)
+    if (push_fires(T.e[i], step)) return true;
+  return false;
+}
+// The fp64 workspace of one instance's push (shared memory in push_kernel): the body frames, the subtree COM of
+// each body's tree root, the composite inertias (cinert layout, COM frame), the dofs' motion axes, the mass
+// matrix (its Cholesky factor after push_solve) and the generalized impulse (Delta qvel after push_solve).
+struct PushWork {
+  double xpos[DIAL_MAXB][3], xquat[DIAL_MAXB][4], xmat[DIAL_MAXB][9];
+  double xipos[DIAL_MAXB][3], ximat[DIAL_MAXB][9];
+  double xanchor[DIAL_MAXB][3], xaxis[DIAL_MAXB][3];
+  double com[DIAL_MAXB][3];
+  double crb[DIAL_MAXB][10];
+  double cdof[DIAL_MAXV][6];
+  double M[DIAL_MAXV][DIAL_MAXV];
+  double g[DIAL_MAXV];
+};
+HD void pd_qmul(const double* a, const double* b, double* r) {
+  const double w = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
+  const double x = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
+  const double y = a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1];
+  const double z = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
+  r[0] = w; r[1] = x; r[2] = y; r[3] = z;
+}
+HD void pd_qrot(const double* q, const double* v, double* r) {   // mjx math.rotate
+  const double s = q[0], uv = q[1] * v[0] + q[2] * v[1] + q[3] * v[2], uu = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  const double c[3] = {q[2] * v[2] - q[3] * v[1], q[3] * v[0] - q[1] * v[2], q[1] * v[1] - q[2] * v[0]};
+  for (int i = 0; i < 3; ++i) r[i] = 2.0 * uv * q[1 + i] + (s * s - uu) * v[i] + 2.0 * s * c[i];
+}
+HD void pd_qnormalize(double* q) {
+  const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  const double d = n + (n == 0.0 ? 1e-6 : 0.0);
+  for (int i = 0; i < 4; ++i) q[i] /= d;
+}
+HD void pd_qmat(const double* q, double* m) {   // row-major 3x3
+  const double w = q[0], x = q[1], y = q[2], z = q[3];
+  m[0] = w * w + x * x - y * y - z * z; m[1] = 2 * (x * y - w * z); m[2] = 2 * (x * z + w * y);
+  m[3] = 2 * (x * y + w * z); m[4] = w * w - x * x + y * y - z * z; m[5] = 2 * (y * z - w * x);
+  m[6] = 2 * (x * z - w * y); m[7] = 2 * (y * z + w * x); m[8] = w * w - x * x - y * y + z * z;
+}
+HD void pd_cross(const double* a, const double* b, double* r) {
+  const double x = a[1] * b[2] - a[2] * b[1], y = a[2] * b[0] - a[0] * b[2], z = a[0] * b[1] - a[1] * b[0];
+  r[0] = x; r[1] = y; r[2] = z;
+}
+// cinert (10) times a motion vector (6) (mjx inert_mul)
+HD void pd_inert_mul(const double* ci, const double* v, double* r) {
+  const double I[9] = {ci[0], ci[3], ci[4], ci[3], ci[1], ci[5], ci[4], ci[5], ci[2]};
+  double pw[3], pv[3];
+  pd_cross(ci + 6, v + 3, pw);
+  pd_cross(ci + 6, v, pv);
+  for (int i = 0; i < 3; ++i) {
+    r[i] = I[3 * i] * v[0] + I[3 * i + 1] * v[1] + I[3 * i + 2] * v[2] + pw[i];
+    r[3 + i] = ci[9] * v[3 + i] - pv[i];
+  }
+}
+// Stage 1 of a push (one caller): the body frames at qpos (quaternions normalised as mjx.kinematics does), the
+// subtree COM of every tree root, each body's inertia about its root's COM, the composite inertias (each body's
+// summed over its subtree, the world's zero) and the dofs' motion axes about their root's COM, on the model m
+// (free, hinge and slide joints).
+DEV void push_kinematics(const dial_model_desc& m, const float* qpos, PushWork& W) {
+  const int nb = m.nbody;
+  for (int i = 0; i < 3; ++i) { W.xpos[0][i] = 0.0; W.xanchor[0][i] = 0.0; W.xaxis[0][i] = 0.0; }
+  W.xquat[0][0] = 1.0; W.xquat[0][1] = 0.0; W.xquat[0][2] = 0.0; W.xquat[0][3] = 0.0;
+  for (int b = 1; b < nb; ++b) {
+    const int p = m.body_parentid[b];
+    double bp[3], bq[4], pos[3], quat[4];
+    for (int i = 0; i < 3; ++i) bp[i] = m.body_pos[b][i];
+    for (int i = 0; i < 4; ++i) bq[i] = m.body_quat[b][i];
+    pd_qrot(W.xquat[p], bp, pos);
+    for (int i = 0; i < 3; ++i) pos[i] += W.xpos[p][i];
+    pd_qmul(W.xquat[p], bq, quat);
+    double anchor[3] = {0.0, 0.0, 0.0}, axis[3] = {0.0, 0.0, 0.0};
+    const int j = m.body_jntadr[b];
+    if (j >= 0) {
+      const int qa = m.jnt_qposadr[j], t = m.jnt_type[j];
+      if (t == JNT_FREE) {
+        for (int i = 0; i < 3; ++i) { pos[i] = qpos[qa + i]; anchor[i] = pos[i]; }
+        axis[2] = 1.0;
+        for (int i = 0; i < 4; ++i) quat[i] = qpos[qa + 3 + i];
+        pd_qnormalize(quat);
+      } else {
+        double jp[3], ja[3], r[3];
+        for (int i = 0; i < 3; ++i) { jp[i] = m.jnt_pos[j][i]; ja[i] = m.jnt_axis[j][i]; }
+        pd_qrot(quat, jp, r);
+        for (int i = 0; i < 3; ++i) anchor[i] = r[i] + pos[i];
+        pd_qrot(quat, ja, axis);
+        const double ang = (double)qpos[qa] - (double)m.qpos0[qa];
+        if (t == JNT_HINGE) {
+          const double s = sin(0.5 * ang), c = cos(0.5 * ang);
+          const double ql[4] = {c, ja[0] * s, ja[1] * s, ja[2] * s};
+          double q2[4];
+          pd_qmul(quat, ql, q2);
+          for (int i = 0; i < 4; ++i) quat[i] = q2[i];
+          pd_qrot(quat, jp, r);
+          for (int i = 0; i < 3; ++i) pos[i] = anchor[i] - r[i];
+        } else {   // slide
+          for (int i = 0; i < 3; ++i) pos[i] += axis[i] * ang;
+        }
+      }
+    }
+    pd_qnormalize(quat);
+    for (int i = 0; i < 3; ++i) { W.xpos[b][i] = pos[i]; W.xanchor[b][i] = anchor[i]; W.xaxis[b][i] = axis[i]; }
+    for (int i = 0; i < 4; ++i) W.xquat[b][i] = quat[i];
+  }
+  // inertial frames; the mass-weighted sums of each tree root (accumulated in com, normalised below)
+  double msum[DIAL_MAXB];
+  for (int b = 0; b < nb; ++b) {
+    double ip[3], iq[4], q2[4], r[3];
+    for (int i = 0; i < 3; ++i) ip[i] = m.body_ipos[b][i];
+    for (int i = 0; i < 4; ++i) iq[i] = m.body_iquat[b][i];
+    pd_qmat(W.xquat[b], W.xmat[b]);
+    pd_qrot(W.xquat[b], ip, r);
+    for (int i = 0; i < 3; ++i) W.xipos[b][i] = W.xpos[b][i] + r[i];
+    pd_qmul(W.xquat[b], iq, q2);
+    pd_qmat(q2, W.ximat[b]);
+    msum[b] = 0.0;
+    for (int i = 0; i < 3; ++i) W.com[b][i] = 0.0;
+  }
+  for (int b = 0; b < nb; ++b) {
+    const int r = m.body_rootid[b];
+    msum[r] += (double)m.body_mass[b];
+    for (int i = 0; i < 3; ++i) W.com[r][i] += (double)m.body_mass[b] * W.xipos[b][i];
+  }
+  for (int b = 0; b < nb; ++b) {   // roots first: a root is its own root and precedes its subtree
+    const int r = m.body_rootid[b];
+    if (r != b) continue;
+    for (int i = 0; i < 3; ++i) W.com[b][i] = msum[b] < (double)DIAL_MINVAL ? W.xipos[b][i] : W.com[b][i] / msum[b];
+  }
+  for (int b = 0; b < nb; ++b) {
+    const int r = m.body_rootid[b];
+    if (r != b) for (int i = 0; i < 3; ++i) W.com[b][i] = W.com[r][i];
+  }
+  // cinert of each body about its root's COM: R diag(I) R^T + m (|o|^2 1 - o o^T), [Ixx Iyy Izz Ixy Ixz Iyz | m o | m]
+  for (int b = 0; b < nb; ++b) {
+    const double mass = m.body_mass[b];
+    double o[3], I[9];
+    for (int i = 0; i < 3; ++i) o[i] = W.xipos[b][i] - W.com[b][i];
+    const double o2 = o[0] * o[0] + o[1] * o[1] + o[2] * o[2];
+    for (int i = 0; i < 3; ++i)
+      for (int k = 0; k < 3; ++k) {
+        double s = 0.0;
+        for (int l = 0; l < 3; ++l) s += W.ximat[b][3 * i + l] * (double)m.body_inertia[b][l] * W.ximat[b][3 * k + l];
+        I[3 * i + k] = s + mass * ((i == k ? o2 : 0.0) - o[i] * o[k]);
+      }
+    double* c = W.crb[b];
+    c[0] = I[0]; c[1] = I[4]; c[2] = I[8]; c[3] = I[1]; c[4] = I[2]; c[5] = I[5];
+    for (int i = 0; i < 3; ++i) c[6 + i] = o[i] * mass;
+    c[9] = mass;
+  }
+  for (int b = nb - 1; b > 0; --b) {
+    const int p = m.body_parentid[b];
+    if (p > 0) for (int i = 0; i < 10; ++i) W.crb[p][i] += W.crb[b][i];
+  }
+  for (int i = 0; i < 10; ++i) W.crb[0][i] = 0.0;
+  // the motion axes of the dofs about their root's COM: [angular | linear]
+  for (int b = 1; b < nb; ++b) {
+    const int j = m.body_jntadr[b];
+    if (j < 0) continue;
+    const int d = m.jnt_dofadr[j], t = m.jnt_type[j];
+    double off[3];
+    for (int i = 0; i < 3; ++i) off[i] = W.com[b][i] - W.xanchor[b][i];
+    if (t == JNT_FREE) {
+      for (int i = 0; i < 3; ++i) {
+        double* tr = W.cdof[d + i];
+        double* rot = W.cdof[d + 3 + i];
+        for (int k = 0; k < 6; ++k) tr[k] = 0.0;
+        tr[3 + i] = 1.0;
+        const double ax[3] = {W.xmat[b][i], W.xmat[b][3 + i], W.xmat[b][6 + i]};
+        for (int k = 0; k < 3; ++k) rot[k] = ax[k];
+        pd_cross(ax, off, rot + 3);
+      }
+    } else if (t == JNT_HINGE) {
+      for (int k = 0; k < 3; ++k) W.cdof[d][k] = W.xaxis[b][k];
+      pd_cross(W.xaxis[b], off, W.cdof[d] + 3);
+    } else {
+      for (int k = 0; k < 3; ++k) { W.cdof[d][k] = 0.0; W.cdof[d][3 + k] = W.xaxis[b][k]; }
+    }
+  }
+}
+// Stage 2 of a push (after stage 1), for the dofs i = a0, a0 + da, ... < nv (a warp passes its lanes): row i of
+// the CRB mass matrix M = cdof^T crb cdof on the ancestor pattern, armature on the diagonal, and the generalized
+// impulse g[i] = sum over the entries firing at `step` of cdof_i . [torque + (p - c) x force; force] dt, p the
+// entry's world point and c its body's root COM (J^T [torque; force] dt).  Each caller writes its own rows only.
+DEV void push_rows(const DevModel& D, const PushTable& T, int step, double dt, PushWork& W, int a0, int da) {
+  const dial_model_desc& m = D.m;
+  const int nv = m.nv;
+  for (int i = a0; i < nv; i += da) {
+    double vi[6];
+    pd_inert_mul(W.crb[m.dof_bodyid[i]], W.cdof[i], vi);
+    for (int j = 0; j < nv; ++j) {
+      double s = 0.0;
+      if ((D.dof_ancmask[i] >> j) & 1u) {
+        for (int k = 0; k < 6; ++k) s += vi[k] * W.cdof[j][k];
+      } else if ((D.dof_ancmask[j] >> i) & 1u) {
+        double vj[6];
+        pd_inert_mul(W.crb[m.dof_bodyid[j]], W.cdof[j], vj);
+        for (int k = 0; k < 6; ++k) s += vj[k] * W.cdof[i][k];
+      }
+      W.M[i][j] = s + (i == j ? (double)m.dof_armature[i] : 0.0);
+    }
+    double g = 0.0;
+    for (int e = 0; e < T.n; ++e) {
+      const dial_push& P = T.e[e];
+      if (!push_fires(P, step) || !((D.body_dofmask[P.body] >> i) & 1u)) continue;
+      double pw[3], f[3], tq[3];
+      for (int k = 0; k < 3; ++k) {
+        pw[k] = W.xpos[P.body][k] + W.xmat[P.body][3 * k] * (double)P.pos[0] + W.xmat[P.body][3 * k + 1] * (double)P.pos[1] +
+                W.xmat[P.body][3 * k + 2] * (double)P.pos[2] - W.com[P.body][k];
+        f[k] = P.force[k];
+      }
+      pd_cross(pw, f, tq);
+      for (int k = 0; k < 3; ++k) g += W.cdof[i][k] * ((double)P.torque[k] + tq[k]) + W.cdof[i][3 + k] * f[k];
+    }
+    W.g[i] = g * dt;
+  }
+}
+// Stage 3 of a push (one caller, after stage 2 of every row): g = M^-1 g by a dense Cholesky factorisation
+// M = L L^T in place (the lower triangle) and two triangular solves.
+DEV void push_solve(int nv, PushWork& W) {
+  for (int k = 0; k < nv; ++k) {
+    double d = W.M[k][k];
+    for (int l = 0; l < k; ++l) d -= W.M[k][l] * W.M[k][l];
+    d = sqrt(d);
+    W.M[k][k] = d;
+    for (int i = k + 1; i < nv; ++i) {
+      double s = W.M[i][k];
+      for (int l = 0; l < k; ++l) s -= W.M[i][l] * W.M[k][l];
+      W.M[i][k] = s / d;
+    }
+  }
+  for (int i = 0; i < nv; ++i) {
+    double s = W.g[i];
+    for (int l = 0; l < i; ++l) s -= W.M[i][l] * W.g[l];
+    W.g[i] = s / W.M[i][i];
+  }
+  for (int i = nv - 1; i >= 0; --i) {
+    double s = W.g[i];
+    for (int l = i + 1; l < nv; ++l) s -= W.M[l][i] * W.g[l];
+    W.g[i] = s / W.M[i][i];
+  }
+}
+// qvel + Delta qvel, rounded once; a zero Delta leaves qvel bit for bit
+HD float push_add(float v, double dv) { return dv == 0.0 ? v : (float)((double)v + dv); }
+
+// ---------------------------------------------------------------------------------
 // per-warp context
 // ---------------------------------------------------------------------------------
 // "Compact chain coordinates": the mass matrix M and the Newton Hessian H = M + J^T D J of

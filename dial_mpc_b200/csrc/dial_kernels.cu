@@ -704,6 +704,29 @@ __global__ void observe_reset_kernel(int b, const ObsSetting* __restrict__ set, 
   ring[b] = r;
 }
 
+// Pushes (dial_plan_set_instance_pushes), one warp per instance b, after the plant's env step and adaptation's
+// belief update: when some entry of its table T[b] fires at its post-step counter, its plant qvel takes the
+// impulse response M^-1 J^T [torque; force] dt in fp64 on its plant model (models[b], else the plan's model M0):
+// push_kinematics on lane 0, the mass-matrix rows and the generalized impulse on every lane, the Cholesky solve
+// on lane 0.  An instance with no entry firing leaves at entry.
+__global__ void __launch_bounds__(32) push_kernel(const DevModel* __restrict__ M0, const DevModel* __restrict__ models,
+                                                  const PushTable* __restrict__ T, const int32_t* __restrict__ cnt,
+                                                  const float* __restrict__ qpos, float* __restrict__ qvel, double dt) {
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const int step = cnt[2 * b];
+  if (!push_any(T[b], step)) return;
+  __shared__ PushWork W;
+  const DevModel& D = models ? models[b] : *M0;
+  const int nq = D.m.nq, nv = D.m.nv;
+  if (lane == 0) push_kinematics(D.m, qpos + (size_t)b * nq, W);
+  __syncwarp();
+  push_rows(D, T[b], step, dt, W, lane, 32);
+  __syncwarp();
+  if (lane == 0) push_solve(nv, W);
+  __syncwarp();
+  for (int i = lane; i < nv; i += 32) qvel[(size_t)b * nv + i] = push_add(qvel[(size_t)b * nv + i], W.g[i]);
+}
+
 // ---------------------------------------------------------------------------------
 // plan object
 // ---------------------------------------------------------------------------------
@@ -754,13 +777,14 @@ template <class T> struct Staged {
 // control-step graph replays what mpc_enqueue enqueues under the key it was captured with.
 struct LaunchKey {
   bool models = false, members = false, sched = false, lims = false, adapt = false, delay = false, obs = false;
+  bool push = false;       // some instance was given a push table: the push launch runs after every env step
   bool predicts = false;   // some instance predicts through a delay d_b > 0: the queue launch also runs without an env step
   int npred = 0;           // prediction launches
   // the planner's rollouts start from the planning state, not the plant state
   bool planning() const { return obs || npred > 0; }
   bool operator!=(const LaunchKey& o) const {
     return models != o.models || members != o.members || sched != o.sched || lims != o.lims || adapt != o.adapt ||
-           delay != o.delay || obs != o.obs || predicts != o.predicts || npred != o.npred;
+           delay != o.delay || obs != o.obs || push != o.push || predicts != o.predicts || npred != o.npred;
   }
 };
 
@@ -850,6 +874,9 @@ struct dial_plan {
   // the device) and, allocated with them by the first call, the rings and observations
   Staged<ObsSetting> obs;
   ObsBuffers ob{};
+  // per-instance push tables (dial_plan_set_instance_pushes): [n_inst] slots (the staging mirrors the device),
+  // allocated by the first table set
+  Staged<PushTable> pushes;
   // the plan's device buffers that cudaMalloc allocated, by the address of the pointer holding each (own)
   std::vector<void**> owned;
   // cudaMalloc `bytes` into `ptr`, which the plan owns from then on (free_since, dial_plan_destroy); with
@@ -897,7 +924,7 @@ static LaunchKey launch_key(const dial_plan* p) {
   LaunchKey k;
   k.models = p->models.d != nullptr; k.members = p->members.d != nullptr;
   k.sched = p->sched.d != nullptr; k.lims = p->lims.d != nullptr; k.adapt = p->pred_qd != nullptr;
-  k.delay = p->delay.d != nullptr; k.obs = p->obs.d != nullptr;
+  k.delay = p->delay.d != nullptr; k.obs = p->obs.d != nullptr; k.push = p->pushes.d != nullptr;
   for (int b = 0; k.delay && b < p->n_inst; ++b) {
     const DelaySetting& s = p->delay.h[b];
     const int n = s.d + (k.obs && p->obs.h[b].on ? p->obs.h[b].k : 0);
@@ -927,7 +954,7 @@ extern "C" int dial_abi_version(void) { return DIAL_ABI_VERSION; }
 extern "C" const char* dial_last_error(void) { return g_err.c_str(); }
 extern "C" size_t dial_sizeof(int which) {
   return which == 0 ? sizeof(dial_model_desc) : which == 1 ? sizeof(dial_plan_desc) : which == 2 ? sizeof(dial_state)
-       : which == 3 ? sizeof(dial_mpc_buffers) : which == 4 ? sizeof(dial_task) : 0;
+       : which == 3 ? sizeof(dial_mpc_buffers) : which == 4 ? sizeof(dial_task) : which == 5 ? sizeof(dial_push) : 0;
 }
 
 // solver instantiation by tree shape: star<3,6> (quadruped), star<5,7> (humanoid), star<5,6>,
@@ -1148,7 +1175,7 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   cudaFree(p->xch.bars_partial);
   p->models.release(); p->members.release(); p->risk.release();
   p->adapt.release(); p->belief_L.release(); p->belief_w.release(); p->sched.release(); p->lims.release();
-  p->delay.release(); p->obs.release();
+  p->delay.release(); p->obs.release(); p->pushes.release();
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   p->free_since(0);
@@ -1551,6 +1578,49 @@ extern "C" int dial_plan_set_instance_observation(dial_plan* p, int b, int delay
   return 0;
 }
 
+extern "C" int dial_plan_set_instance_pushes(dial_plan* p, int b, int n, const dial_push* pushes, void* stream) {
+  static const char* fn = "dial_plan_set_instance_pushes";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (int rc = need_instance(p, fn, b)) return rc;
+  if (n < 0 || n > DIAL_MAXPUSH)
+    return fail(std::string(fn) + ": n " + std::to_string(n) + " out of range (0.." DIAL_STR(DIAL_MAXPUSH) ")");
+  if (n > 0 && !pushes) return fail(std::string(fn) + ": null pushes");
+  const int nbody = p->hM.m.nbody;
+  for (int i = 0; i < n; ++i) {
+    const dial_push& e = pushes[i];
+    const std::string at = std::string(fn) + ": pushes[" + std::to_string(i) + "].";
+    if (e.body < 1 || e.body >= nbody)
+      return fail(at + "body " + std::to_string(e.body) + (e.body == 0 ? " is the world" : " out of range") +
+                  " (1.." + std::to_string(nbody - 1) + ")");
+    if (e.step < 1) return fail(at + "step must be >= 1, got " + std::to_string(e.step));
+    if (e.n_steps < 1) return fail(at + "n_steps must be >= 1, got " + std::to_string(e.n_steps));
+    for (int k = 0; k < 9; ++k) {
+      const float x = k < 3 ? e.pos[k] : k < 6 ? e.force[k - 3] : e.torque[k - 6];
+      if (!std::isfinite(x))
+        return fail(at + (k < 3 ? "pos[" : k < 6 ? "force[" : "torque[") + std::to_string(k % 3) + "] is not finite, got " + fmt_g(x));
+    }
+  }
+  const dial_plan_desc& c = p->hP.c;
+  if (c.Ntotal != c.Nsample || p->xch.on) return fail(std::string(fn) + ": sharded plans (Ntotal != Nsample) have no per-instance pushes");
+  if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
+  if (n == 0 && !p->pushes.d) return 0;   // no instance has a table: b is already unpushed
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (!p->pushes.d) {
+    PushTable none;
+    memset(&none, 0, sizeof(none));
+    if ((e = p->pushes.allocate(p->n_inst, 1, none)) != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  }
+  e = p->pushes.put(b, [&](PushTable* T) {
+    memset(T, 0, sizeof(*T));
+    T->n = n;
+    for (int i = 0; i < n; ++i) T->e[i] = pushes[i];
+  }, st);
+  p->key = launch_key(p);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
 extern "C" int dial_plan_observed_state(dial_plan* p, float* qpos, float* qvel, float* warm, int32_t* counters,
                                         int32_t* age, void* stream) {
   static const char* fn = "dial_plan_observed_state";
@@ -1915,6 +1985,12 @@ static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_
   }
   if (adapt) {   // each adapting instance's belief from its members' predictions and the observed qvel
     ens_belief_kernel<<<ni, 32, 0, st>>>(p->pred_qd, B.qvel, p->adapt.d, K, p->hM.m.nv, p->belief_L.d, p->belief_w.d, p->dEll);
+    p->launches++;
+    CUDA_OK(cudaGetLastError());
+  }
+  if (env_step == 1 && k.push) {   // pushes, on the post-step plant state; dt: the env step's duration
+    const double dt = (double)c.n_frames * (double)p->hM.m.timestep;
+    push_kernel<<<ni, 32, 0, st>>>(p->dM, p->models.d, p->pushes.d, B.counters, B.qpos, B.qvel, dt);
     p->launches++;
     CUDA_OK(cudaGetLastError());
   }

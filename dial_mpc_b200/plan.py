@@ -225,6 +225,13 @@ class Plan:
         self._check(self.lib.dial_plan_observed_state(self.handle, _ptr(qpos), _ptr(qvel), _ptr(warm), ints[0], ints[1],
                                                       _stream()))
 
+    def set_instance_pushes(self, b: int, pushes) -> None:
+        """Instance b's push table from the next ``mpc_step`` on: a sequence of at most 16 ``_capi.dial_push``
+        (empty: no pushes).  A stream-ordered copy on the current stream (``dial_plan_set_instance_pushes``)."""
+        pushes = list(pushes)
+        arr = (_capi.dial_push * max(len(pushes), 1))(*pushes)
+        self._check(self.lib.dial_plan_set_instance_pushes(self.handle, int(b), len(pushes), arr, _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

@@ -45,6 +45,7 @@ extern "C" {
 #define DIAL_MAXENS 16  /* planning models (ensemble members) of one instance */
 #define DIAL_MAXDIFFUSE 64 /* diffusion iterations of one control step (dial_mpc_step) */
 #define DIAL_MAXDELAY 16   /* control steps of latency of one instance (dial_plan_set_instance_delay) */
+#define DIAL_MAXPUSH 16    /* entries of one instance's push table (dial_plan_set_instance_pushes) */
 #define DIAL_IPC_HANDLE_BYTES 64
 
 /* environments (reward functors fused into the rollout kernel) */
@@ -189,7 +190,7 @@ typedef struct dial_plan dial_plan;
 int dial_abi_version(void);
 const char* dial_last_error(void);
 /* sizeof() of the descriptor structs as compiled into the library: which = 0 model, 1 plan,
- * 2 state, 3 mpc buffers, 4 task (lets foreign-language bindings verify their struct layout). */
+ * 2 state, 3 mpc buffers, 4 task, 5 push (lets foreign-language bindings verify their struct layout). */
 size_t dial_sizeof(int which);
 
 /* Create / destroy a plan (uploads model + config, allocates all workspaces). */
@@ -579,6 +580,42 @@ int dial_plan_set_instance_observation(dial_plan* plan, int b, int delay, const 
  * the first step after the first setting.  Stream-ordered copies on `stream`. */
 int dial_plan_observed_state(dial_plan* plan, float* qpos, float* qvel, float* warm, int32_t* counters,
                              int32_t* age, void* stream);
+
+/* One entry of an instance's push table (dial_plan_set_instance_pushes): after each env step of dial_mpc_step
+ * whose post-step counter info["step"] lies in [step, step + n_steps), the plant takes the impulse of the
+ * force `force` [N] applied at the point `pos` of body `body` and of the torque `torque` [N m], held for the
+ * env step's duration.  pos is in the body's frame, force and torque in the world frame. */
+typedef struct dial_push {
+  int32_t step;      /* first post-step counter it fires at, >= 1 */
+  int32_t n_steps;   /* env steps it fires in, >= 1 */
+  int32_t body;      /* 1..nbody-1 (not the world) */
+  float pos[3], force[3], torque[3];
+} dial_push;
+
+/* Per-instance pushes of dial_mpc_step: instance b's plant may be pushed between env steps, the standard test
+ * of how well a controller recovers.  A push is an impulse on the plant state, applied after the env step
+ * (and after adaptation's belief update) and before the shift, the observation and the prediction:
+ *   qvel += M(q)^-1 J^T [torque; force] dt
+ * with M the instance's plant mass matrix (armature included) at the post-step qpos, J the spatial Jacobian
+ * (rotational rows, then translational) of the world point of `pos` on `body`, and dt = n_frames * timestep
+ * the env step's duration; qpos is not changed.  Entries that fire in the same step add up.  A force held over
+ * n env steps is a train of n impulses with the force's total impulse, each applied at the end of its step: the
+ * physics steps inside an env step do not see it.  The reward of the env step at which a push fires does not
+ * see it, the next one does; adaptation scores its members against the unpushed qvel; the observation ring and
+ * the prediction start from the pushed state.  The planner is not told about pushes.  The trigger is the
+ * plant's own counter, so a replayed graph needs no state of its own, and moving the counter (as a new bound
+ * state does) moves the trigger with it.  Computed in fp64 from the fp32 state, then rounded once into qvel.
+ * Launches: once some instance was given a table, one push launch runs after every env step; an instance with
+ * no entry firing at its counter leaves it at entry.  A plan on which no table is ever set launches what it
+ * launched before. */
+
+/* Instance b's push table: n (0..DIAL_MAXPUSH) entries [host] (nullable when n = 0); n = 0 clears the table.
+ * The copy is stream-ordered on `stream` (the plan must be bound, dial_mpc_bind).  The first table set on a plan
+ * allocates the tables and drops the captured graphs; later calls keep them and take effect at the next
+ * replay.  Fails for b out of range, n out of range, a body out of range or the world body, step < 1,
+ * n_steps < 1, a non-finite pos, force or torque, and sharded or unbound plans; the error names the bad
+ * argument. */
+int dial_plan_set_instance_pushes(dial_plan* plan, int b, int n, const dial_push* pushes, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops

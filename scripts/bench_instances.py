@@ -24,8 +24,11 @@ a YAML flow mapping applied to every instance (``'{delay: 2, qpos: 0.01, qvel: 0
 one such mapping or a list of one per instance (null: none), so that the step also runs the observe launch and,
 for instances predicting through ``--delays``, max(k + d) prediction launches (use ``--env-step 1`` for the
 rings to move).
+``--pushes FILE.yaml``: each instance's plant is pushed between env steps (``DeviceLoop(..., pushes=...)``): one
+push spec for every instance or a list of one per instance (null: none), so that every step with an env step also
+runs the push launch (use ``--env-step 1``; an entry firing in every step measures the cost of a push).
 ``--profile-kernels``: instead of the timing, run the steps without graph capture under torch.profiler and
-print the mean device time per launch of the rollout, update, ensemble reduction, delay queue and observe
+print the mean device time per launch of the rollout, update, ensemble reduction, delay queue, observe and push
 kernels."""
 import argparse
 import copy
@@ -95,6 +98,10 @@ def main():
     ap.add_argument("--observe", default=None, metavar="SPEC_OR_FILE",
                     help="an observe spec for every instance (a YAML flow mapping such as '{delay: 2, qpos: 0.01}') or "
                          "a YAML file with one spec or a list of one per instance (DeviceLoop(..., observe=...))")
+    ap.add_argument("--pushes", default=None, metavar="FILE.yaml",
+                    help="a YAML file with one push spec for every instance or a list of one per instance (null: none) "
+                         "(DeviceLoop(..., pushes=...)); a push launch runs after every env step (--env-step 1), and "
+                         "a spec such as [{step: 1, steps: 1000000000, body: base, force: [50, 0, 0]}] fires in every one")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
@@ -110,7 +117,8 @@ def main():
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, delay_setting, observe_setting, schedule_setting
+    from dial_mpc_b200.core.dial_core import (MBDPI, DeviceLoop, delay_setting, observe_setting, push_setting,
+                                              schedule_setting)
 
     B, b = args.instances, BASELINE[args.config]
     cfg = dial_config(args.config, world=1)
@@ -183,12 +191,25 @@ def main():
             ap.error(f"--observe {args.observe}: {e}")
         # with the observe launch the prediction also runs through each predicting instance's observation delay
         n_pred = max([d + k for (d, p), k in zip(settings, ks) if p] or [0])
+    pushes = None
+    if args.pushes is not None:
+        import yaml
+        try:
+            pushes = yaml.safe_load(open(args.pushes))
+            per = isinstance(pushes, list) and len(pushes) > 0 and all(x is None or isinstance(x, list) for x in pushes)
+            if per and len(pushes) != B:
+                raise ValueError(f"a list of push specs needs {B} entries (one per instance), got {len(pushes)}")
+            for spec in pushes if per else [pushes]:
+                push_setting(spec, env.sys)
+        except (ValueError, yaml.YAMLError) as e:
+            ap.error(f"--pushes {args.pushes}: {e}")
     if B == 1:
         loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt,
-                          schedule=schedule, delay=delay, observe=observe)
+                          schedule=schedule, delay=delay, observe=observe, pushes=pushes)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
-                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule, delay=delay, observe=observe)
+                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule, delay=delay, observe=observe,
+                          pushes=pushes)
     es = args.env_step
     # without --schedules every step runs the config's Ndiffuse on every instance, as before
     nd = None if schedule is not None else cfg.Ndiffuse
@@ -209,7 +230,7 @@ def main():
             if "rollout_kernel" in ev.name:
                 rollouts.append((ev.time_range.start, ev.time_range.elapsed_us()))
             for key in ("update_kernel", "ensemble_reduce_kernel", "trajbar", "ens_gather_kernel", "ens_belief_kernel",
-                        "delay_queue_kernel", "observe_kernel"):
+                        "delay_queue_kernel", "observe_kernel", "push_kernel"):
                 if key in ev.name:
                     n, tot = acc.get(key, (0, 0.0))
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
@@ -222,7 +243,7 @@ def main():
             n, tot = acc.get(key, (0, 0.0))
             acc[key] = (n + 1, tot + us)
         print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
-                              risk=args.risk, adapt=args.adapt, delays=args.delays, observe=args.observe, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              risk=args.risk, adapt=args.adapt, delays=args.delays, observe=args.observe, pushes=args.pushes, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
                               launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
         return
     evs = []
@@ -239,7 +260,7 @@ def main():
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
                           distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
-                          schedules=args.schedules, delays=args.delays, observe=args.observe, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
+                          schedules=args.schedules, delays=args.delays, observe=args.observe, pushes=args.pushes, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
                           value=sum(n_diffuse) * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
 
