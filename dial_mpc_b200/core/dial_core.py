@@ -315,7 +315,7 @@ class DeviceLoop:
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
                  compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                 schedule=None, delay=None, observe=None, pushes=None):
+                 schedule=None, delay=None, observe=None, pushes=None, plant=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -375,7 +375,14 @@ class DeviceLoop:
         (``push_setting``: a list of ``{"step": s, "steps": n, "body": name, "pos": p, "force": f, "torque": t}``).
         After each env step whose post-step counter lies in [s, s + n), the plant's qvel takes the impulse of
         the force at the point p of the body and of the torque, held over that env step.  The planner is not
-        told; the trigger moves with the counter (``set_state(step=...)``) (``set_pushes``)."""
+        told; the trigger moves with the counter (``set_state(step=...)``) (``set_pushes``).
+
+        ``plant``: each instance's plant fidelity, one plant spec for every instance or a list of B specs (or
+        Nones) or None (``plant_setting``: a mapping of ``substeps`` or ``sim_dt``, ``iterations``,
+        ``ls_iterations`` and ``tolerance``, each defaulting to the planner's own).  With a spec, the instance's
+        env step makes substeps x n_frames physics steps of timestep / substeps on its plant model with those
+        solver settings, the control held across them; the planner, the members and the predictions keep the
+        plan's discretisation (``set_plant``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -463,6 +470,12 @@ class DeviceLoop:
                                         lambda s: isinstance(s, (list, tuple)) and len(s) > 0 and
                                         all(x is None or isinstance(x, (list, tuple)) for x in s))
             pushes = [push_setting(spec, m) for spec in pushes]
+        if plant is not None:
+            if mbdpi.world_size != 1:
+                raise ValueError("plant= needs an unsharded plan (world_size 1)")
+            plant = self._per_instance("plant", plant, f"one plant spec or a list of {B}",
+                                       lambda s: isinstance(s, (list, tuple)))
+            plant = [plant_setting(spec, m) for spec in plant]
         # each instance's DialConfig, whether it has a table of its own, and the iteration limits last
         # uploaded (None: no limits, every instance runs every iteration of a step)
         self._cfg, self._own, self._lims = [a] * B, [False] * B, None
@@ -537,6 +550,9 @@ class DeviceLoop:
         for b, table in enumerate(pushes or ()):
             if table:                                   # nor does a loop without pushes
                 self.plan.set_instance_pushes(b, table)
+        for b, f in enumerate(plant or ()):
+            if f is not None:                           # nor does a loop without plant settings
+                self.plan.set_instance_plant(b, f)
 
     @staticmethod
     def _model(env_or_sys):
@@ -724,6 +740,13 @@ class DeviceLoop:
         it).  A stream-ordered copy on the current stream.  The first table of a loop changes the launch sequence:
         the next steps capture their graphs again.  Later calls keep them."""
         self.plan.set_instance_pushes(self._instance(b), push_setting(spec, self.mbdpi.env.sys))
+
+    def set_plant(self, b: int, spec) -> None:
+        """Instance b's plant fidelity from the next ``step`` on (a plant spec, ``plant_setting``; None clears it:
+        the plant then steps like the planner).  Stream-ordered on the current stream.  The first setting of a
+        loop, and any later one that changes the set of distinct substep counts in use, changes the launch
+        sequence: the next steps capture their graphs again.  Other calls keep them."""
+        self.plan.set_instance_plant(self._instance(b), plant_setting(spec, self.mbdpi.env.sys))
 
     def observed_state(self) -> Dict[str, torch.Tensor]:
         """The observation the last step planned from, before any prediction: new tensors ``qpos``, ``qvel``,
@@ -1148,6 +1171,59 @@ def push_setting(spec, sys) -> list:
     return out
 
 
+PLANT_KEYS = ("substeps", "sim_dt", "iterations", "ls_iterations", "tolerance")
+
+
+def plant_setting(spec, sys):
+    """A plant spec -> the ``_capi.dial_plant`` of ``dial_plan_set_instance_plant`` for the model of ``sys`` (a
+    ``System``, an env or a ``CompiledModel``: the planner's model), or None for a None spec (no setting).  The
+    spec maps any of ``substeps`` (physics substeps per planner physics step, 1..16, default 1) or ``sim_dt``
+    (the plant's physics step in seconds; timestep / sim_dt must be an integer, the substeps, so that the env
+    step's dt / sim_dt is an integer too), ``iterations`` (Newton iterations, 1..100), ``ls_iterations`` (line
+    search iterations, 1..50) and ``tolerance`` (finite, >= 0).  The solver settings default to the model's own;
+    MuJoCo's defaults are 100, 50 and 1e-8.  An empty mapping is the identity setting: the plant steps like the
+    planner.  Raises ValueError naming the bad key or value."""
+    model = getattr(getattr(sys, "sys", sys), "model", getattr(sys, "sys", sys))
+    if spec is None:
+        return None
+    if not isinstance(spec, dict):
+        raise ValueError(f"a plant spec is a mapping of {', '.join(PLANT_KEYS)}, got {spec!r}")
+    extra = sorted(set(spec) - set(PLANT_KEYS), key=str)
+    if extra:
+        raise ValueError(f"unknown key {extra[0]!r} (a plant spec takes {', '.join(map(repr, PLANT_KEYS))})")
+    if "substeps" in spec and "sim_dt" in spec:
+        raise ValueError("a plant spec takes substeps or sim_dt, not both")
+
+    def count(name, v, hi):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= hi:
+            raise ValueError(f"{name} must be an int in 1..{hi}, got {v!r}")
+        return int(v)
+
+    kmax = _capi.DEFINES["DIAL_MAXSUBSTEPS"]
+    ts = float(model.timestep)
+    if "sim_dt" in spec:
+        s = spec["sim_dt"]
+        if isinstance(s, bool) or not isinstance(s, (int, float, np.integer, np.floating)) or not math.isfinite(s) or s <= 0:
+            raise ValueError(f"sim_dt must be a finite number > 0, got {s!r}")
+        k = round(ts / float(s))
+        if k < 1 or abs(ts / float(s) - k) > 1e-6 * k:
+            raise ValueError(f"sim_dt {s!r} must divide the model's timestep {ts:g} into an integer number of substeps")
+        if k > kmax:
+            raise ValueError(f"sim_dt {s!r} gives {k} substeps of the model's timestep {ts:g}, at most {kmax}")
+    else:
+        k = count("substeps", spec.get("substeps", 1), kmax)
+    f = _capi.dial_plant()
+    f.substeps = k
+    f.iterations = count("iterations", spec.get("iterations", int(model.iterations)), 100)
+    f.ls_iterations = count("ls_iterations", spec.get("ls_iterations", int(model.ls_iterations)), 50)
+    tol = spec.get("tolerance", float(model.tolerance))
+    if isinstance(tol, bool) or not isinstance(tol, (int, float, np.integer, np.floating)) or not math.isfinite(tol) or \
+            tol < 0 or abs(float(tol)) > float(np.finfo(np.float32).max):
+        raise ValueError(f"tolerance must be a finite number >= 0, got {tol!r}")
+    f.tolerance = float(tol)
+    return f
+
+
 def load_setting(spec, key: str, K: int, nv: Optional[int] = None):
     """The ``risk``, ``adapt`` or ``prior`` entry ``key`` of an ``--ensemble`` file or an
     ``--instance-overrides`` mapping, checked for K members and nv dofs (``risk_setting``,
@@ -1204,7 +1280,7 @@ def load_ensemble(spec, env):
 
 
 def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                  schedule=None, delay=None, observe=None, pushes=None):
+                  schedule=None, delay=None, observe=None, pushes=None, plant=None):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
@@ -1214,7 +1290,7 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
     specs or None (``DeviceLoop(..., schedule=...)``); each instance runs its own Ndiffuse_init, then Ndiffuse.
     ``delay``: one delay spec or B of them (``DeviceLoop(..., delay=...)``).  ``observe``: one observe spec or B
     of them (``DeviceLoop(..., observe=...)``).  ``pushes``: one push spec or B of them
-    (``DeviceLoop(..., pushes=...)``)."""
+    (``DeviceLoop(..., pushes=...)``).  ``plant``: one plant spec or B of them (``DeviceLoop(..., plant=...)``)."""
     mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
     states, rngs = [], []
     for b in range(B):
@@ -1222,7 +1298,7 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
     loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior,
-                      schedule=schedule, delay=delay, observe=observe, pushes=pushes)
+                      schedule=schedule, delay=delay, observe=observe, pushes=pushes, plant=plant)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -1307,6 +1383,13 @@ def main():
                              "counter lies in [step, step + steps) the robot takes the impulse of 'force' [N] at 'pos' "
                              "(body frame, default the body's origin) and 'torque' [N m] (world frame) held over that "
                              "step; the planner is not told; an --instance-overrides mapping may carry its own 'push'")
+    parser.add_argument("--plant", type=str, default=None, metavar="SPEC",
+                        help="step every instance's simulated robot at its own physics fidelity: a YAML flow mapping "
+                             "such as '{sim_dt: 0.005, iterations: 100, ls_iterations: 50, tolerance: 1e-8}' or "
+                             "'{substeps: 4}'; each env step makes 'substeps' (or timestep / sim_dt) physics steps per "
+                             "planner physics step with the control held, solved with the given settings (default: "
+                             "the planner's); the planner keeps its model; an --instance-overrides mapping may carry "
+                             "its own 'plant'")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -1355,6 +1438,14 @@ def main():
             push = yaml.safe_load(args.push)
         except yaml.YAMLError as e:
             parser.error(f"--push: not a YAML list: {e}")
+    fidelity = None
+    if args.plant is not None:
+        if args.eager:
+            parser.error("--plant runs on the CUDA-graph loop; it excludes --eager")
+        try:
+            fidelity = yaml.safe_load(args.plant)
+        except yaml.YAMLError as e:
+            parser.error(f"--plant: not a YAML mapping: {e}")
     rng = drandom.PRNGKey(seed=dial_config.seed)
     env_config_type = dial_envs.get_config(dial_config.env_name)
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
@@ -1371,6 +1462,11 @@ def main():
             push_setting(push, env.sys)
         except ValueError as e:
             parser.error(f"--push: {e}")
+    if fidelity is not None:
+        try:
+            plant_setting(fidelity, env.sys)
+        except ValueError as e:
+            parser.error(f"--plant: {e}")
     envs = None
     members, plant, risk, adapt, prior = None, None, None, None, None
     if args.ensemble is not None:
@@ -1394,7 +1490,7 @@ def main():
         # DialConfig fields: the sampling schedule (SCHEDULE_FIELDS), or fields shared by the plan, which
         # schedule_setting rejects by name
         dial_fields = {f.name for f in dataclasses.fields(DialConfig)} - env_fields
-        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay", "observe", "push"}
+        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay", "observe", "push", "plant"}
         envs = []
         settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
         uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
@@ -1402,10 +1498,11 @@ def main():
         delays = [delay] * args.instances
         observes = [observe] * args.instances
         pushes = [push] * args.instances
+        fidelities = [fidelity] * args.instances
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
-                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt, delay, observe, push "
+                parser.error(f"--instance-overrides entry {b} must map {env_config_type.__name__} fields, sys, risk, adapt, delay, observe, push, plant "
                              f"or the sampling fields {', '.join(SCHEDULE_FIELDS)}, got "
                              f"{sorted(set(ov) - known) if isinstance(ov, dict) else ov!r}")
             ov = dict(ov)
@@ -1439,6 +1536,13 @@ def main():
                     parser.error(f"--instance-overrides entry {b}: push: {e}")
                 pushes[b] = ov["push"]
             ov.pop("push", None)
+            if ov.get("plant") is not None:
+                try:
+                    plant_setting(ov["plant"], env.sys)
+                except ValueError as e:
+                    parser.error(f"--instance-overrides entry {b}: plant: {e}")
+                fidelities[b] = ov["plant"]
+            ov.pop("plant", None)
             for key in ("risk", "adapt"):
                 if ov.get(key) is not None:
                     if members is None:
@@ -1479,10 +1583,13 @@ def main():
             observe = observes
         if args.instance_overrides is not None and any(q is not None for q in pushes):
             push = pushes
+        if args.instance_overrides is not None and any(f is not None for f in fidelities):
+            fidelity = fidelities
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
                       ensemble=members, risk=risk, adapt=adapt, prior=prior,
                       schedule=schedule if args.instance_overrides is not None and any(schedule) else None,
-                      delay=None if delay is None else _delay_specs(delay), observe=observe, pushes=push)
+                      delay=None if delay is None else _delay_specs(delay), observe=observe, pushes=push,
+                      plant=fidelity)
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
@@ -1497,11 +1604,13 @@ def main():
         parser.error("--observe needs an unsharded plan (one process)")
     if push is not None and mbdpi.world_size != 1:
         parser.error("--push needs an unsharded plan (one process)")
+    if fidelity is not None and mbdpi.world_size != 1:
+        parser.error("--plant needs an unsharded plan (one process)")
     if mbdpi.world_size == 1 and not args.eager:
         # one CUDA graph per control step; the host launches it and logs
         loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk,
                           adapt=adapt, prior=prior, delay=None if delay is None else _delay_specs(delay),
-                          observe=observe, pushes=push)
+                          observe=observe, pushes=push, plant=fidelity)
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):

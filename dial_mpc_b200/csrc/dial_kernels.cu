@@ -778,13 +778,16 @@ template <class T> struct Staged {
 struct LaunchKey {
   bool models = false, members = false, sched = false, lims = false, adapt = false, delay = false, obs = false;
   bool push = false;       // some instance was given a push table: the push launch runs after every env step
+  bool plant = false;      // some instance was given a plant fidelity: the plant's env step runs on the plant slots
+  uint32_t plant_ks = 0;   // the distinct substep counts in use (bit k - 1: substeps k), one plant launch each
   bool predicts = false;   // some instance predicts through a delay d_b > 0: the queue launch also runs without an env step
   int npred = 0;           // prediction launches
   // the planner's rollouts start from the planning state, not the plant state
   bool planning() const { return obs || npred > 0; }
   bool operator!=(const LaunchKey& o) const {
     return models != o.models || members != o.members || sched != o.sched || lims != o.lims || adapt != o.adapt ||
-           delay != o.delay || obs != o.obs || push != o.push || predicts != o.predicts || npred != o.npred;
+           delay != o.delay || obs != o.obs || push != o.push || plant != o.plant || plant_ks != o.plant_ks ||
+           predicts != o.predicts || npred != o.npred;
   }
 };
 
@@ -877,6 +880,15 @@ struct dial_plan {
   // per-instance push tables (dial_plan_set_instance_pushes): [n_inst] slots (the staging mirrors the device),
   // allocated by the first table set
   Staged<PushTable> pushes;
+  // per-instance plant fidelity (dial_plan_set_instance_plant), allocated by the first setting: the settings
+  // [n_inst] (host only, substeps 0: none); the plant model slots [n_inst] (instance b's model, models[b] or the
+  // plan's, with its setting's timestep / k and solver settings); the plan descriptors of the plant, slot k - 1
+  // with n_frames = k * n_frames (refreshed while k is in use); and per substep count k the 0/1 mask [n_inst]
+  // of the instances in its group, slot k - 1 (the iteration limits of its launch)
+  std::vector<dial_plant> plant;
+  Staged<DevModel> plant_models;
+  Staged<DevPlan> plant_plans;
+  Staged<int32_t> plant_mask;
   // the plan's device buffers that cudaMalloc allocated, by the address of the pointer holding each (own)
   std::vector<void**> owned;
   // cudaMalloc `bytes` into `ptr`, which the plan owns from then on (free_since, dial_plan_destroy); with
@@ -917,6 +929,11 @@ static void drop_graphs(dial_plan* p) {
   p->mpc_graphs.clear();
 }
 
+// instance b's plant substep count: its setting's, or 1 without one
+static int plant_substeps(const dial_plan* p, int b) {
+  return p->plant.empty() || p->plant[b].substeps == 0 ? 1 : p->plant[b].substeps;
+}
+
 // The launch key of the plan's current settings (the staging mirrors the device).  The prediction runs
 // max(k_b + d_b) launches over the predicting instances, k_b the observation delay of an observing instance
 // while the observe launch runs, else 0.
@@ -925,6 +942,8 @@ static LaunchKey launch_key(const dial_plan* p) {
   k.models = p->models.d != nullptr; k.members = p->members.d != nullptr;
   k.sched = p->sched.d != nullptr; k.lims = p->lims.d != nullptr; k.adapt = p->pred_qd != nullptr;
   k.delay = p->delay.d != nullptr; k.obs = p->obs.d != nullptr; k.push = p->pushes.d != nullptr;
+  k.plant = p->plant_models.d != nullptr;
+  for (int b = 0; k.plant && b < p->n_inst; ++b) k.plant_ks |= 1u << (plant_substeps(p, b) - 1);
   for (int b = 0; k.delay && b < p->n_inst; ++b) {
     const DelaySetting& s = p->delay.h[b];
     const int n = s.d + (k.obs && p->obs.h[b].on ? p->obs.h[b].k : 0);
@@ -954,12 +973,16 @@ extern "C" int dial_abi_version(void) { return DIAL_ABI_VERSION; }
 extern "C" const char* dial_last_error(void) { return g_err.c_str(); }
 extern "C" size_t dial_sizeof(int which) {
   return which == 0 ? sizeof(dial_model_desc) : which == 1 ? sizeof(dial_plan_desc) : which == 2 ? sizeof(dial_state)
-       : which == 3 ? sizeof(dial_mpc_buffers) : which == 4 ? sizeof(dial_task) : which == 5 ? sizeof(dial_push) : 0;
+       : which == 3 ? sizeof(dial_mpc_buffers) : which == 4 ? sizeof(dial_task) : which == 5 ? sizeof(dial_push)
+       : which == 6 ? sizeof(dial_plant) : 0;
 }
 
 // solver instantiation by tree shape: star<3,6> (quadruped), star<5,7> (humanoid), star<5,6>,
 // dense<22> (elliptic cones), generic tree.  `wpc` warps per CTA (1..16; one kernel serves all).
-static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, cudaStream_t st) {
+// `dP`: the plan descriptor the launch reads (null: the plan's own); `generic`: the generic kernel of the
+// plan's variant even where a shape-specialised one matches (whose solver counts and n_frames are fixed).
+static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, cudaStream_t st,
+                                  const DevPlan* dP = nullptr, bool generic = false) {
   const size_t smem = sizeof(DevModel) + sizeof(DevPlan) + (size_t)wpc * p->hM.warp_floats * sizeof(float);
   int grid = (A.nrows + wpc - 1) / wpc;
   // per-instance or member models: ceil(model_rows / wpc) CTAs per model slot (rollout_kernel's row mapping)
@@ -971,24 +994,25 @@ static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, c
     if (e != cudaSuccess) return e;
   }
   p->launches++;
+  if (!dP) dP = p->dP;
 #ifndef DIAL_ONLY_VARIANT
-  if (p->shape > 0) return kShapes[p->shape - 1].launch(p->dM, p->dP, A, grid, wpc, smem, st);
+  if (p->shape > 0 && !generic) return kShapes[p->shape - 1].launch(p->dM, dP, A, grid, wpc, smem, st);
 #endif
   switch (p->variant) {
 #if DIAL_HAS_VARIANT(1)
-    case 1: return dial_launch_rollout_v1(p->dM, p->dP, A, grid, wpc, smem, st);
+    case 1: return dial_launch_rollout_v1(p->dM, dP, A, grid, wpc, smem, st);
 #endif
 #if DIAL_HAS_VARIANT(2)
-    case 2: return dial_launch_rollout_v2(p->dM, p->dP, A, grid, wpc, smem, st);
+    case 2: return dial_launch_rollout_v2(p->dM, dP, A, grid, wpc, smem, st);
 #endif
 #if DIAL_HAS_VARIANT(3)
-    case 3: return dial_launch_rollout_v3(p->dM, p->dP, A, grid, wpc, smem, st);
+    case 3: return dial_launch_rollout_v3(p->dM, dP, A, grid, wpc, smem, st);
 #endif
 #if DIAL_HAS_VARIANT(4)
-    case 4: return dial_launch_rollout_v4(p->dM, p->dP, A, grid, wpc, smem, st);
+    case 4: return dial_launch_rollout_v4(p->dM, dP, A, grid, wpc, smem, st);
 #endif
 #if DIAL_HAS_VARIANT(0)
-    case 0: return dial_launch_rollout_v0(p->dM, p->dP, A, grid, wpc, smem, st);
+    case 0: return dial_launch_rollout_v0(p->dM, dP, A, grid, wpc, smem, st);
 #endif
     default: return cudaErrorInvalidDeviceFunction;
   }
@@ -1176,6 +1200,7 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   p->models.release(); p->members.release(); p->risk.release();
   p->adapt.release(); p->belief_L.release(); p->belief_w.release(); p->sched.release(); p->lims.release();
   p->delay.release(); p->obs.release(); p->pushes.release();
+  p->plant_models.release(); p->plant_plans.release(); p->plant_mask.release();
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   p->free_since(0);
@@ -1197,6 +1222,27 @@ extern "C" int dial_rollout(dial_plan* p, const dial_state* s, const float* us, 
   return 0;
 }
 
+// The plant's plan descriptors of the substep counts in `ks` (bit k - 1: k), from the plan's host mirror with
+// n_frames = k * n_frames, stream-ordered on `st` (nothing before the first plant setting)
+static cudaError_t put_plant_plans(dial_plan* p, uint32_t ks, cudaStream_t st) {
+  cudaError_t e = cudaSuccess;
+  for (int k = 1; p->plant_plans.d && k <= DIAL_MAXSUBSTEPS && e == cudaSuccess; ++k)
+    if ((ks >> (k - 1)) & 1u)
+      e = p->plant_plans.put(k - 1, [&](DevPlan* h) { *h = p->hP; h->c.n_frames = k * p->hP.c.n_frames; }, st);
+  return e;
+}
+
+// Instance b's plant model: its instance model (the staging mirrors the device) or the plan's, with the
+// timestep and solver settings of its plant setting
+static DevModel plant_model(const dial_plan* p, int b) {
+  DevModel D = p->models.d ? p->models.h[b] : p->hM;
+  const dial_plant& f = p->plant[b];
+  if (f.substeps == 0) return D;
+  D.m.timestep = D.m.timestep / (float)f.substeps;
+  D.m.iterations = f.iterations; D.m.ls_iterations = f.ls_iterations; D.m.tolerance = f.tolerance;
+  return D;
+}
+
 extern "C" int dial_plan_set_command(dial_plan* p, int cmd_step, const float* vel, const float* ang, void* stream) {
   if (!p) return fail("dial_plan_set_command: null plan");
   if (cmd_step >= 0 && (!vel || !ang)) return fail("dial_plan_set_command: null command");
@@ -1207,6 +1253,7 @@ extern "C" int dial_plan_set_command(dial_plan* p, int cmd_step, const float* ve
   const size_t off = offsetof(dial_plan_desc, cmd_step);
   CUDA_OK(cudaMemcpyAsync((char*)p->dP + off, (const char*)&p->hP.c + off, sizeof(int32_t) + 6 * sizeof(float),
                           cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  CUDA_OK(put_plant_plans(p, p->key.plant_ks, (cudaStream_t)stream));
   return 0;
 }
 
@@ -1228,6 +1275,7 @@ extern "C" int dial_plan_set_stages(dial_plan* p, int n_stage, const float* pose
   const size_t off = offsetof(dial_plan_desc, n_stage), end = offsetof(dial_plan_desc, n_user);
   CUDA_OK(cudaMemcpyAsync((char*)p->dP + off, (const char*)&p->hP.c + off, end - off, cudaMemcpyHostToDevice,
                           (cudaStream_t)stream));
+  CUDA_OK(put_plant_plans(p, p->key.plant_ks, (cudaStream_t)stream));
   return 0;
 }
 
@@ -1276,7 +1324,13 @@ extern "C" int dial_plan_set_instance_model(dial_plan* p, int b, const dial_mode
   if (!p || !m) return fail(std::string(fn) + ": null argument");
   if (int rc = need_instance(p, fn, b)) return rc;
   if (p->hP.c.Ntotal != p->hP.c.Nsample) return fail(std::string(fn) + ": sharded plans (Ntotal != Nsample) share one model");
-  return set_model_slot(p, fn, p->models, (size_t)p->n_inst, (size_t)b, m, (cudaStream_t)stream);
+  if (int rc = set_model_slot(p, fn, p->models, (size_t)p->n_inst, (size_t)b, m, (cudaStream_t)stream)) return rc;
+  // instance b's plant: the new model with its fidelity kept
+  if (p->plant_models.d) {
+    cudaError_t e = p->plant_models.put(b, [&](DevModel* h) { *h = plant_model(p, b); }, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  }
+  return 0;
 }
 
 extern "C" int dial_plan_set_ensemble_model(dial_plan* p, int b, int k, const dial_model_desc* m, void* stream) {
@@ -1617,6 +1671,59 @@ extern "C" int dial_plan_set_instance_pushes(dial_plan* p, int b, int n, const d
     for (int i = 0; i < n; ++i) T->e[i] = pushes[i];
   }, st);
   p->key = launch_key(p);
+  if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int dial_plan_set_instance_plant(dial_plan* p, int b, const dial_plant* f, void* stream) {
+  static const char* fn = "dial_plan_set_instance_plant";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (int rc = need_instance(p, fn, b)) return rc;
+  if (f) {   // (the comparisons also reject NaN)
+    const std::string at = std::string(fn) + ": ";
+    if (f->substeps < 1 || f->substeps > DIAL_MAXSUBSTEPS)
+      return fail(at + "substeps " + std::to_string(f->substeps) + " out of range (1.." DIAL_STR(DIAL_MAXSUBSTEPS) ")");
+    if (f->iterations < 1 || f->iterations > 100)
+      return fail(at + "iterations " + std::to_string(f->iterations) + " out of range (1..100)");
+    if (f->ls_iterations < 1 || f->ls_iterations > 50)
+      return fail(at + "ls_iterations " + std::to_string(f->ls_iterations) + " out of range (1..50)");
+    if (!(f->tolerance >= 0.f && f->tolerance <= FLT_MAX))
+      return fail(at + "tolerance must be finite and >= 0, got " + fmt_g(f->tolerance));
+  }
+  const dial_plan_desc& c = p->hP.c;
+  if (c.Ntotal != c.Nsample || p->xch.on) return fail(std::string(fn) + ": sharded plans (Ntotal != Nsample) have no per-instance plant");
+  if (!p->mpc_bound) return fail(std::string(fn) + ": call dial_mpc_bind first");
+  if (!f && !p->plant_models.d) return 0;   // no instance has a setting: b already steps like its planner
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t B = (size_t)p->n_inst;
+  cudaError_t e = cudaSuccess;
+  if (!p->plant_models.d) {
+    // first setting: every plant slot holds its instance's model (uploaded synchronously: nothing reads the
+    // slots yet), every plan slot the plan's descriptor, every instance is in the group of substeps 1
+    p->plant.assign(B, dial_plant{0, 0, 0, 0.f});
+    if ((e = p->plant_models.allocate(B, 1, p->hM)) == cudaSuccess && p->models.d) {
+      for (size_t i = 0; i < B; ++i) p->plant_models.h[i] = p->models.h[i];
+      e = cudaMemcpy(p->plant_models.d, p->plant_models.h, B * sizeof(DevModel), cudaMemcpyHostToDevice);
+    }
+    if (e == cudaSuccess) e = p->plant_plans.allocate(DIAL_MAXSUBSTEPS, 1, p->hP);
+    if (e == cudaSuccess && B > 1) e = p->plant_mask.allocate(DIAL_MAXSUBSTEPS, B, 0);
+    if (e == cudaSuccess && B > 1) e = p->plant_mask.put(0, [&](int32_t* M) { for (size_t i = 0; i < B; ++i) M[i] = 1; }, st);
+    if (e != cudaSuccess) {
+      p->plant_models.release(); p->plant_plans.release(); p->plant_mask.release(); p->plant.clear();
+      return fail(std::string(fn) + ": " + cudaGetErrorString(e));
+    }
+  }
+  const int k0 = plant_substeps(p, b);
+  p->plant[b] = f ? *f : dial_plant{0, 0, 0, 0.f};
+  const int k1 = plant_substeps(p, b);
+  const uint32_t ks0 = p->key.plant_ks;
+  p->key = launch_key(p);
+  e = p->plant_models.put(b, [&](DevModel* h) { *h = plant_model(p, b); }, st);
+  // the groups b left and joined; the plan slots of substep counts that came into use
+  for (int k : {k0, k1})
+    if (e == cudaSuccess && B > 1 && k0 != k1)
+      e = p->plant_mask.put(k - 1, [&](int32_t* M) { for (size_t i = 0; i < B; ++i) M[i] = plant_substeps(p, (int)i) == k; }, st);
+  if (e == cudaSuccess) e = put_plant_plans(p, p->key.plant_ks & ~ks0, st);
   if (e != cudaSuccess) return fail(std::string(fn) + ": " + cudaGetErrorString(e));
   return 0;
 }
@@ -1981,7 +2088,17 @@ static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
     A.models = p->models.d;
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
-    CUDA_OK(launch_rollout(p, A, 1, st));
+    if (!k.plant) CUDA_OK(launch_rollout(p, A, 1, st));
+    // with plant fidelities: one launch of the generic kernel per distinct substep count k, on the plant slots
+    // and the plan descriptor of k; batched, the rows of the other groups exit at entry (mask k as the
+    // launch's iteration limits, iteration 0), so every instance's state, counters, reward and ctrl are
+    // written once
+    for (int s_ = 0; k.plant && s_ < DIAL_MAXSUBSTEPS; ++s_) {
+      if (!((k.plant_ks >> s_) & 1u)) continue;
+      A.models = p->plant_models.d;
+      if (batched) { A.iter_lim = p->plant_mask.d + (size_t)s_ * ni; A.iter = 0; }
+      CUDA_OK(launch_rollout(p, A, 1, st, p->plant_plans.d + s_, true));
+    }
   }
   if (adapt) {   // each adapting instance's belief from its members' predictions and the observed qvel
     ens_belief_kernel<<<ni, 32, 0, st>>>(p->pred_qd, B.qvel, p->adapt.d, K, p->hM.m.nv, p->belief_L.d, p->belief_w.d, p->dEll);

@@ -232,6 +232,12 @@ class Plan:
         arr = (_capi.dial_push * max(len(pushes), 1))(*pushes)
         self._check(self.lib.dial_plan_set_instance_pushes(self.handle, int(b), len(pushes), arr, _stream()))
 
+    def set_instance_plant(self, b: int, plant) -> None:
+        """Instance b's plant fidelity from the next ``mpc_step`` on: a ``_capi.dial_plant`` (None: the plan's own).
+        Stream-ordered on the current stream (``dial_plan_set_instance_plant``)."""
+        self._check(self.lib.dial_plan_set_instance_plant(self.handle, int(b), None if plant is None else C.byref(plant),
+                                                          _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

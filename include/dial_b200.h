@@ -46,6 +46,7 @@ extern "C" {
 #define DIAL_MAXDIFFUSE 64 /* diffusion iterations of one control step (dial_mpc_step) */
 #define DIAL_MAXDELAY 16   /* control steps of latency of one instance (dial_plan_set_instance_delay) */
 #define DIAL_MAXPUSH 16    /* entries of one instance's push table (dial_plan_set_instance_pushes) */
+#define DIAL_MAXSUBSTEPS 16 /* physics substeps per plan physics step of one instance's plant (dial_plan_set_instance_plant) */
 #define DIAL_IPC_HANDLE_BYTES 64
 
 /* environments (reward functors fused into the rollout kernel) */
@@ -190,7 +191,8 @@ typedef struct dial_plan dial_plan;
 int dial_abi_version(void);
 const char* dial_last_error(void);
 /* sizeof() of the descriptor structs as compiled into the library: which = 0 model, 1 plan,
- * 2 state, 3 mpc buffers, 4 task, 5 push (lets foreign-language bindings verify their struct layout). */
+ * 2 state, 3 mpc buffers, 4 task, 5 push, 6 plant (lets foreign-language bindings verify their struct
+ * layout). */
 size_t dial_sizeof(int which);
 
 /* Create / destroy a plan (uploads model + config, allocates all workspaces). */
@@ -616,6 +618,37 @@ typedef struct dial_push {
  * n_steps < 1, a non-finite pos, force or torque, and sharded or unbound plans; the error names the bad
  * argument. */
 int dial_plan_set_instance_pushes(dial_plan* plan, int b, int n, const dial_push* pushes, void* stream);
+
+/* One instance's plant fidelity (dial_plan_set_instance_plant): how finely its plant integrates and solves the
+ * physics of an env step.  The planner's own settings are the plan model's timestep, iterations, ls_iterations
+ * and tolerance with substeps 1. */
+typedef struct dial_plant {
+  int32_t substeps, iterations, ls_iterations;   /* 1..DIAL_MAXSUBSTEPS, 1..100, 1..50 */
+  float tolerance;                                /* finite, >= 0 */
+} dial_plant;
+
+/* Per-instance plant fidelity of dial_mpc_step: instance b's plant may integrate the same physics more finely
+ * and solve its contacts further than the planner's model, as a real robot or a finer simulator does.  With a
+ * setting, instance b's env step makes substeps * n_frames physics steps of timestep / substeps on its plant
+ * model: its instance model (dial_plan_set_instance_model) or the plan's model, with the setting's iterations,
+ * ls_iterations and tolerance.  The control is computed once, from the pre-step state, and held across all of
+ * them; the reward is computed once, on the post-step state; info["step"] and the env step's duration
+ * n_frames * timestep (dial_plan_desc.dt) are unchanged.  Nothing else changes: the planner's rollouts,
+ * ensemble members, adaptation's member steps, the prediction through a delay or observation and the push
+ * impulse keep the plan's own discretisation.  substeps 1 with the plan model's solver settings computes
+ * bitwise what an instance without a setting computes.
+ * Launches: once some instance was given a setting, the plant's env step is one launch of the plan's generic
+ * solver variant (never a shape-specialised kernel) per distinct substep count in use, each over every
+ * instance with the others exiting at entry; an instance without a setting is in the group of substeps 1.  A
+ * plan on which no setting is ever made launches what it launched before. */
+
+/* Instance b's plant fidelity [host]; f = NULL clears it (b's plant then steps like its planner).  The copies
+ * are stream-ordered on `stream` (the plan must be bound, dial_mpc_bind).  The first setting on a plan
+ * allocates the plant model slots and drops the captured graphs, and so does any later call that changes the
+ * set of distinct substep counts in use; other calls keep them and take effect at the next replay.  A later
+ * dial_plan_set_instance_model(b) reaches b's plant with its fidelity kept.  Fails for b out of range, a field
+ * out of range, and sharded or unbound plans; the error names the bad argument. */
+int dial_plan_set_instance_plant(dial_plan* plan, int b, const dial_plant* f, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops

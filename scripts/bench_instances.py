@@ -27,6 +27,10 @@ rings to move).
 ``--pushes FILE.yaml``: each instance's plant is pushed between env steps (``DeviceLoop(..., pushes=...)``): one
 push spec for every instance or a list of one per instance (null: none), so that every step with an env step also
 runs the push launch (use ``--env-step 1``; an entry firing in every step measures the cost of a push).
+``--plant SPEC``: every instance's plant steps at its own fidelity (``DeviceLoop(..., plant=...)``): a YAML flow
+mapping such as ``'{substeps: 4, iterations: 100, ls_iterations: 50, tolerance: 1e-8}'`` applied to every instance,
+or a YAML file with one spec or a list of one per instance (null: none), so that a step with an env step runs one
+plant launch per distinct substep count (use ``--env-step 1``).
 ``--profile-kernels``: instead of the timing, run the steps without graph capture under torch.profiler and
 print the mean device time per launch of the rollout, update, ensemble reduction, delay queue, observe and push
 kernels."""
@@ -102,6 +106,9 @@ def main():
                     help="a YAML file with one push spec for every instance or a list of one per instance (null: none) "
                          "(DeviceLoop(..., pushes=...)); a push launch runs after every env step (--env-step 1), and "
                          "a spec such as [{step: 1, steps: 1000000000, body: base, force: [50, 0, 0]}] fires in every one")
+    ap.add_argument("--plant", default=None, metavar="SPEC_OR_FILE",
+                    help="a plant spec for every instance (a YAML flow mapping such as '{substeps: 4}') or a YAML file "
+                         "with one spec or a list of one per instance (DeviceLoop(..., plant=...))")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
@@ -117,8 +124,8 @@ def main():
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import (MBDPI, DeviceLoop, delay_setting, observe_setting, push_setting,
-                                              schedule_setting)
+    from dial_mpc_b200.core.dial_core import (MBDPI, DeviceLoop, delay_setting, observe_setting, plant_setting,
+                                              push_setting, schedule_setting)
 
     B, b = args.instances, BASELINE[args.config]
     cfg = dial_config(args.config, world=1)
@@ -203,13 +210,22 @@ def main():
                 push_setting(spec, env.sys)
         except (ValueError, yaml.YAMLError) as e:
             ap.error(f"--pushes {args.pushes}: {e}")
+    plant = None
+    if args.plant is not None:
+        import yaml
+        try:
+            plant = yaml.safe_load(open(args.plant)) if os.path.exists(args.plant) else yaml.safe_load(args.plant)
+            for spec in plant if isinstance(plant, list) else [plant]:
+                plant_setting(spec, env.sys)
+        except (ValueError, yaml.YAMLError) as e:
+            ap.error(f"--plant {args.plant}: {e}")
     if B == 1:
         loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt,
-                          schedule=schedule, delay=delay, observe=observe, pushes=pushes)
+                          schedule=schedule, delay=delay, observe=observe, pushes=pushes, plant=plant)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
                           ensemble=members, risk=risk, adapt=adapt, schedule=schedule, delay=delay, observe=observe,
-                          pushes=pushes)
+                          pushes=pushes, plant=plant)
     es = args.env_step
     # without --schedules every step runs the config's Ndiffuse on every instance, as before
     nd = None if schedule is not None else cfg.Ndiffuse
@@ -236,14 +252,17 @@ def main():
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
         # the rollout launches of one step in order: [member prediction, env step (env_step 1)], [the delay
         # prediction steps], the planner's
-        per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) + \
+        # with plant settings the env step is one launch per distinct substep count
+        specs = (plant if isinstance(plant, list) else [plant] * B) if plant is not None else []
+        n_plant = len({plant_setting(sp, env.sys).substeps if sp is not None else 1 for sp in specs}) if specs else 1
+        per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) * n_plant + \
             ["delay prediction"] * n_pred + ["plan"] * max(n_diffuse)
         for i, (_, us) in enumerate(sorted(rollouts)):
             key = f"rollout_kernel ({per_step[i % len(per_step)]})"
             n, tot = acc.get(key, (0, 0.0))
             acc[key] = (n + 1, tot + us)
         print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
-                              risk=args.risk, adapt=args.adapt, delays=args.delays, observe=args.observe, pushes=args.pushes, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              risk=args.risk, adapt=args.adapt, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
                               launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
         return
     evs = []
@@ -260,7 +279,7 @@ def main():
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
                           distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
-                          schedules=args.schedules, delays=args.delays, observe=args.observe, pushes=args.pushes, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
+                          schedules=args.schedules, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
                           value=sum(n_diffuse) * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
 
