@@ -9,12 +9,14 @@ sharded over several GPUs (one process per GPU).
 from __future__ import annotations
 
 import argparse
+import collections
 import dataclasses
 import importlib
 import math
 import os
 import sys
 import time
+import types
 from typing import Any, Dict, Optional
 
 import numpy as np
@@ -400,82 +402,16 @@ class DeviceLoop:
         if any(rand) and not all(rand):
             raise RuntimeError("randomize_tasks draws per-instance commands: in a batched DeviceLoop either every "
                                "state carries randomize_target or none does")
-        if envs is not None:
-            envs = list(envs)
-            if len(envs) != B:
-                raise ValueError(f"a plan of {B} instances needs {B} envs, got {len(envs)}")
-            for env_b in envs:
-                self._check_shared(mbdpi.env, env_b)
+        settings = resolve_settings(B, mbdpi.n_ensemble, mbdpi.env, a, mbdpi.world_size, rand[0], envs=envs,
+                                    ensemble=ensemble, risk=risk, prior=prior, adapt=adapt, schedule=schedule,
+                                    delay=delay, observe=observe, pushes=pushes, plant=plant)
+        envs = [spec for spec, _ in settings["envs"]] if "envs" in settings else None
         lead = (B,) if B > 1 else ()
         key = np.ascontiguousarray(rng, dtype=np.uint32)
         if key.shape != lead + (2,):
             raise ValueError(f"rng must have shape {lead + (2,)}, got {key.shape}")
         if Y0 is not None and tuple(np.shape(Y0)) != lead + (a.Hnode + 1, mbdpi.nu):
             raise ValueError(f"Y0 must have shape {lead + (a.Hnode + 1, mbdpi.nu)}, got {tuple(np.shape(Y0))}")
-        # the ensemble settings: B of each, every one checked before anything is bound or uploaded
-        K = mbdpi.n_ensemble
-        members = []
-        if ensemble is not None:
-            self._need_ensemble("ensemble=", 1, ValueError)
-            shape = f"a list of {K} models or {B} such lists"
-            members = self._per_instance("ensemble", list(ensemble), shape,
-                                         lambda e: len(e) > 0 and all(isinstance(r, (list, tuple)) for r in e))
-            if any(len(r) != K for r in members):
-                raise ValueError(f"ensemble must be {shape}, got {[len(r) for r in members]}")
-        if risk is not None:
-            self._need_ensemble("risk=", 1, ValueError)
-            risk = self._per_instance("risk", risk, f"one risk spec or a list of {B}",
-                                      lambda r: isinstance(r, (list, tuple)))
-            for spec in risk:
-                risk_setting(spec, K)
-        for name, arg in (("adapt", adapt), ("prior", prior)):
-            if arg is not None:
-                self._need_ensemble(f"{name}=", 2, ValueError)
-        if prior is not None:
-            prior = self._per_instance("prior", list(prior), f"K weights or a list of {B} such lists",
-                                       lambda p: len(p) > 0 and all(isinstance(r, (list, tuple, np.ndarray)) for r in p))
-            for w in prior:
-                prior_setting(w, K)
-        if adapt is not None:
-            adapt = self._per_instance("adapt", adapt, f"one adapt spec or a list of {B}",
-                                       lambda s: isinstance(s, (list, tuple)))
-            for spec in adapt:
-                if spec is not None:
-                    adapt_setting(spec, K, m.nv)
-        if schedule is not None:
-            schedule = self._per_instance("schedule", schedule, f"one schedule spec or a list of {B}",
-                                          lambda s: isinstance(s, (list, tuple)))
-            for spec in schedule:
-                if spec is not None:
-                    schedule_setting(spec, a)
-        if delay is not None:
-            if mbdpi.world_size != 1:
-                raise ValueError("delay= needs an unsharded plan (world_size 1)")
-            delay = self._per_instance("delay", delay, f"one delay spec or a list of {B}",
-                                       lambda s: isinstance(s, (list, tuple)))
-            delay = [None if spec is None else delay_setting(spec) for spec in delay]
-        if observe is not None:
-            if mbdpi.world_size != 1:
-                raise ValueError("observe= needs an unsharded plan (world_size 1)")
-            observe = self._per_instance("observe", observe, f"one observe spec or a list of {B}",
-                                         lambda s: isinstance(s, (list, tuple)))
-            observe = [None if spec is None else observe_setting(spec, m) for spec in observe]
-            if rand[0] and any(o is not None and o[0] > 0 for o in observe):
-                raise ValueError(self._RAND_OBSERVE)
-        if pushes is not None:
-            if mbdpi.world_size != 1:
-                raise ValueError("pushes= needs an unsharded plan (world_size 1)")
-            # a list of B lists (or Nones) is per instance; a list of mappings is one spec for every instance
-            pushes = self._per_instance("pushes", pushes, f"one push spec or a list of {B}",
-                                        lambda s: isinstance(s, (list, tuple)) and len(s) > 0 and
-                                        all(x is None or isinstance(x, (list, tuple)) for x in s))
-            pushes = [push_setting(spec, m) for spec in pushes]
-        if plant is not None:
-            if mbdpi.world_size != 1:
-                raise ValueError("plant= needs an unsharded plan (world_size 1)")
-            plant = self._per_instance("plant", plant, f"one plant spec or a list of {B}",
-                                       lambda s: isinstance(s, (list, tuple)))
-            plant = [plant_setting(spec, m) for spec in plant]
         # each instance's DialConfig, whether it has a table of its own, and the iteration limits last
         # uploaded (None: no limits, every instance runs every iteration of a step)
         self._cfg, self._own, self._lims = [a] * B, [False] * B, None
@@ -522,51 +458,11 @@ class DeviceLoop:
             # seq-jump: the jump sequence drawn at reset is constant afterwards; one upload at bind time
             pl.set_stages(mbdpi.env.stage_tables(states[0].info))
         pl.mpc_bind(self.buf, mbdpi.M_shift.cpu().numpy())
-        # a model equal to mbdpi.env's is not uploaded: without one the plan allocates no model slots
-        base = bytes(_capi.fill_model_desc(m.model))
-        for b, env_b in enumerate(envs or ()):
-            if bytes(_capi.fill_model_desc(env_b.sys.model)) != base:
-                self.set_model(b, env_b)
-        for b, row in enumerate(members):
-            for k, member in enumerate(row):
-                if bytes(_capi.fill_model_desc(self._model(member))) != base:
-                    self.set_ensemble_model(b, k, member)
-        for b, spec in enumerate(risk or ()):
-            self.set_risk(b, spec)
-        for b, w in enumerate(prior or ()):
-            self.set_belief(b, w)
-        for b, spec in enumerate(adapt or ()):
-            if spec is not None:
-                self.set_adapt(b, spec)
-        for b, spec in enumerate(schedule or ()):
-            if spec is not None:
-                self.set_schedule(b, spec)
-        for b, d in enumerate(delay or ()):
-            if d is not None and d != (0, False):   # a loop without delays keeps the plan's launches
-                self.set_delay(b, {"steps": d[0], "predict": d[1]})
-        for b, o in enumerate(observe or ()):
-            if o is not None and self._observing(o):   # nor does a loop without observations
-                self._set_observation(b, o)
-        for b, table in enumerate(pushes or ()):
-            if table:                                   # nor does a loop without pushes
-                self.plan.set_instance_pushes(b, table)
-        for b, f in enumerate(plant or ()):
-            if f is not None:                           # nor does a loop without plant settings
-                self.plan.set_instance_plant(b, f)
-
-    @staticmethod
-    def _model(env_or_sys):
-        """The ``CompiledModel`` of an env, a ``System`` or a ``CompiledModel``."""
-        m = getattr(env_or_sys, "sys", env_or_sys)
-        return getattr(m, "model", m)
-
-    def _per_instance(self, name: str, value, shape: str, per_instance) -> list:
-        """``value`` as B values: its items when ``per_instance(value)``, else ``value`` for every instance.
-        Raises ValueError '<name> must be <shape>' when the items are not B."""
-        rows = list(value) if per_instance(value) else [value] * self.n_instances
-        if len(rows) != self.n_instances:
-            raise ValueError(f"{name} must be {shape}, got a list of {len(rows)}")
-        return rows
+        # a setting that changes nothing is not applied: the plan then allocates nothing for it and keeps its launches
+        for s in SETTINGS:
+            for b, (spec, setting) in enumerate(settings.get(s.key, ())):
+                if not s.identity(setting):
+                    s.apply(self, b, spec, setting)
 
     def _instance(self, b) -> int:
         b = int(b)
@@ -574,9 +470,9 @@ class DeviceLoop:
             raise IndexError(f"instance {b} out of range (0..{self.n_instances - 1})")
         return b
 
-    def _need_ensemble(self, what: str, k: int, exc=RuntimeError) -> None:
+    def _need_ensemble(self, what: str, k: int) -> None:
         if self.mbdpi.n_ensemble < k:
-            raise exc(f"{what} needs an MBDPI built with n_ensemble >= {k}")
+            raise RuntimeError(f"{what} needs an MBDPI built with n_ensemble >= {k}")
 
     @staticmethod
     def _check_shared(ref_env, env) -> None:
@@ -628,7 +524,7 @@ class DeviceLoop:
         b, k = self._instance(b), int(k)
         if not 0 <= k < self.mbdpi.n_ensemble:
             raise IndexError(f"member {k} out of range (0..{self.mbdpi.n_ensemble - 1})")
-        self.plan.set_ensemble_model(b, k, self._model(env_or_sys))
+        self.plan.set_ensemble_model(b, k, _model(env_or_sys))
 
     def set_risk(self, b: int, spec) -> None:
         """Instance b's risk measure over its members' rewards from the next ``step`` on (a risk spec,
@@ -909,6 +805,35 @@ def save_run(output_dir, rollout, infos, timestamp=None):
     return states, preds
 
 
+def _model(env_or_sys):
+    """The ``CompiledModel`` of an env, a ``System`` or a ``CompiledModel``."""
+    m = getattr(env_or_sys, "sys", env_or_sys)
+    return getattr(m, "model", m)
+
+
+def _mapping(spec, keys, not_mapping: str, takes: str, at: str = "") -> dict:
+    """``spec`` if it is a mapping of some of ``keys``; else ValueError '<at><not_mapping><spec>' or '<at>unknown key
+    'k' (<takes>)'."""
+    if not isinstance(spec, dict):
+        raise ValueError(f"{at}{not_mapping}{spec!r}")
+    extra = sorted(set(spec) - set(keys), key=str)
+    if extra:
+        raise ValueError(f"{at}unknown key {extra[0]!r} ({takes})")
+    return spec
+
+
+def _num(v) -> bool:
+    """A finite real number: a Python or NumPy int or float, not a bool."""
+    return not isinstance(v, bool) and isinstance(v, (int, float, np.integer, np.floating)) and math.isfinite(v)
+
+
+def _int(v, lo: int, hi: int, error: str) -> int:
+    """A Python or NumPy int (not a bool) in lo..hi; else ValueError '<error>, got <v>'."""
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+        raise ValueError(f"{error}, got {v!r}")
+    return int(v)
+
+
 RISK_AGGREGATES = ("mean", "worst", "cvar")
 
 
@@ -917,12 +842,8 @@ def risk_setting(spec, K: int):
     "mean"}``: the member mean (the default); ``{"aggregate": "worst"}``: the minimum, CVaR with alpha = 1/K;
     ``{"aggregate": "cvar", "alpha": a}``: the mean of the worst fraction a in (0, 1] of the members.
     Raises ValueError naming the bad key or value."""
-    if not isinstance(spec, dict):
-        raise ValueError(f"a risk spec maps 'aggregate' ({', '.join(RISK_AGGREGATES)}) and, for cvar, 'alpha'; "
-                         f"got {spec!r}")
-    extra = sorted(set(spec) - {"aggregate", "alpha"}, key=str)
-    if extra:
-        raise ValueError(f"unknown key {extra[0]!r} (a risk spec takes 'aggregate' and, for cvar, 'alpha')")
+    _mapping(spec, ("aggregate", "alpha"), f"a risk spec maps 'aggregate' ({', '.join(RISK_AGGREGATES)}) and, for "
+             "cvar, 'alpha'; got ", "a risk spec takes 'aggregate' and, for cvar, 'alpha'")
     agg = spec.get("aggregate")
     if agg not in RISK_AGGREGATES:
         raise ValueError(f"aggregate must be one of {', '.join(RISK_AGGREGATES)}, got {agg!r}")
@@ -934,8 +855,7 @@ def risk_setting(spec, K: int):
     if "alpha" not in spec:
         raise ValueError("aggregate cvar needs alpha, the fraction of the members it averages, in (0, 1]")
     a = spec["alpha"]
-    if isinstance(a, bool) or not isinstance(a, (int, float)) or not math.isfinite(a) or not 0 < a <= 1 \
-            or not np.float32(a) > 0:
+    if not (_num(a) and 0 < a <= 1 and np.float32(a) > 0):
         raise ValueError(f"alpha must be a finite number in (0, 1], got {a!r}")
     return cvar, float(a)
 
@@ -946,34 +866,27 @@ def adapt_setting(spec, K: int, nv: int):
     numbers, each finite and > 0; ``forget`` (default 1.0): in (0, 1], how much of the old log-belief each
     env step keeps; ``prune`` (default 0.0): in [0, 1/K), members with a smaller weight are left out of
     the score.  Raises ValueError naming the bad key or value."""
-    if not isinstance(spec, dict):
-        raise ValueError(f"an adapt spec maps 'sigma' and optionally 'forget' and 'prune'; got {spec!r}")
-    extra = sorted(set(spec) - {"sigma", "forget", "prune"}, key=str)
-    if extra:
-        raise ValueError(f"unknown key {extra[0]!r} (an adapt spec takes 'sigma', 'forget' and 'prune')")
+    _mapping(spec, ("sigma", "forget", "prune"), "an adapt spec maps 'sigma' and optionally 'forget' and 'prune'; got ",
+             "an adapt spec takes 'sigma', 'forget' and 'prune'")
     if "sigma" not in spec:
         raise ValueError("adapt needs sigma, the scale of the qvel residuals: one number or one per dof")
-
-    def num(x):
-        return not isinstance(x, bool) and isinstance(x, (int, float)) and math.isfinite(x)
-
     s = spec["sigma"]
     if isinstance(s, (list, tuple)):
         if len(s) != nv:
             raise ValueError(f"sigma must be one number or a list of {nv} (one per dof), got a list of {len(s)}")
-        bad = [x for x in s if not (num(x) and np.float32(x) > 0)]
+        bad = [x for x in s if not (_num(x) and np.float32(x) > 0)]
         if bad:
             raise ValueError(f"sigma must be finite and > 0, got {bad[0]!r}")
         sigma = np.asarray(s, np.float32)
-    elif num(s) and np.float32(s) > 0:
+    elif _num(s) and np.float32(s) > 0:
         sigma = np.full(nv, s, np.float32)
     else:
         raise ValueError(f"sigma must be a finite number > 0 or a list of {nv}, got {s!r}")
     forget = spec.get("forget", 1.0)
-    if not (num(forget) and 0 < np.float32(forget) <= 1):
+    if not (_num(forget) and 0 < np.float32(forget) <= 1):
         raise ValueError(f"forget must be a finite number in (0, 1], got {forget!r}")
     prune = spec.get("prune", 0.0)
-    if not (num(prune) and 0 <= np.float32(prune) and float(np.float32(prune)) < 1.0 / K):
+    if not (_num(prune) and 0 <= np.float32(prune) and float(np.float32(prune)) < 1.0 / K):
         raise ValueError(f"prune must be a number in [0, 1/K) = [0, {1.0 / K:g}), got {prune!r}")
     return float(forget), float(prune), sigma
 
@@ -987,8 +900,7 @@ def prior_setting(w, K: int):
     if not isinstance(w, list) or len(w) != K:
         raise ValueError(f"a belief is a list of {K} weights (one per member), got {w!r}")
     for x in w:
-        if isinstance(x, bool) or not isinstance(x, (int, float, np.floating, np.integer)) or \
-                not math.isfinite(x) or not np.float32(x) >= 0:
+        if not (_num(x) and np.float32(x) >= 0):
             raise ValueError(f"every weight must be finite and >= 0, got {x!r}")
     a = np.asarray(w, np.float32)
     if not a.astype(np.float64).sum() > 0:
@@ -1015,15 +927,14 @@ def schedule_setting(spec, args: DialConfig) -> DialConfig:
                              f"{', '.join(SCHEDULE_FIELDS)}")
         if key not in SCHEDULE_FIELDS:
             raise ValueError(f"unknown key {key!r} (a schedule takes {', '.join(SCHEDULE_FIELDS)})")
-    nmax = _capi.DEFINES["DIAL_MAXDIFFUSE"]
+    out = {}
     for key, v in spec.items():
         if key.startswith("Ndiffuse"):
-            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= nmax:
-                raise ValueError(f"{key} must be an int in 1..{nmax}, got {v!r}")
-        elif isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or \
-                not (v >= 0 if key == "sigma_scale" else (v > 0 and np.float32(v) > 0)):
+            v = _int(v, 1, _capi.DEFINES["DIAL_MAXDIFFUSE"], f"{key} must be an int in 1..{_capi.DEFINES['DIAL_MAXDIFFUSE']}")
+        elif not (_num(v) and (v >= 0 if key == "sigma_scale" else (v > 0 and np.float32(v) > 0))):
             raise ValueError(f"{key} must be a finite number {'>= 0' if key == 'sigma_scale' else '> 0'}, got {v!r}")
-    return dataclasses.replace(args, **{k: (int(v) if k.startswith("Ndiffuse") else v) for k, v in spec.items()})
+        out[key] = v
+    return dataclasses.replace(args, **out)
 
 
 def delay_setting(spec):
@@ -1031,17 +942,9 @@ def delay_setting(spec):
     step t reaches the plant at step t + d, planned from the plant state) or ``{"steps": d, "predict": p}``
     (``predict``, default False: plan from the state predicted through the d queued actions), d in 0..16.
     Raises ValueError naming the bad key or value."""
-    dmax = _capi.DEFINES["DIAL_MAXDELAY"]
-
-    def steps(v):
-        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= v <= dmax:
-            raise ValueError(f"steps must be an int in 0..{dmax}, got {v!r}")
-        return int(v)
-
+    steps = lambda v: _int(v, 0, _capi.DEFINES["DIAL_MAXDELAY"], f"steps must be an int in 0..{_capi.DEFINES['DIAL_MAXDELAY']}")
     if isinstance(spec, dict):
-        extra = sorted(set(spec) - {"steps", "predict"}, key=str)
-        if extra:
-            raise ValueError(f"unknown key {extra[0]!r} (a delay spec takes 'steps' and 'predict')")
+        _mapping(spec, ("steps", "predict"), "", "a delay spec takes 'steps' and 'predict'")
         if "steps" not in spec:
             raise ValueError("a delay spec mapping needs steps, the delay in control steps")
         p = spec.get("predict", False)
@@ -1051,6 +954,17 @@ def delay_setting(spec):
     if isinstance(spec, bool) or not isinstance(spec, (int, np.integer)):
         raise ValueError(f"a delay spec is an int (control steps) or a mapping of 'steps' and 'predict', got {spec!r}")
     return steps(spec), False
+
+
+def delay_spec(text: str) -> dict:
+    """The delay spec of a ``STEPS[:predict]`` command-line value.  Raises ValueError for any other text; the
+    steps themselves are checked by ``delay_setting``."""
+    steps, sep, mode = text.partition(":")
+    if sep and mode != "predict":
+        raise ValueError(f"the suffix must be ':predict', got {text!r}")
+    if not steps.strip().lstrip("-").isdigit():
+        raise ValueError(f"STEPS must be an int, got {steps!r}")
+    return {"steps": int(steps), "predict": bool(sep)}
 
 
 OBSERVE_KEYS = ("delay", "qpos", "qvel", "seed")
@@ -1064,24 +978,14 @@ def observe_setting(spec, sys):
     ``System.tree_replace`` resolves a dof field by joint name; a free joint takes one number or 6, 3 position
     and 3 rotation) and ``seed`` (the noise key is ``PRNGKey(seed)``, default 0: instances with other
     standard deviations see the same draws, scaled).  Raises ValueError naming the bad key or value."""
-    model = getattr(getattr(sys, "sys", sys), "model", getattr(sys, "sys", sys))
+    model = _model(sys)
     nv = model.nv
     dmax = _capi.DEFINES["DIAL_MAXDELAY"]
-    if not isinstance(spec, dict):
-        raise ValueError(f"an observe spec is a mapping of {', '.join(OBSERVE_KEYS)}, got {spec!r}")
-    extra = sorted(set(spec) - set(OBSERVE_KEYS), key=str)
-    if extra:
-        raise ValueError(f"unknown key {extra[0]!r} (an observe spec takes {', '.join(map(repr, OBSERVE_KEYS))})")
-
-    def count(name, v, hi=None):
-        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 0 or (hi is not None and v > hi):
-            raise ValueError(f"{name} must be an int in 0..{hi}, got {v!r}" if hi is not None else
-                             f"{name} must be an int >= 0, got {v!r}")
-        return int(v)
+    _mapping(spec, OBSERVE_KEYS, f"an observe spec is a mapping of {', '.join(OBSERVE_KEYS)}, got ",
+             f"an observe spec takes {', '.join(map(repr, OBSERVE_KEYS))}")
 
     def std(name, v):
-        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)) or \
-                not math.isfinite(v) or v < 0:
+        if not (_num(v) and v >= 0):
             raise ValueError(f"{name} must be a finite number >= 0, got {v!r}")
         return float(v)
 
@@ -1108,9 +1012,9 @@ def observe_setting(spec, sys):
         out[:] = std(name, S)
         return out
 
-    delay = count("delay", spec.get("delay", 0), dmax)
+    delay = _int(spec.get("delay", 0), 0, dmax, f"delay must be an int in 0..{dmax}")
     q, v = stds("qpos", spec.get("qpos", 0.0)), stds("qvel", spec.get("qvel", 0.0))
-    key = drandom.PRNGKey(count("seed", spec.get("seed", 0), 0xFFFFFFFF))
+    key = drandom.PRNGKey(_int(spec.get("seed", 0), 0, 0xFFFFFFFF, f"seed must be an int in 0..{0xFFFFFFFF}"))
     return delay, q, v, np.asarray(key, np.uint32)
 
 
@@ -1125,7 +1029,7 @@ def push_setting(spec, sys) -> list:
     in the body's frame, default its origin), ``force`` [N] and ``torque`` [N m] (world frame, default zero).
     After each env step it fires in, the plant's qvel takes the impulse of the force and torque held over that
     step.  An empty list (or None) is no pushes.  Raises ValueError naming the entry and the bad key or value."""
-    model = getattr(getattr(sys, "sys", sys), "model", getattr(sys, "sys", sys))
+    model = _model(sys)
     pmax = _capi.DEFINES["DIAL_MAXPUSH"]
     if spec is None:
         return []
@@ -1134,28 +1038,12 @@ def push_setting(spec, sys) -> list:
     if len(spec) > pmax:
         raise ValueError(f"a push spec has at most {pmax} entries, got {len(spec)}")
     bodies = model.names.get("body", [])
+    fmax = float(np.finfo(np.float32).max)
     out = []
     for i, e in enumerate(spec):
         at = f"push {i}: "
-        if not isinstance(e, dict):
-            raise ValueError(f"{at}an entry is a mapping of {', '.join(PUSH_KEYS)}, got {e!r}")
-        extra = sorted(set(e) - set(PUSH_KEYS), key=str)
-        if extra:
-            raise ValueError(f"{at}unknown key {extra[0]!r} (an entry takes {', '.join(map(repr, PUSH_KEYS))})")
-
-        def count(name, v):
-            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= 0x7FFFFFFF:
-                raise ValueError(f"{at}{name} must be an int >= 1, got {v!r}")
-            return int(v)
-
-        def vec(name, v):
-            ok = isinstance(v, (list, tuple, np.ndarray)) and len(v) == 3 and all(
-                not isinstance(x, bool) and isinstance(x, (int, float, np.integer, np.floating)) and
-                math.isfinite(x) and abs(float(x)) <= float(np.finfo(np.float32).max) for x in v)
-            if not ok:
-                raise ValueError(f"{at}{name} must be a list of 3 finite numbers, got {v!r}")
-            return [float(x) for x in v]
-
+        _mapping(e, PUSH_KEYS, f"an entry is a mapping of {', '.join(PUSH_KEYS)}, got ",
+                 f"an entry takes {', '.join(map(repr, PUSH_KEYS))}", at)
         if "step" not in e:
             raise ValueError(f"{at}needs step, the post-step counter it fires at")
         if "body" not in e:
@@ -1164,9 +1052,14 @@ def push_setting(spec, sys) -> list:
         if not isinstance(body, str) or body not in bodies[1:]:
             raise ValueError(f"{at}unknown body {body!r} (known: {bodies[1:]})")
         p = _capi.dial_push()
-        p.step, p.n_steps, p.body = count("step", e["step"]), count("steps", e.get("steps", 1)), bodies.index(body)
+        p.step, p.n_steps = (_int(e.get(k, 1), 1, 0x7FFFFFFF, f"{at}{k} must be an int >= 1") for k in ("step", "steps"))
+        p.body = bodies.index(body)
         for name in ("pos", "force", "torque"):
-            getattr(p, name)[:] = vec(name, e.get(name, [0.0, 0.0, 0.0]))
+            v = e.get(name, [0.0, 0.0, 0.0])
+            if not (isinstance(v, (list, tuple, np.ndarray)) and len(v) == 3 and
+                    all(_num(x) and abs(float(x)) <= fmax for x in v)):
+                raise ValueError(f"{at}{name} must be a list of 3 finite numbers, got {v!r}")
+            getattr(p, name)[:] = [float(x) for x in v]
         out.append(p)
     return out
 
@@ -1183,27 +1076,18 @@ def plant_setting(spec, sys):
     search iterations, 1..50) and ``tolerance`` (finite, >= 0).  The solver settings default to the model's own;
     MuJoCo's defaults are 100, 50 and 1e-8.  An empty mapping is the identity setting: the plant steps like the
     planner.  Raises ValueError naming the bad key or value."""
-    model = getattr(getattr(sys, "sys", sys), "model", getattr(sys, "sys", sys))
+    model = _model(sys)
     if spec is None:
         return None
-    if not isinstance(spec, dict):
-        raise ValueError(f"a plant spec is a mapping of {', '.join(PLANT_KEYS)}, got {spec!r}")
-    extra = sorted(set(spec) - set(PLANT_KEYS), key=str)
-    if extra:
-        raise ValueError(f"unknown key {extra[0]!r} (a plant spec takes {', '.join(map(repr, PLANT_KEYS))})")
+    _mapping(spec, PLANT_KEYS, f"a plant spec is a mapping of {', '.join(PLANT_KEYS)}, got ",
+             f"a plant spec takes {', '.join(map(repr, PLANT_KEYS))}")
     if "substeps" in spec and "sim_dt" in spec:
         raise ValueError("a plant spec takes substeps or sim_dt, not both")
-
-    def count(name, v, hi):
-        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= hi:
-            raise ValueError(f"{name} must be an int in 1..{hi}, got {v!r}")
-        return int(v)
-
     kmax = _capi.DEFINES["DIAL_MAXSUBSTEPS"]
     ts = float(model.timestep)
     if "sim_dt" in spec:
         s = spec["sim_dt"]
-        if isinstance(s, bool) or not isinstance(s, (int, float, np.integer, np.floating)) or not math.isfinite(s) or s <= 0:
+        if not (_num(s) and s > 0):
             raise ValueError(f"sim_dt must be a finite number > 0, got {s!r}")
         k = round(ts / float(s))
         if k < 1 or abs(ts / float(s) - k) > 1e-6 * k:
@@ -1211,17 +1095,126 @@ def plant_setting(spec, sys):
         if k > kmax:
             raise ValueError(f"sim_dt {s!r} gives {k} substeps of the model's timestep {ts:g}, at most {kmax}")
     else:
-        k = count("substeps", spec.get("substeps", 1), kmax)
+        k = _int(spec.get("substeps", 1), 1, kmax, f"substeps must be an int in 1..{kmax}")
     f = _capi.dial_plant()
     f.substeps = k
-    f.iterations = count("iterations", spec.get("iterations", int(model.iterations)), 100)
-    f.ls_iterations = count("ls_iterations", spec.get("ls_iterations", int(model.ls_iterations)), 50)
+    f.iterations = _int(spec.get("iterations", int(model.iterations)), 1, 100, "iterations must be an int in 1..100")
+    f.ls_iterations = _int(spec.get("ls_iterations", int(model.ls_iterations)), 1, 50,
+                           "ls_iterations must be an int in 1..50")
     tol = spec.get("tolerance", float(model.tolerance))
-    if isinstance(tol, bool) or not isinstance(tol, (int, float, np.integer, np.floating)) or not math.isfinite(tol) or \
-            tol < 0 or abs(float(tol)) > float(np.finfo(np.float32).max):
+    if not (_num(tol) and tol >= 0 and abs(float(tol)) <= float(np.finfo(np.float32).max)):
         raise ValueError(f"tolerance must be a finite number >= 0, got {tol!r}")
     f.tolerance = float(tol)
     return f
+
+
+def _each(parse):
+    """A per-spec parser as a parser of the B specs of a setting; a None spec stays None."""
+    return lambda specs, c: [None if spec is None else parse(spec, c) for spec in specs]
+
+
+def _plant_model(env, c):
+    """An instance's env, checked against the planner's: its ``sys`` when its model differs, else None."""
+    DeviceLoop._check_shared(c.env, env)
+    return env.sys if bytes(_capi.fill_model_desc(env.sys.model)) != c.base else None
+
+
+def _members(rows, c):
+    """Every instance's K members: each a ``System`` or ``CompiledModel``, None where it is the planner's model."""
+    if any(len(r) != c.K for r in rows):
+        raise ValueError(f"ensemble must be a list of {c.K} models or {c.B} such lists, got {[len(r) for r in rows]}")
+    return [[None if bytes(_capi.fill_model_desc(_model(m))) == c.base else m for m in r] for r in rows]
+
+
+def _observation(spec, c):
+    o = observe_setting(spec, c.env)
+    if c.rand and o[0] > 0:
+        raise ValueError(DeviceLoop._RAND_OBSERVE)
+    return o
+
+
+def _lists(v):
+    return isinstance(v, (list, tuple))
+
+
+_Setting = collections.namedtuple("_Setting", "key flag shape per parse identity apply ens unsharded seq",
+                                  defaults=(0, False, False))
+
+# DeviceLoop's per-instance settings in their order of application (a plant slot copies its instance's model the
+# first time it is set, the planning models copy member (b, 0)).  key: the DeviceLoop keyword; flag: the
+# command-line flag and --instance-overrides key; shape: the error for a list of other than B specs; per(value):
+# the value is B specs (else one spec for every instance; seq: list(value) first); parse(specs, c): the B
+# settings, checked; identity(setting): a setting that changes nothing, not applied at bind, so that a loop
+# without it keeps the plan's launches; apply(loop, b, spec, setting); ens: needs an ensemble of at least that
+# many members; unsharded: needs world_size 1.
+SETTINGS = (
+    _Setting("envs", None, "a plan of {B} instances needs {B} envs, got {n}", lambda v: True,
+             lambda envs, c: [_plant_model(e, c) for e in envs], lambda s: s is None,
+             lambda loop, b, spec, s: loop.set_model(b, spec), seq=True),
+    _Setting("ensemble", None, "ensemble must be a list of {K} models or {B} such lists, got a list of {n}",
+             lambda e: len(e) > 0 and all(_lists(r) for r in e), _members, lambda s: not any(m is not None for m in s),
+             lambda loop, b, spec, s: [loop.set_ensemble_model(b, k, m) for k, m in enumerate(s) if m is not None],
+             ens=1, seq=True),
+    _Setting("risk", None, "risk must be one risk spec or a list of {B}, got a list of {n}", _lists,
+             lambda specs, c: [risk_setting(spec, c.K) for spec in specs], lambda s: False,
+             lambda loop, b, spec, s: loop.set_risk(b, spec), ens=1),
+    _Setting("prior", None, "prior must be K weights or a list of {B} such lists, got a list of {n}",
+             lambda p: len(p) > 0 and all(isinstance(r, (list, tuple, np.ndarray)) for r in p),
+             lambda specs, c: [prior_setting(w, c.K) for w in specs], lambda s: False,
+             lambda loop, b, spec, s: loop.set_belief(b, s), ens=2, seq=True),
+    _Setting("adapt", None, "adapt must be one adapt spec or a list of {B}, got a list of {n}", _lists,
+             _each(lambda spec, c: adapt_setting(spec, c.K, c.nv)), lambda s: s is None,
+             lambda loop, b, spec, s: loop.set_adapt(b, spec), ens=2),
+    _Setting("schedule", None, "schedule must be one schedule spec or a list of {B}, got a list of {n}", _lists,
+             _each(lambda spec, c: schedule_setting(spec, c.cfg)), lambda s: s is None,
+             lambda loop, b, spec, s: loop.set_schedule(b, spec)),
+    _Setting("delay", "delay", "delay must be one delay spec or a list of {B}, got a list of {n}", _lists,
+             lambda specs, c: [(0, False) if spec is None else delay_setting(spec) for spec in specs],
+             lambda s: s == (0, False), lambda loop, b, spec, s: loop.set_delay(b, spec), unsharded=True),
+    _Setting("observe", "observe", "observe must be one observe spec or a list of {B}, got a list of {n}", _lists,
+             _each(_observation), lambda s: s is None or not DeviceLoop._observing(s),
+             lambda loop, b, spec, s: loop._set_observation(b, s), unsharded=True),
+    # a list of B lists (or Nones) is per instance; a list of mappings is one spec for every instance
+    _Setting("pushes", "push", "pushes must be one push spec or a list of {B}, got a list of {n}",
+             lambda v: _lists(v) and len(v) > 0 and all(x is None or _lists(x) for x in v),
+             lambda specs, c: [push_setting(spec, c.env) for spec in specs], lambda s: not s,
+             lambda loop, b, spec, s: loop.plan.set_instance_pushes(b, s), unsharded=True),
+    _Setting("plant", "plant", "plant must be one plant spec or a list of {B}, got a list of {n}", _lists,
+             lambda specs, c: [plant_setting(spec, c.env) for spec in specs], lambda s: s is None,
+             lambda loop, b, spec, s: loop.plan.set_instance_plant(b, s), unsharded=True),
+)
+
+
+def _context(B: int, K: int, env, cfg: DialConfig, rand: bool):
+    """What the parsers of ``SETTINGS`` check a spec against."""
+    return types.SimpleNamespace(B=B, K=K, env=env, nv=env.sys.nv, cfg=cfg, rand=rand,
+                                 base=bytes(_capi.fill_model_desc(_model(env))))
+
+
+def resolve_settings(B: int, K: int, env, cfg: DialConfig, world_size: int = 1, rand: bool = False, **given) -> dict:
+    """DeviceLoop's per-instance keywords (``SETTINGS``: envs, ensemble, risk, prior, adapt, schedule, delay,
+    observe, pushes, plant; None or missing: not set) for a plan of B instances and K ensemble members on ``env``'s
+    model and ``cfg``, sharded over ``world_size`` GPUs, with per-instance random tasks (``rand``) or not ->
+    ``{key: [(spec, setting)] * B}`` for every keyword given, each spec checked and parsed.  A keyword is one spec
+    for every instance or a list of B specs.  Raises ValueError naming the keyword, the spec or the value."""
+    c = _context(B, K, env, cfg, rand)
+    out = {}
+    for s in SETTINGS:
+        value = given.pop(s.key, None)
+        if value is None:
+            continue
+        if K < s.ens:
+            raise ValueError(f"{s.key}= needs an MBDPI built with n_ensemble >= {s.ens}")
+        if s.unsharded and world_size != 1:
+            raise ValueError(f"{s.key}= needs an unsharded plan (world_size 1)")
+        value = list(value) if s.seq else value
+        specs = list(value) if s.per(value) else [value] * B
+        if len(specs) != B:
+            raise ValueError(s.shape.format(B=B, K=K, n=len(specs)))
+        out[s.key] = list(zip(specs, s.parse(specs, c)))
+    if given:
+        raise TypeError(f"unknown per-instance setting {sorted(given)[0]!r}")
+    return out
 
 
 def load_setting(spec, key: str, K: int, nv: Optional[int] = None):
@@ -1279,26 +1272,21 @@ def load_ensemble(spec, env):
     return out, plant
 
 
-def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                  schedule=None, delay=None, observe=None, pushes=None, plant=None):
+def run_instances(dial_config, env, B, Nstep, **settings):
     """``B`` closed loops of ``main`` advanced by one CUDA graph per control step; instance b is the
     plain run with seed ``dial_config.seed + b`` (on ``envs[b]``, its own task and plant, when given).  With
     ``randomize_tasks`` each instance draws its own commands or jump sequence from its reset key.
-    ``ensemble``: K planning models shared by every instance (``DeviceLoop(..., ensemble=...)``), scored
-    under ``risk`` (one risk spec or B of them, ``DeviceLoop(..., risk=...)``), adapting to the plant under
-    ``adapt`` from the belief ``prior`` (``DeviceLoop(..., adapt=..., prior=...)``).  ``schedule``: B schedule
-    specs or None (``DeviceLoop(..., schedule=...)``); each instance runs its own Ndiffuse_init, then Ndiffuse.
-    ``delay``: one delay spec or B of them (``DeviceLoop(..., delay=...)``).  ``observe``: one observe spec or B
-    of them (``DeviceLoop(..., observe=...)``).  ``pushes``: one push spec or B of them
-    (``DeviceLoop(..., pushes=...)``).  ``plant``: one plant spec or B of them (``DeviceLoop(..., plant=...)``)."""
-    mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(ensemble) if ensemble else 0)
+    ``settings``: DeviceLoop's per-instance keywords (``envs``, ``ensemble``, ``risk``, ``prior``, ``adapt``,
+    ``schedule``, ``delay``, ``observe``, ``pushes``, ``plant``); with ``ensemble``, K planning models shared by
+    every instance; each instance runs its own Ndiffuse_init, then Ndiffuse."""
+    envs = settings.get("envs")
+    mbdpi = MBDPI(dial_config, env, n_instances=B, n_ensemble=len(settings.get("ensemble") or ()))
     states, rngs = [], []
     for b in range(B):
         rng, rng_reset = drandom.split(drandom.PRNGKey(seed=dial_config.seed + b))
         states.append((envs[b] if envs is not None else env).reset(rng_reset))
         rngs.append(drandom.split(rng)[1])
-    loop = DeviceLoop(mbdpi, states, np.stack(rngs), envs=envs, ensemble=ensemble, risk=risk, adapt=adapt, prior=prior,
-                      schedule=schedule, delay=delay, observe=observe, pushes=pushes, plant=plant)
+    loop = DeviceLoop(mbdpi, states, np.stack(rngs), **settings)
     buf = loop.buf
     rews, rollout, infos = [], [], []
     t0, tlast = time.time(), -1
@@ -1321,11 +1309,14 @@ def run_instances(dial_config, env, B, Nstep, envs=None, ensemble=None, risk=Non
         save_run(dial_config.output_dir, [r[b] for r in rollout], [x[b] for x in infos], timestamp=f"{timestamp}_inst{b}")
 
 
-def _delay_specs(delay):
-    """(steps, predict), or a list of them, as delay specs for ``DeviceLoop(..., delay=...)``."""
-    if isinstance(delay, list):
-        return [{"steps": d, "predict": p} for d, p in delay]
-    return {"steps": delay[0], "predict": delay[1]}
+def _spec_from_text(flag: str, text: str):
+    """The spec of a per-instance setting's command-line value: ``STEPS[:predict]`` for --delay, YAML otherwise."""
+    if flag == "delay":
+        return delay_spec(text)
+    try:
+        return yaml.safe_load(text)
+    except yaml.YAMLError as e:
+        raise ValueError(f"not a YAML {'list' if flag == 'push' else 'mapping'}: {e}") from None
 
 
 def _print_belief(loop) -> None:
@@ -1409,64 +1400,30 @@ def main():
         parser.error("--instances must be at least 1")
     if args.instances > 1 and args.eager:
         parser.error("--instances runs on the CUDA-graph loop; it excludes --eager")
-    delay = None
-    if args.delay is not None:
+    flagged = [s for s in SETTINGS if s.flag]
+    given = {s.key: None for s in flagged}     # DeviceLoop keyword -> the spec of its flag
+    for s in flagged:
+        text = getattr(args, s.flag)
+        if text is None:
+            continue
         if args.eager:
-            parser.error("--delay runs on the CUDA-graph loop; it excludes --eager")
-        steps, sep, mode = args.delay.partition(":")
+            parser.error(f"--{s.flag} runs on the CUDA-graph loop; it excludes --eager")
         try:
-            if sep and mode != "predict":
-                raise ValueError(f"the suffix must be ':predict', got {args.delay!r}")
-            if not steps.strip().lstrip("-").isdigit():
-                raise ValueError(f"STEPS must be an int, got {steps!r}")
-            delay = delay_setting({"steps": int(steps), "predict": bool(sep)})
+            given[s.key] = _spec_from_text(s.flag, text)
         except ValueError as e:
-            parser.error(f"--delay: {e}")
-    observe = None
-    if args.observe is not None:
-        if args.eager:
-            parser.error("--observe runs on the CUDA-graph loop; it excludes --eager")
-        try:
-            observe = yaml.safe_load(args.observe)
-        except yaml.YAMLError as e:
-            parser.error(f"--observe: not a YAML mapping: {e}")
-    push = None
-    if args.push is not None:
-        if args.eager:
-            parser.error("--push runs on the CUDA-graph loop; it excludes --eager")
-        try:
-            push = yaml.safe_load(args.push)
-        except yaml.YAMLError as e:
-            parser.error(f"--push: not a YAML list: {e}")
-    fidelity = None
-    if args.plant is not None:
-        if args.eager:
-            parser.error("--plant runs on the CUDA-graph loop; it excludes --eager")
-        try:
-            fidelity = yaml.safe_load(args.plant)
-        except yaml.YAMLError as e:
-            parser.error(f"--plant: not a YAML mapping: {e}")
+            parser.error(f"--{s.flag}: {e}")
     rng = drandom.PRNGKey(seed=dial_config.seed)
     env_config_type = dial_envs.get_config(dial_config.env_name)
     env_config = load_dataclass_from_dict(env_config_type, config_dict, convert_list_to_array=True)
     env = dial_envs.get_environment(dial_config.env_name, config=env_config)
-    if observe is not None:
-        try:
-            observe_setting(observe, env.sys)
-            if observe.get("delay", 0) > 0 and getattr(env_config, "randomize_tasks", False):
-                raise ValueError(DeviceLoop._RAND_OBSERVE)
-        except ValueError as e:
-            parser.error(f"--observe: {e}")
-    if push is not None:
-        try:
-            push_setting(push, env.sys)
-        except ValueError as e:
-            parser.error(f"--push: {e}")
-    if fidelity is not None:
-        try:
-            plant_setting(fidelity, env.sys)
-        except ValueError as e:
-            parser.error(f"--plant: {e}")
+    # a flag or an override key holds one spec: it is checked by the setting's parser, not split into B
+    ctx = _context(args.instances, 0, env, dial_config, bool(getattr(env_config, "randomize_tasks", False)))
+    for s in flagged:
+        if given[s.key] is not None:
+            try:
+                s.parse([given[s.key]], ctx)
+            except ValueError as e:
+                parser.error(f"--{s.flag}: {e}")
     envs = None
     members, plant, risk, adapt, prior = None, None, None, None, None
     if args.ensemble is not None:
@@ -1495,10 +1452,7 @@ def main():
         settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
         uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
         schedule = [None] * args.instances
-        delays = [delay] * args.instances
-        observes = [observe] * args.instances
-        pushes = [push] * args.instances
-        fidelities = [fidelity] * args.instances
+        per = {s.key: [given[s.key]] * args.instances for s in flagged}
         for b, ov in enumerate(overrides):
             ov = ov or {}
             if not isinstance(ov, dict) or set(ov) - known:
@@ -1514,35 +1468,14 @@ def main():
                     parser.error(f"--instance-overrides entry {b}: {e}")
                 schedule[b] = spec
             sys_ov = ov.pop("sys", None)
-            if ov.get("delay") is not None:
-                try:
-                    delays[b] = delay_setting(ov["delay"])
-                except ValueError as e:
-                    parser.error(f"--instance-overrides entry {b}: delay: {e}")
-            ov.pop("delay", None)
-            if ov.get("observe") is not None:
-                try:
-                    observe_setting(ov["observe"], env.sys)
-                    if ov["observe"].get("delay", 0) > 0 and getattr(env_config, "randomize_tasks", False):
-                        raise ValueError(DeviceLoop._RAND_OBSERVE)
-                except ValueError as e:
-                    parser.error(f"--instance-overrides entry {b}: observe: {e}")
-                observes[b] = ov["observe"]
-            ov.pop("observe", None)
-            if ov.get("push") is not None:
-                try:
-                    push_setting(ov["push"], env.sys)
-                except ValueError as e:
-                    parser.error(f"--instance-overrides entry {b}: push: {e}")
-                pushes[b] = ov["push"]
-            ov.pop("push", None)
-            if ov.get("plant") is not None:
-                try:
-                    plant_setting(ov["plant"], env.sys)
-                except ValueError as e:
-                    parser.error(f"--instance-overrides entry {b}: plant: {e}")
-                fidelities[b] = ov["plant"]
-            ov.pop("plant", None)
+            for s in flagged:
+                spec = ov.pop(s.flag, None)
+                if spec is not None:
+                    try:
+                        s.parse([spec], ctx)
+                    except ValueError as e:
+                        parser.error(f"--instance-overrides entry {b}: {s.flag}: {e}")
+                    per[s.key][b] = spec
             for key in ("risk", "adapt"):
                 if ov.get(key) is not None:
                     if members is None:
@@ -1577,19 +1510,12 @@ def main():
             risk = [r or {"aggregate": "mean"} for r in settings["risk"]]
         if args.instance_overrides is not None and any(a is not None for a in settings["adapt"]):
             adapt = settings["adapt"]
-        if args.instance_overrides is not None and any(d is not None for d in delays):
-            delay = [d or (0, False) for d in delays]
-        if args.instance_overrides is not None and any(o is not None for o in observes):
-            observe = observes
-        if args.instance_overrides is not None and any(q is not None for q in pushes):
-            push = pushes
-        if args.instance_overrides is not None and any(f is not None for f in fidelities):
-            fidelity = fidelities
+        for key, specs in (per.items() if args.instance_overrides is not None else ()):
+            if any(spec is not None for spec in specs):
+                given[key] = specs
         run_instances(dial_config, env, args.instances, args.n_steps or dial_config.n_steps, envs=envs,
                       ensemble=members, risk=risk, adapt=adapt, prior=prior,
-                      schedule=schedule if args.instance_overrides is not None and any(schedule) else None,
-                      delay=None if delay is None else _delay_specs(delay), observe=observe, pushes=push,
-                      plant=fidelity)
+                      schedule=schedule if args.instance_overrides is not None and any(schedule) else None, **given)
         return
     mbdpi = MBDPI(dial_config, env, n_ensemble=len(members) if members else 0)
     rng, rng_reset = drandom.split(rng)
@@ -1598,19 +1524,10 @@ def main():
     rng_exp, rng = drandom.split(rng)
     Nstep = args.n_steps or dial_config.n_steps
     rews, rollout, infos = [], [], []
-    if delay is not None and mbdpi.world_size != 1:
-        parser.error("--delay needs an unsharded plan (one process)")
-    if observe is not None and mbdpi.world_size != 1:
-        parser.error("--observe needs an unsharded plan (one process)")
-    if push is not None and mbdpi.world_size != 1:
-        parser.error("--push needs an unsharded plan (one process)")
-    if fidelity is not None and mbdpi.world_size != 1:
-        parser.error("--plant needs an unsharded plan (one process)")
-    if mbdpi.world_size == 1 and not args.eager:
+    if not args.eager:
         # one CUDA graph per control step; the host launches it and logs
         loop = DeviceLoop(mbdpi, state, rng, Y0, envs=[plant_env] if members else None, ensemble=members, risk=risk,
-                          adapt=adapt, prior=prior, delay=None if delay is None else _delay_specs(delay),
-                          observe=observe, pushes=push, plant=fidelity)
+                          adapt=adapt, prior=prior, **given)
         b = loop.buf
         t0, tlast = time.time(), -1
         for t in range(Nstep):
@@ -1639,7 +1556,7 @@ def main():
                 print(f"step {t}: rew={float(state.reward):.3e} freq={freq:.1f} Hz")
     rew = torch.stack([torch.as_tensor(r) for r in rews]).mean()
     print(f"mean reward = {float(rew):.2e}")
-    if mbdpi.world_size == 1 and not args.eager:
+    if not args.eager:
         _print_belief(loop)
     save_run(dial_config.output_dir, rollout, infos)
 

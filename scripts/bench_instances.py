@@ -16,8 +16,9 @@ feet ``FR FL RR RL``, else every pair's friction scaled so; a per-instance model
 (dial_plan_desc.n_ens) spread as ``--distinct-models`` spreads the instances (member k: base mass
 +3 kg * k / K, friction 1 - 0.5 k / K), bound through ``dial_plan_set_ensemble_model``, and scores each
 sample by the ``--risk`` measure of its member rewards (mean, worst or cvar:ALPHA; default mean).
-``--delays FILE.yaml``: a YAML list of one delay spec per instance (``DeviceLoop(..., delay=...)``: an int or
-``{steps: d, predict: true}``), so that the step also moves the action queues and, for predicting instances,
+``--schedules``, ``--delays``, ``--observe``, ``--pushes`` and ``--plant`` each take one spec for every instance or
+a list of one per instance (null: none), as YAML text or a YAML file.
+``--delays SPEC_OR_FILE``: delay specs (``DeviceLoop(..., delay=...)``: an int or ``{steps: d, predict: true}``), so that the step also moves the action queues and, for predicting instances,
 runs the prediction launches (use ``--env-step 1`` for the queues to move).
 ``--observe SPEC_OR_FILE``: each instance plans from an observation of its plant (``DeviceLoop(..., observe=...)``):
 a YAML flow mapping applied to every instance (``'{delay: 2, qpos: 0.01, qvel: 0.1}'``) or a YAML file holding
@@ -94,11 +95,11 @@ def main():
                     help="the timed steps' env_step: 2 (shift + plan, the default) or 1 (env step + shift + plan; "
                          "--adapt runs its predictions and belief update in env steps only)")
     ap.add_argument("--schedules", default=None, metavar="FILE.yaml",
-                    help="a YAML list of one schedule spec per instance (null: the config's; DeviceLoop(..., "
-                         "schedule=...)); each instance then runs its own Ndiffuse")
+                    help="a schedule spec for every instance or a list of one per instance (null: the config's; "
+                         "DeviceLoop(..., schedule=...)); each instance then runs its own Ndiffuse")
     ap.add_argument("--delays", default=None, metavar="FILE.yaml",
-                    help="a YAML list of one delay spec per instance (an int or {steps: d, predict: true}; "
-                         "DeviceLoop(..., delay=...))")
+                    help="a delay spec for every instance or a list of one per instance (an int or "
+                         "{steps: d, predict: true}; DeviceLoop(..., delay=...))")
     ap.add_argument("--observe", default=None, metavar="SPEC_OR_FILE",
                     help="an observe spec for every instance (a YAML flow mapping such as '{delay: 2, qpos: 0.01}') or "
                          "a YAML file with one spec or a list of one per instance (DeviceLoop(..., observe=...))")
@@ -124,8 +125,7 @@ def main():
     import torch
     from baseline_configs import BASELINE, dial_config, product_env
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import (MBDPI, DeviceLoop, delay_setting, observe_setting, plant_setting,
-                                              push_setting, schedule_setting)
+    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, resolve_settings
 
     B, b = args.instances, BASELINE[args.config]
     cfg = dial_config(args.config, world=1)
@@ -163,72 +163,35 @@ def main():
         adapt = adapt_spec(args.adapt) if args.adapt is not None else None
     except ValueError as e:
         ap.error(f"--adapt {args.adapt}: {e}")
-    schedule, n_diffuse = None, [cfg.Ndiffuse] * B
-    if args.schedules is not None:
-        import yaml
-        schedule = yaml.safe_load(open(args.schedules))
-        if not isinstance(schedule, list) or len(schedule) != B:
-            ap.error(f"--schedules must hold a list of {B} schedule specs (one per instance)")
-        try:
-            n_diffuse = [schedule_setting(s or {}, cfg).Ndiffuse for s in schedule]
-        except ValueError as e:
-            ap.error(f"--schedules {args.schedules}: {e}")
-    delay, n_pred, settings = None, 0, [(0, False)] * B
-    if args.delays is not None:
-        import yaml
-        delay = yaml.safe_load(open(args.delays))
-        if not isinstance(delay, list) or len(delay) != B:
-            ap.error(f"--delays must hold a list of {B} delay specs (one per instance)")
-        try:
-            settings = [delay_setting(0 if s is None else s) for s in delay]
-        except ValueError as e:
-            ap.error(f"--delays {args.delays}: {e}")
-        delay = [{"steps": d, "predict": p} for d, p in settings]
-        n_pred = max([d for d, p in settings if p] or [0])
-    observe = None
-    if args.observe is not None:
-        import yaml
-        try:
-            observe = yaml.safe_load(open(args.observe) if os.path.isfile(args.observe) else args.observe)
-            if isinstance(observe, list) and len(observe) != B:
-                raise ValueError(f"a list of observe specs needs {B} entries (one per instance), got {len(observe)}")
-            specs = observe if isinstance(observe, list) else [observe] * B
-            ks = [0 if o is None else observe_setting(o, env.sys)[0] for o in specs]
-        except (ValueError, yaml.YAMLError) as e:
-            ap.error(f"--observe {args.observe}: {e}")
-        # with the observe launch the prediction also runs through each predicting instance's observation delay
-        n_pred = max([d + k for (d, p), k in zip(settings, ks) if p] or [0])
-    pushes = None
-    if args.pushes is not None:
-        import yaml
-        try:
-            pushes = yaml.safe_load(open(args.pushes))
-            per = isinstance(pushes, list) and len(pushes) > 0 and all(x is None or isinstance(x, list) for x in pushes)
-            if per and len(pushes) != B:
-                raise ValueError(f"a list of push specs needs {B} entries (one per instance), got {len(pushes)}")
-            for spec in pushes if per else [pushes]:
-                push_setting(spec, env.sys)
-        except (ValueError, yaml.YAMLError) as e:
-            ap.error(f"--pushes {args.pushes}: {e}")
-    plant = None
-    if args.plant is not None:
-        import yaml
-        try:
-            plant = yaml.safe_load(open(args.plant)) if os.path.exists(args.plant) else yaml.safe_load(args.plant)
-            for spec in plant if isinstance(plant, list) else [plant]:
-                plant_setting(spec, env.sys)
-        except (ValueError, yaml.YAMLError) as e:
-            ap.error(f"--plant {args.plant}: {e}")
+    import yaml
+    # each per-instance setting is one spec for every instance or a list of B (DeviceLoop's rule), given as YAML text
+    # or a YAML file
+    given, settings = {}, {}
+    for key, opt, text in (("schedule", "--schedules", args.schedules), ("delay", "--delays", args.delays),
+                           ("observe", "--observe", args.observe), ("pushes", "--pushes", args.pushes),
+                           ("plant", "--plant", args.plant)):
+        if text is not None:
+            try:
+                given[key] = yaml.safe_load(open(text) if os.path.isfile(text) else text)
+                settings.update(resolve_settings(B, args.ensemble, env, cfg, **{key: given[key]}))
+            except (ValueError, yaml.YAMLError) as e:
+                ap.error(f"{opt} {text}: {e}")
+    setting = lambda key, none: [s for _, s in settings.get(key, [(None, none)] * B)]
+    n_diffuse = [cfg.Ndiffuse if s is None else s.Ndiffuse for s in setting("schedule", None)]
+    # a predicting instance's prediction runs through its observation delay and its control latency
+    n_pred = max([d + (o[0] if o else 0) for (d, p), o in zip(setting("delay", (0, False)), setting("observe", None))
+                  if p] or [0])
+    # with plant settings the env step is one launch per distinct substep count
+    n_plant = len({1 if f is None else f.substeps for f in setting("plant", None)})
     if B == 1:
         loop = DeviceLoop(mb, state, drandom.PRNGKey(cfg.seed), envs=envs, ensemble=members, risk=risk, adapt=adapt,
-                          schedule=schedule, delay=delay, observe=observe, pushes=pushes, plant=plant)
+                          **given)
     else:
         loop = DeviceLoop(mb, [state] * B, np.stack([drandom.PRNGKey(cfg.seed + i) for i in range(B)]), envs=envs,
-                          ensemble=members, risk=risk, adapt=adapt, schedule=schedule, delay=delay, observe=observe,
-                          pushes=pushes, plant=plant)
+                          ensemble=members, risk=risk, adapt=adapt, **given)
     es = args.env_step
     # without --schedules every step runs the config's Ndiffuse on every instance, as before
-    nd = None if schedule is not None else cfg.Ndiffuse
+    nd = None if "schedule" in given else cfg.Ndiffuse
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=mb.device)
     for _ in range(max(args.warmup, 3)):
         loop.step(nd, env_step=es)
@@ -252,9 +215,6 @@ def main():
                     acc[key] = (n + 1, tot + ev.time_range.elapsed_us())
         # the rollout launches of one step in order: [member prediction, env step (env_step 1)], [the delay
         # prediction steps], the planner's
-        # with plant settings the env step is one launch per distinct substep count
-        specs = (plant if isinstance(plant, list) else [plant] * B) if plant is not None else []
-        n_plant = len({plant_setting(sp, env.sys).substeps if sp is not None else 1 for sp in specs}) if specs else 1
         per_step = ["prediction"] * (es == 1 and adapt is not None) + ["env step"] * (es == 1) * n_plant + \
             ["delay prediction"] * n_pred + ["plan"] * max(n_diffuse)
         for i, (_, us) in enumerate(sorted(rollouts)):
@@ -279,7 +239,7 @@ def main():
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
                           distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
-                          schedules=args.schedules, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, Ndiffuse_per_instance=n_diffuse if schedule is not None else None,
+                          schedules=args.schedules, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, Ndiffuse_per_instance=n_diffuse if "schedule" in given else None,
                           value=sum(n_diffuse) * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
 

@@ -56,12 +56,14 @@ def main():
     import torch
     import yaml
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, load_ensemble, load_setting
+    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, delay_spec, load_ensemble, load_setting
 
     delay = None
     if args.delay is not None:
-        steps, _, mode = args.delay.partition(":")
-        delay = {"steps": int(steps), "predict": mode == "predict"}
+        try:
+            delay = delay_spec(args.delay)
+        except ValueError as e:
+            ap.error(f"--delay: {e}")
     push = yaml.safe_load(args.push) if args.push is not None else None
     B = len(PLANTS)
     results = []

@@ -41,7 +41,7 @@ def main():
     import yaml
     from baseline_configs import BASELINE, dial_config, product_env
     from dial_mpc_b200 import random as drandom
-    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, load_ensemble, load_setting
+    from dial_mpc_b200.core.dial_core import MBDPI, DeviceLoop, delay_spec, load_ensemble, load_setting
 
     cfg = dial_config(0, world=1)
     if args.seed is not None:
@@ -49,8 +49,10 @@ def main():
     env = product_env(BASELINE[0]["env"])
     delay = None
     if args.delay is not None:
-        steps, _, mode = args.delay.partition(":")
-        delay = {"steps": int(steps), "predict": mode == "predict"}
+        try:
+            delay = delay_spec(args.delay)
+        except ValueError as e:
+            ap.error(f"--delay: {e}")
     members, plant, kw = None, None, {}
     if args.ensemble is not None:
         spec = yaml.safe_load(open(args.ensemble))
