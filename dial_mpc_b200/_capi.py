@@ -69,6 +69,7 @@ dial_mpc_buffers = _mk("dial_mpc_buffers")
 dial_task = _mk("dial_task")
 dial_push = _mk("dial_push")
 dial_plant = _mk("dial_plant")
+dial_terrain = _mk("dial_terrain")
 
 TASK_FIELDS = tuple(name for name, _ in _STRUCTS["dial_task"])
 # the plan descriptor's task block has the layout of dial_task (a plan's own task is read through it)
@@ -272,13 +273,16 @@ def _bind(path: str) -> C.CDLL:
     lib.dial_plan_set_instance_pushes.restype = C.c_int
     lib.dial_plan_set_instance_plant.argtypes = [V, I, C.POINTER(dial_plant), V]
     lib.dial_plan_set_instance_plant.restype = C.c_int
+    lib.dial_plan_set_instance_terrain.argtypes = [V, I, I, C.POINTER(dial_terrain), V]
+    lib.dial_plan_set_instance_terrain.restype = C.c_int
     for fn in ("dial_rollout", "dial_env_step", "dial_env_step_kin", "dial_plan_set_command", "dial_plan_set_stages", "dial_pipeline_init", "dial_reverse_rollout",
                "dial_reverse_update", "dial_reverse_update_x", "dial_reverse_update_fused", "dial_reverse_trajbar",
                "dial_reverse_trajectories", "dial_exchange_create", "dial_exchange_connect", "dial_exchange_status"):
         getattr(lib, fn).restype = C.c_int
     if lib.dial_abi_version() != DEFINES["DIAL_ABI_VERSION"]:
         raise RuntimeError(f"{os.path.basename(path)} ABI version does not match include/dial_b200.h")
-    for i, t in enumerate((dial_model_desc, dial_plan_desc, dial_state, dial_mpc_buffers, dial_task, dial_push, dial_plant)):
+    for i, t in enumerate((dial_model_desc, dial_plan_desc, dial_state, dial_mpc_buffers, dial_task, dial_push, dial_plant,
+                              dial_terrain)):
         if lib.dial_sizeof(i) != C.sizeof(t):
             raise RuntimeError(f"struct layout mismatch for {t.__name__}: C {lib.dial_sizeof(i)} vs ctypes {C.sizeof(t)}")
     return lib
@@ -311,4 +315,4 @@ EXPORTS = ["dial_abi_version", "dial_last_error", "dial_sizeof", "dial_plan_crea
            "dial_plan_set_ensemble_belief", "dial_plan_ensemble_belief", "dial_plan_set_instance_schedule",
            "dial_plan_set_instance_iterations", "dial_plan_set_instance_delay", "dial_plan_pending_actions",
            "dial_plan_planning_state", "dial_plan_set_instance_observation", "dial_plan_observed_state",
-           "dial_plan_set_instance_pushes", "dial_plan_set_instance_plant"]
+           "dial_plan_set_instance_pushes", "dial_plan_set_instance_plant", "dial_plan_set_instance_terrain"]

@@ -28,6 +28,7 @@ from dial_mpc_b200 import _capi
 from dial_mpc_b200 import random as drandom
 from dial_mpc_b200.core.dial_config import DialConfig
 from dial_mpc_b200.plan import Plan
+from dial_mpc_b200.terrain import PLANNER as TERRAIN_PLANNER, PLANT as TERRAIN_PLANT, terrain_setting, terrains
 from dial_mpc_b200.utils.io_utils import get_example_path, load_dataclass_from_dict
 from dial_mpc_b200.utils.spline import interp_matrix
 
@@ -317,7 +318,7 @@ class DeviceLoop:
 
     def __init__(self, mbdpi: "MBDPI", state, rng, Y0=None, n_diffuse_max: Optional[int] = None,
                  compute_bars: bool = True, noise=None, envs=None, ensemble=None, risk=None, adapt=None, prior=None,
-                 schedule=None, delay=None, observe=None, pushes=None, plant=None):
+                 schedule=None, delay=None, observe=None, pushes=None, plant=None, terrain=None):
         """``noise`` [>= n_diffuse_max, Hnode+1]: annealing schedule, default ``mbdpi.schedule`` (the
         deploy planner passes its own, dial_plan.py:199-209).
 
@@ -384,7 +385,13 @@ class DeviceLoop:
         ``ls_iterations`` and ``tolerance``, each defaulting to the planner's own).  With a spec, the instance's
         env step makes substeps x n_frames physics steps of timestep / substeps on its plant model with those
         solver settings, the control held across them; the planner, the members and the predictions keep the
-        plan's discretisation (``set_plant``)."""
+        plan's discretisation (``set_plant``).
+
+        ``terrain``: each instance's ground, one terrain spec for every instance or a list of B specs (or Nones) or
+        None (``terrain.terrain_setting``: ``{"kind": "rough", "amplitude": a, "wavelength": w, "seed": s}``,
+        ``{"kind": "slope", "angle": deg}`` or ``{"kind": "grid", "heights": ..., "spacing": s}``, with
+        ``"planner": True`` for a planner that plans on the same ground).  The heightfield replaces the floor
+        plane in the instance's env steps, and the built-in rewards measure heights above it (``set_terrain``)."""
         if mbdpi.world_size != 1 and not mbdpi.xch:
             raise RuntimeError("DeviceLoop on a sharded plan needs the peer-memory exchange (dial_exchange_*); "
                                f"it is off: {mbdpi.xch_error or 'DIAL_EXCHANGE=nccl'}")
@@ -404,7 +411,7 @@ class DeviceLoop:
                                "state carries randomize_target or none does")
         settings = resolve_settings(B, mbdpi.n_ensemble, mbdpi.env, a, mbdpi.world_size, rand[0], envs=envs,
                                     ensemble=ensemble, risk=risk, prior=prior, adapt=adapt, schedule=schedule,
-                                    delay=delay, observe=observe, pushes=pushes, plant=plant)
+                                    delay=delay, observe=observe, pushes=pushes, plant=plant, terrain=terrain)
         envs = [spec for spec, _ in settings["envs"]] if "envs" in settings else None
         lead = (B,) if B > 1 else ()
         key = np.ascontiguousarray(rng, dtype=np.uint32)
@@ -643,6 +650,13 @@ class DeviceLoop:
         loop, and any later one that changes the set of distinct substep counts in use, changes the launch
         sequence: the next steps capture their graphs again.  Other calls keep them."""
         self.plan.set_instance_plant(self._instance(b), plant_setting(spec, self.mbdpi.env.sys))
+
+    def set_terrain(self, b: int, spec) -> None:
+        """Instance b's terrain from the next ``step`` on (a terrain spec, ``terrain.terrain_setting``; None: the
+        flat floor on both sides).  Stream-ordered on the current stream.  The first terrain on a side, and a grid
+        larger than the instance's earlier ones, change the launch sequence: the next steps capture their graphs
+        again.  Other calls keep them."""
+        _set_terrain(self, self._instance(b), None if spec is None else terrain_setting(spec, self.mbdpi.env.sys))
 
     def observed_state(self) -> Dict[str, torch.Tensor]:
         """The observation the last step planned from, before any prediction: new tensors ``qpos``, ``qvel``,
@@ -1108,6 +1122,13 @@ def plant_setting(spec, sys):
     return f
 
 
+def _set_terrain(loop, b, setting):
+    """Instance b's plant and planner terrains from a ``TerrainSetting`` (None: flat on both sides)."""
+    plant, planner = terrains(setting)
+    loop.plan.set_instance_terrain(b, TERRAIN_PLANT, plant)
+    loop.plan.set_instance_terrain(b, TERRAIN_PLANNER, planner)
+
+
 def _each(parse):
     """A per-spec parser as a parser of the B specs of a setting; a None spec stays None."""
     return lambda specs, c: [None if spec is None else parse(spec, c) for spec in specs]
@@ -1182,6 +1203,9 @@ SETTINGS = (
     _Setting("plant", "plant", "plant must be one plant spec or a list of {B}, got a list of {n}", _lists,
              lambda specs, c: [plant_setting(spec, c.env) for spec in specs], lambda s: s is None,
              lambda loop, b, spec, s: loop.plan.set_instance_plant(b, s), unsharded=True),
+    _Setting("terrain", "terrain", "terrain must be one terrain spec or a list of {B}, got a list of {n}", _lists,
+             _each(lambda spec, c: terrain_setting(spec, c.env.sys)), lambda s: s is None,
+             lambda loop, b, spec, s: _set_terrain(loop, b, s), unsharded=True),
 )
 
 
@@ -1193,7 +1217,7 @@ def _context(B: int, K: int, env, cfg: DialConfig, rand: bool):
 
 def resolve_settings(B: int, K: int, env, cfg: DialConfig, world_size: int = 1, rand: bool = False, **given) -> dict:
     """DeviceLoop's per-instance keywords (``SETTINGS``: envs, ensemble, risk, prior, adapt, schedule, delay,
-    observe, pushes, plant; None or missing: not set) for a plan of B instances and K ensemble members on ``env``'s
+    observe, pushes, plant, terrain; None or missing: not set) for a plan of B instances and K ensemble members on ``env``'s
     model and ``cfg``, sharded over ``world_size`` GPUs, with per-instance random tasks (``rand``) or not ->
     ``{key: [(spec, setting)] * B}`` for every keyword given, each spec checked and parsed.  A keyword is one spec
     for every instance or a list of B specs.  Raises ValueError naming the keyword, the spec or the value."""
@@ -1381,6 +1405,12 @@ def main():
                              "planner physics step with the control held, solved with the given settings (default: "
                              "the planner's); the planner keeps its model; an --instance-overrides mapping may carry "
                              "its own 'plant'")
+    parser.add_argument("--terrain", type=str, default=None, metavar="SPEC",
+                        help="give every instance's simulated robot its own ground: a YAML flow mapping such as "
+                             "'{kind: rough, amplitude: 0.03, wavelength: 0.3, seed: 1}', '{kind: slope, angle: 10}' "
+                             "or '{kind: grid, heights: ground.npy, spacing: 0.05}'; 'planner: true' lets the planner "
+                             "plan on the same ground (default: it plans on the flat floor); an --instance-overrides "
+                             "mapping may carry its own 'terrain'")
     args = parser.parse_args()
     from dial_mpc_b200.examples import examples
     if args.list_examples:
@@ -1447,7 +1477,7 @@ def main():
         # DialConfig fields: the sampling schedule (SCHEDULE_FIELDS), or fields shared by the plan, which
         # schedule_setting rejects by name
         dial_fields = {f.name for f in dataclasses.fields(DialConfig)} - env_fields
-        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay", "observe", "push", "plant"}
+        known = env_fields | dial_fields | {"sys", "risk", "adapt", "delay", "observe", "push", "plant", "terrain"}
         envs = []
         settings = {"risk": [risk] * args.instances, "adapt": [adapt] * args.instances}
         uses = {"risk": "it scores the members' rewards", "adapt": "it weights the members"}
@@ -1505,6 +1535,8 @@ def main():
         plant_env.sys = env.sys.tree_replace(plant)
         if args.instances > 1:
             envs = [plant_env] * args.instances
+    if given["terrain"] is None:
+        del given["terrain"]   # (passed only when some instance has a terrain)
     if args.instances > 1:
         if args.instance_overrides is not None and any(r is not None for r in settings["risk"]):
             risk = [r or {"aggregate": "mean"} for r in settings["risk"]]

@@ -48,6 +48,11 @@ DEV bool cta_sync_or(bool p) { return __syncthreads_or(p) != 0; }
 DEV void fast_sincos(float x, float& s, float& c) { __sincosf(x, &s, &c); }
 DEV float fast_cos(float x) { return __cosf(x); }
 #endif
+#ifdef DIAL_HOST_EMUL
+inline float ldg(const float* p) { return *p; }
+#else
+DEV float ldg(const float* p) { return __ldg(p); }   // the read-only data path
+#endif
 
 // TEST-ONLY (emulator build with -DDIAL_EMUL_TRACE): iteration counts of the solvers
 #if defined(DIAL_HOST_EMUL) && defined(DIAL_EMUL_TRACE)
@@ -188,6 +193,41 @@ DEV int delay_queue_step(float* ring, int head, int d, int nu, const float* y0, 
   return h1;
 }
 
+// One instance's terrain on one side (dial_plan_set_instance_terrain, include/dial_b200.h): nx == 0 is the flat
+// floor.  `inv` = 1 / spacing; h [ny][nx] is plan-owned device memory.
+struct alignas(16) DevTerrain {
+  int32_t nx, ny;
+  float x0, y0, inv, pad_;
+  const float* h;
+};
+
+// The plane of the terrain's surface under (x, y): returns its height H(x, y) there and the slopes (sx, sy) of
+// the triangle beneath.  Outside the grid the point is clamped into it and the plane is horizontal.  Three
+// loads through the read-only path.
+DEV float terrain_at(const DevTerrain& T, float x, float y, float& sx, float& sy) {
+  const float gx = (float)(T.nx - 1), gy = (float)(T.ny - 1);
+  float u = (x - T.x0) * T.inv, v = (y - T.y0) * T.inv;
+  const bool inside = u >= 0.f && u <= gx && v >= 0.f && v <= gy;   // (false for NaN)
+  u = fminf(fmaxf(u, 0.f), gx); v = fminf(fmaxf(v, 0.f), gy);        // (NaN -> 0)
+  const int i = (int)u < T.nx - 2 ? (int)u : T.nx - 2, j = (int)v < T.ny - 2 ? (int)v : T.ny - 2;
+  const float fu = u - (float)i, fv = v - (float)j;
+  const float* h = T.h + (size_t)j * T.nx + i;
+  // the cell's diagonal runs from (i, j) to (i+1, j+1): below it the triangle (i, j), (i+1, j), (i+1, j+1),
+  // above it (i, j), (i, j+1), (i+1, j+1); hm is the height of the triangle's third vertex
+  const bool lower = fu >= fv;
+  const float h00 = ldg(h), h11 = ldg(h + T.nx + 1), hm = ldg(lower ? h + 1 : h + T.nx);
+  const float a = lower ? hm - h00 : h11 - hm, b = lower ? h11 - hm : hm - h00;   // rise per cell along x, y
+  sx = inside ? a * T.inv : 0.f;
+  sy = inside ? b * T.inv : 0.f;
+  return h00 + fu * a + fv * b;
+}
+// H(x, y) of a terrain descriptor, 0 for none or the flat floor (dial_terrain_height of a custom reward)
+DEV float terrain_height(const void* t, float x, float y) {
+  const DevTerrain* T = static_cast<const DevTerrain*>(t);
+  float sx, sy;
+  return T && T->nx > 0 ? terrain_at(*T, x, y, sx, sy) : 0.f;
+}
+
 // arguments of one rollout launch
 struct RolloutArgs {
   int32_t nrows;        // sample rows rolled by this launch
@@ -254,6 +294,10 @@ struct RolloutArgs {
   const InstSchedule* sched;
   const int32_t* iter_lim;
   int32_t iter;
+  // per-instance terrain (dial_plan_set_instance_terrain), [instances] or null: row r reads entry
+  // r / rows_per_inst (entry 0 when rows_per_inst == 0); nx == 0 is the flat floor.  Read by the terrain
+  // builds (-DDIAL_TERRAIN) only.
+  const DevTerrain* terrain;
 };
 
 // rows of one model slot of `models`: a member block of an ensemble plan, else an instance
@@ -1180,6 +1224,9 @@ struct WarpCtx {
   int s_top;           // first dof of its chain
   uint32_t s_conmask;  // contacts whose rows can be non-zero in this lane's column
   int e_cb;            // edge lanes: first position of the contact's chain (NRP if the body hangs off the root chain)
+#ifdef DIAL_TERRAIN
+  const DevTerrain* ter;   // this row's terrain, null on the flat floor
+#endif
 };
 
 #define SM(name) (w.s + w.M->o_##name)
@@ -2746,6 +2793,16 @@ DEV V3 frame_tangent(V3 n) {   // second row of mjx math.make_frame(n)
   return vnormalize(alt - n * dot(n, alt), bn);
 }
 
+// A floor contact on a terrain: the plane of the triangle under the sphere centre c replaces the floor's, as
+// its normal n and the point org = (c.x, c.y, H) on it.  A flat triangle gives exactly the floor's normal
+// (0, 0, 1), so a flat terrain at the floor's height computes bitwise what the floor computes.
+DEV void terrain_plane(const DevTerrain& T, V3 c, V3& n, V3& org) {
+  float sx, sy;
+  const float H = terrain_at(T, c.x, c.y, sx, sy);
+  n = (sx == 0.f && sy == 0.f) ? v3(0.f, 0.f, 1.f) : v3(-sx, -sy, 1.f) * (1.f / sqrtf(1.f + sx * sx + sy * sy));
+  org = v3(c.x, c.y, H);
+}
+
 template <class SH = ShapeRT>
 DEV void collide(WarpCtx& w) {
   const DevModel& M = *w.M;
@@ -2767,18 +2824,27 @@ DEV void collide(WarpCtx& w) {
   if (kind == PAIR_PLANE_SPHERE || kind == PAIR_PLANE_CAPSULE) {
     n = mat_z(X1, m.geom_quat[g1]);
     const float radius = m.geom_size[g2][0];
-    V3 center = gp2;
+    V3 center = gp2, org = gp1;
     if (kind == PAIR_PLANE_CAPSULE) {
       V3 ax = mat_z(X2, m.geom_quat[g2]);
+#ifdef DIAL_TERRAIN
+      // this end sphere's own triangle, before the frame is built from n (the same centre is computed again
+      // below, where the flat builds compute it: moving that line changes their register allocation)
+      center = gp2 + ax * ((M.con_sub[lane] == 0 ? 1.f : -1.f) * m.geom_size[g2][1]);
+      if (w.ter && b1 == 0) terrain_plane(*w.ter, center, n, org);
+#endif
       float bn;
       V3 bd = vnormalize(ax - n * dot(n, ax), bn);
       V3 alt = (n.y > -0.5f && n.y < 0.5f) ? v3(0, 1, 0) : v3(0, 0, 1);
       t1 = bn < 0.5f ? alt : bd;
       center = gp2 + ax * ((M.con_sub[lane] == 0 ? 1.f : -1.f) * m.geom_size[g2][1]);
     } else {
+#ifdef DIAL_TERRAIN
+      if (w.ter && b1 == 0) terrain_plane(*w.ter, center, n, org);
+#endif
       t1 = frame_tangent(n);
     }
-    dist = dot(center - gp1, n) - radius;
+    dist = dot(center - org, n) - radius;
     p = center - n * (radius + 0.5f * dist);
   } else {
     V3 q1 = gp1, q2 = gp2;
@@ -3490,6 +3556,14 @@ DEV void reward_partials(WarpCtx& w, const dial_task& T, int step, int stage, fl
         int sid = c.feet_site[f], sb = m.site_bodyid[sid];
         const float* X = SM(xmat) + 9 * sb;
         z = SM(xpos)[3 * sb + 2] + X[6] * m.site_pos[sid][0] + X[7] * m.site_pos[sid][1] + X[8] * m.site_pos[sid][2];
+#ifdef DIAL_TERRAIN
+        if (w.ter) {   // the foot's height above the terrain beneath it
+          const float fx = SM(xpos)[3 * sb] + X[0] * m.site_pos[sid][0] + X[1] * m.site_pos[sid][1] + X[2] * m.site_pos[sid][2];
+          const float fy = SM(xpos)[3 * sb + 1] + X[3] * m.site_pos[sid][0] + X[4] * m.site_pos[sid][1] + X[5] * m.site_pos[sid][2];
+          float sx, sy;
+          z -= terrain_at(*w.ter, fx, fy, sx, sy);
+        }
+#endif
         float e = (zt - z) / 0.05f;
         p0 = -e * e;
       } else if (env == DIAL_ENV_H1_WALK) {
@@ -3541,6 +3615,11 @@ DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, flo
     x.contact_dist = SM(cdist); x.contact_pos = SM(cpos);
     x.site_bodyid = m.site_bodyid; x.site_pos = &m.site_pos[0][0];
     x.user = T.user;
+#ifdef DIAL_TERRAIN
+    x.terrain = w.ter;
+#else
+    x.terrain = nullptr;
+#endif
     return dial_custom_reward(&x);
   }
 #endif
@@ -3573,7 +3652,11 @@ DEV float reward_lane0(WarpCtx& w, const dial_task& T, int step, int& stage, flo
     float r_yaw = -wy * wy;
     float r_vel = -((bk.vb.x - vtx) * (bk.vb.x - vtx) + (bk.vb.y - vty) * (bk.vb.y - vty));
     float r_ang = -(bk.ab.z - atz) * (bk.ab.z - atz);
-    float r_h = -(bk.pos.z - T.pos_tar[2]) * (bk.pos.z - T.pos_tar[2]);
+    float bz = bk.pos.z;
+#ifdef DIAL_TERRAIN
+    if (w.ter) { float sx, sy; bz -= terrain_at(*w.ter, bk.pos.x, bk.pos.y, sx, sy); }   // above the terrain beneath
+#endif
+    float r_h = -(bz - T.pos_tar[2]) * (bz - T.pos_tar[2]);
     if (env == DIAL_ENV_GO2_WALK) {
       rew = 0.1f * r_gaits + 0.5f * r_upright + 0.3f * r_yaw + r_vel + r_ang + r_h;
     } else if (env == DIAL_ENV_H1_LOCO) {
@@ -3626,6 +3709,9 @@ DEV void rollout_warp(const DevModel* Mp, const DevPlan* Pp, float* slab, const 
   // instance of a batched launch and the row inside it (the sample index)
   const int inst = A.rows_per_inst > 0 ? row / A.rows_per_inst : 0;
   const int lrow = row - inst * A.rows_per_inst;
+#ifdef DIAL_TERRAIN
+  w.ter = A.terrain && A.terrain[inst].nx > 0 ? A.terrain + inst : nullptr;
+#endif
   // ancestor chain of this lane's dof
   w.nch = 0; w.ndesc = 0; w.mylevel = -1; w.parent = -1;
 #pragma unroll

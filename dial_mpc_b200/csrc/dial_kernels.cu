@@ -52,6 +52,27 @@ DIAL_DECL_LAUNCH(3)
 #if DIAL_HAS_VARIANT(4)
 DIAL_DECL_LAUNCH(4)
 #endif
+// Terrain builds (dial_rollout_variant.cu with -DDIAL_TERRAIN) of every stock variant but the dense one, which
+// has none: the launches that read a terrain (dial_plan_set_instance_terrain) run them.  A custom build holds
+// one when compiled with DIAL_TERRAIN, and its one kernel then serves every launch.
+#if defined(DIAL_ONLY_VARIANT) && !defined(DIAL_TERRAIN)
+#define DIAL_HAS_TERRAIN(v) 0
+#else
+#define DIAL_HAS_TERRAIN(v) (DIAL_HAS_VARIANT(v) && (v) != 3)
+#endif
+#define DIAL_DECL_TERRAIN(v) cudaError_t dial_launch_rollout_v##v##_terrain(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t);
+#if DIAL_HAS_TERRAIN(0)
+DIAL_DECL_TERRAIN(0)
+#endif
+#if DIAL_HAS_TERRAIN(1)
+DIAL_DECL_TERRAIN(1)
+#endif
+#if DIAL_HAS_TERRAIN(2)
+DIAL_DECL_TERRAIN(2)
+#endif
+#if DIAL_HAS_TERRAIN(4)
+DIAL_DECL_TERRAIN(4)
+#endif
 // Shape-specialised star<3,6> kernels (dial_rollout_variant.cu with -DDIAL_SHAPE_NAME=s): the stock Go2
 // scene, with the structure values that dial_mpc_b200.modelc.shape derives from its model.  A plan launches one only when dial_shape_matches_<s> finds every fixed
 // value equal to its own model and plan.  Custom-reward builds hold none.
@@ -780,6 +801,8 @@ struct LaunchKey {
   bool push = false;       // some instance was given a push table: the push launch runs after every env step
   bool plant = false;      // some instance was given a plant fidelity: the plant's env step runs on the plant slots
   uint32_t plant_ks = 0;   // the distinct substep counts in use (bit k - 1: substeps k), one plant launch each
+  bool terrain[2] = {false, false};   // some instance was given a terrain on side DIAL_TERRAIN_PLANT / _PLANNER:
+                                      // that side's launches read the terrain table, in the terrain build
   bool predicts = false;   // some instance predicts through a delay d_b > 0: the queue launch also runs without an env step
   int npred = 0;           // prediction launches
   // the planner's rollouts start from the planning state, not the plant state
@@ -787,7 +810,7 @@ struct LaunchKey {
   bool operator!=(const LaunchKey& o) const {
     return models != o.models || members != o.members || sched != o.sched || lims != o.lims || adapt != o.adapt ||
            delay != o.delay || obs != o.obs || push != o.push || plant != o.plant || plant_ks != o.plant_ks ||
-           predicts != o.predicts || npred != o.npred;
+           predicts != o.predicts || npred != o.npred || terrain[0] != o.terrain[0] || terrain[1] != o.terrain[1];
   }
 };
 
@@ -889,6 +912,11 @@ struct dial_plan {
   Staged<DevModel> plant_models;
   Staged<DevPlan> plant_plans;
   Staged<int32_t> plant_mask;
+  // per-instance terrain (dial_plan_set_instance_terrain), per side, allocated by the first terrain on that side:
+  // the descriptors [n_inst] (nx 0: flat) and each instance's heights, one slot as wide as the largest table
+  // it was given so far
+  Staged<DevTerrain> terrain[2];
+  std::vector<Staged<float>> heights[2];
   // the plan's device buffers that cudaMalloc allocated, by the address of the pointer holding each (own)
   std::vector<void**> owned;
   // cudaMalloc `bytes` into `ptr`, which the plan owns from then on (free_since, dial_plan_destroy); with
@@ -943,6 +971,7 @@ static LaunchKey launch_key(const dial_plan* p) {
   k.sched = p->sched.d != nullptr; k.lims = p->lims.d != nullptr; k.adapt = p->pred_qd != nullptr;
   k.delay = p->delay.d != nullptr; k.obs = p->obs.d != nullptr; k.push = p->pushes.d != nullptr;
   k.plant = p->plant_models.d != nullptr;
+  k.terrain[0] = p->terrain[0].d != nullptr; k.terrain[1] = p->terrain[1].d != nullptr;
   for (int b = 0; k.plant && b < p->n_inst; ++b) k.plant_ks |= 1u << (plant_substeps(p, b) - 1);
   for (int b = 0; k.delay && b < p->n_inst; ++b) {
     const DelaySetting& s = p->delay.h[b];
@@ -974,7 +1003,7 @@ extern "C" const char* dial_last_error(void) { return g_err.c_str(); }
 extern "C" size_t dial_sizeof(int which) {
   return which == 0 ? sizeof(dial_model_desc) : which == 1 ? sizeof(dial_plan_desc) : which == 2 ? sizeof(dial_state)
        : which == 3 ? sizeof(dial_mpc_buffers) : which == 4 ? sizeof(dial_task) : which == 5 ? sizeof(dial_push)
-       : which == 6 ? sizeof(dial_plant) : 0;
+       : which == 6 ? sizeof(dial_plant) : which == 7 ? sizeof(dial_terrain) : 0;
 }
 
 // solver instantiation by tree shape: star<3,6> (quadruped), star<5,7> (humanoid), star<5,6>,
@@ -995,6 +1024,23 @@ static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, c
   }
   p->launches++;
   if (!dP) dP = p->dP;
+  if (A.terrain) {   // a launch that reads a terrain table: the terrain build of the plan's variant
+    switch (p->variant) {
+#if DIAL_HAS_TERRAIN(1)
+      case 1: return dial_launch_rollout_v1_terrain(p->dM, dP, A, grid, wpc, smem, st);
+#endif
+#if DIAL_HAS_TERRAIN(2)
+      case 2: return dial_launch_rollout_v2_terrain(p->dM, dP, A, grid, wpc, smem, st);
+#endif
+#if DIAL_HAS_TERRAIN(4)
+      case 4: return dial_launch_rollout_v4_terrain(p->dM, dP, A, grid, wpc, smem, st);
+#endif
+#if DIAL_HAS_TERRAIN(0)
+      case 0: return dial_launch_rollout_v0_terrain(p->dM, dP, A, grid, wpc, smem, st);
+#endif
+      default: return cudaErrorInvalidDeviceFunction;
+    }
+  }
 #ifndef DIAL_ONLY_VARIANT
   if (p->shape > 0 && !generic) return kShapes[p->shape - 1].launch(p->dM, dP, A, grid, wpc, smem, st);
 #endif
@@ -1201,6 +1247,10 @@ extern "C" void dial_plan_destroy(dial_plan* p) {
   p->adapt.release(); p->belief_L.release(); p->belief_w.release(); p->sched.release(); p->lims.release();
   p->delay.release(); p->obs.release(); p->pushes.release();
   p->plant_models.release(); p->plant_plans.release(); p->plant_mask.release();
+  for (int s = 0; s < 2; ++s) {
+    p->terrain[s].release();
+    for (auto& h : p->heights[s]) h.release();
+  }
   for (int i = 0; i < 2; ++i) { if (p->ev_main[i]) cudaEventDestroy(p->ev_main[i]); if (p->ev_side[i]) cudaEventDestroy(p->ev_side[i]); }
   if (p->side) cudaStreamDestroy(p->side);
   p->free_since(0);
@@ -1728,6 +1778,68 @@ extern "C" int dial_plan_set_instance_plant(dial_plan* p, int b, const dial_plan
   return 0;
 }
 
+extern "C" int dial_plan_set_instance_terrain(dial_plan* p, int b, int side, const dial_terrain* t, void* stream) {
+  static const char* fn = "dial_plan_set_instance_terrain";
+  if (!p) return fail(std::string(fn) + ": null plan");
+  if (int rc = need_instance(p, fn, b)) return rc;
+  const std::string at = std::string(fn) + ": ";
+  if (side != DIAL_TERRAIN_PLANT && side != DIAL_TERRAIN_PLANNER)
+    return fail(at + "side " + std::to_string(side) + " out of range (0 plant, 1 planner)");
+  if (t) {
+    if (t->nx < 2 || t->nx > DIAL_MAXTERRAIN || t->ny < 2 || t->ny > DIAL_MAXTERRAIN)
+      return fail(at + "grid " + std::to_string(t->nx) + " x " + std::to_string(t->ny) + " out of range (2.." DIAL_STR(DIAL_MAXTERRAIN) " per side)");
+    if (!(t->spacing > 0.f && t->spacing <= FLT_MAX)) return fail(at + "spacing must be finite and > 0, got " + fmt_g(t->spacing));
+    if (!std::isfinite(t->x0) || !std::isfinite(t->y0)) return fail(at + "origin must be finite, got (" + fmt_g(t->x0) + ", " + fmt_g(t->y0) + ")");
+    if (!t->heights) return fail(at + "null heights");
+    for (int j = 0; j < t->ny; ++j)
+      for (int i = 0; i < t->nx; ++i)
+        if (!std::isfinite(t->heights[(size_t)j * t->nx + i]))
+          return fail(at + "heights[" + std::to_string(j) + "][" + std::to_string(i) + "] is not finite, got " + fmt_g(t->heights[(size_t)j * t->nx + i]));
+  }
+  const dial_model_desc& m = p->hM.m;
+  bool floor = false;
+  for (int k = 0; k < m.npair; ++k)
+    floor |= (m.pair_kind[k] == PAIR_PLANE_SPHERE || m.pair_kind[k] == PAIR_PLANE_CAPSULE) && m.geom_bodyid[m.pair_geom1[k]] == 0;
+  if (!floor) return fail(at + "the model has no floor pair (a plane geom on the world body against a sphere or capsule)");
+  if (p->hM.dense) return fail(at + "the dense solver path has no terrain build");
+  if (!DIAL_HAS_TERRAIN(p->variant)) return fail(at + "this custom build has no terrain kernel (compile it with DIAL_TERRAIN)");
+  const dial_plan_desc& c = p->hP.c;
+  if (c.Ntotal != c.Nsample || p->xch.on) return fail(at + "sharded plans (Ntotal != Nsample) have no per-instance terrain");
+  if (!p->mpc_bound) return fail(at + "call dial_mpc_bind first");
+  Staged<DevTerrain>& D = p->terrain[side];
+  if (!t && !D.d) return 0;   // no instance has a terrain on this side: b is already flat
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (!D.d) {   // first terrain on this side: flat descriptors, no heights yet
+    DevTerrain flat;
+    memset(&flat, 0, sizeof(flat));
+    if ((e = D.allocate(p->n_inst, 1, flat)) != cudaSuccess) return fail(at + cudaGetErrorString(e));
+    p->heights[side].assign(p->n_inst, Staged<float>());
+  }
+  Staged<float>& Hs = p->heights[side][b];
+  const size_t n = t ? (size_t)t->nx * t->ny : 0;
+  if (t && (!Hs.d || Hs.width < n)) {
+    // a table larger than b's allocation: a new one (the old one is freed once the device is idle), and the
+    // graphs are captured again
+    Staged<float> grown;
+    if ((e = grown.allocate(1, n, 0.f)) != cudaSuccess) return fail(at + cudaGetErrorString(e));
+    if ((e = cudaDeviceSynchronize()) != cudaSuccess) { grown.release(); return fail(at + cudaGetErrorString(e)); }
+    Hs.release();
+    Hs = grown;
+    drop_graphs(p);
+  }
+  if (t) e = Hs.put(0, [&](float* h) { memcpy(h, t->heights, n * sizeof(float)); }, st);
+  if (e == cudaSuccess)
+    e = D.put(b, [&](DevTerrain* T) {
+      memset(T, 0, sizeof(*T));
+      if (!t) return;
+      T->nx = t->nx; T->ny = t->ny; T->x0 = t->x0; T->y0 = t->y0; T->inv = 1.f / t->spacing; T->h = Hs.d;
+    }, st);
+  p->key = launch_key(p);
+  if (e != cudaSuccess) return fail(at + cudaGetErrorString(e));
+  return 0;
+}
+
 extern "C" int dial_plan_observed_state(dial_plan* p, float* qpos, float* qvel, float* warm, int32_t* counters,
                                         int32_t* age, void* stream) {
   static const char* fn = "dial_plan_observed_state";
@@ -2048,6 +2160,9 @@ static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_
   const bool batched = ni > 1;
   const dial_plan::DelayQueue& Q = p->queue;
   const dial_plan::PlanningState& P = p->planning;
+  // the terrain tables the plant's env step and the planner's launches read (null: every instance on the floor)
+  const DevTerrain* plant_terrain = k.terrain[DIAL_TERRAIN_PLANT] ? p->terrain[DIAL_TERRAIN_PLANT].d : nullptr;
+  const DevTerrain* planner_terrain = k.terrain[DIAL_TERRAIN_PLANNER] ? p->terrain[DIAL_TERRAIN_PLANNER].d : nullptr;
   float* Y[2] = {B.Y, p->mpc_Y1};
   int cur = 0;
   // control latency, once some instance was given a delay: the queues move in a step with an env step, which
@@ -2075,6 +2190,7 @@ static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_
     A.rows_per_inst = K; A.rows_per_model = 1; A.models = p->members.d;
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = K; }
     A.qd = p->pred_qd;
+    A.terrain = planner_terrain;
     CUDA_OK(launch_rollout(p, A, 1, st));
   }
   if (env_step == 1) {
@@ -2088,6 +2204,7 @@ static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_
     if (B.tasks) { A.tasks = B.tasks; A.task_rows = batched ? 1 : 0; }
     A.models = p->models.d;
     A.qpos_out = B.qpos; A.qvel_out = B.qvel; A.warm_out = B.qacc_warmstart; A.ctrl_out = B.ctrl;
+    A.terrain = plant_terrain;
     if (!k.plant) CUDA_OK(launch_rollout(p, A, 1, st));
     // with plant fidelities: one launch of the generic kernel per distinct substep count k, on the plant slots
     // and the plan descriptor of k; batched, the rows of the other groups exit at entry (mask k as the
@@ -2149,6 +2266,7 @@ static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_
     A.models = p->n_ens > 0 ? P.models : p->models.d;
     A.iter_lim = k.obs ? p->ob.len : Q.len; A.iter = j;
     A.qpos_out = P.qpos; A.qvel_out = P.qvel; A.warm_out = P.warm;
+    A.terrain = planner_terrain;
     CUDA_OK(launch_rollout(p, A, 1, st));
   }
   if (k.planning()) { qpos0 = P.qpos; qvel0 = P.qvel; warm0 = P.warm; cnt0 = P.cnt; }
@@ -2184,6 +2302,7 @@ static int mpc_enqueue(dial_plan* p, const LaunchKey& k, int n_diffuse, int env_
     p->cur ^= 1;
     A.rews = K > 1 ? p->ens_rews : B.rews; A.q = p->traj_q[p->cur]; A.qd = p->traj_qd[p->cur]; A.xpos = p->traj_x[p->cur];
     A.dbg = p->dbg;
+    A.terrain = planner_terrain;
     fill_xch(p, A);
     CUDA_OK(launch_rollout_any(p, A, st));
     if (K > 1) {   // each sample's score under its instance's risk measure (K = 1: the reward itself)

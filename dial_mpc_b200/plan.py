@@ -238,6 +238,14 @@ class Plan:
         self._check(self.lib.dial_plan_set_instance_plant(self.handle, int(b), None if plant is None else C.byref(plant),
                                                           _stream()))
 
+    def set_instance_terrain(self, b: int, side: int, terrain) -> None:
+        """Instance b's terrain on ``side`` (``terrain.PLANT`` or ``terrain.PLANNER``) from the next ``mpc_step`` on:
+        a ``terrain.Terrain`` (None: the flat floor).  The heights are copied into plan-owned device memory,
+        stream-ordered on the current stream (``dial_plan_set_instance_terrain``)."""
+        t = None if terrain is None else terrain.c_struct()
+        self._check(self.lib.dial_plan_set_instance_terrain(self.handle, int(b), int(side),
+                                                            None if t is None else C.byref(t), _stream()))
+
     def _check(self, rc: int) -> None:
         if rc != 0:
             raise RuntimeError(f"dial_b200: {self.lib.dial_last_error().decode()} (rc={rc})")

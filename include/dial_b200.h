@@ -47,6 +47,9 @@ extern "C" {
 #define DIAL_MAXDELAY 16   /* control steps of latency of one instance (dial_plan_set_instance_delay) */
 #define DIAL_MAXPUSH 16    /* entries of one instance's push table (dial_plan_set_instance_pushes) */
 #define DIAL_MAXSUBSTEPS 16 /* physics substeps per plan physics step of one instance's plant (dial_plan_set_instance_plant) */
+#define DIAL_MAXTERRAIN 1024 /* grid vertices per side of one instance's terrain (dial_plan_set_instance_terrain) */
+#define DIAL_TERRAIN_PLANT 0   /* the side of dial_plan_set_instance_terrain: the plant's env step */
+#define DIAL_TERRAIN_PLANNER 1 /* the planner's rollouts, ensemble members, adaptation and predictions */
 #define DIAL_IPC_HANDLE_BYTES 64
 
 /* environments (reward functors fused into the rollout kernel) */
@@ -191,7 +194,7 @@ typedef struct dial_plan dial_plan;
 int dial_abi_version(void);
 const char* dial_last_error(void);
 /* sizeof() of the descriptor structs as compiled into the library: which = 0 model, 1 plan,
- * 2 state, 3 mpc buffers, 4 task, 5 push, 6 plant (lets foreign-language bindings verify their struct
+ * 2 state, 3 mpc buffers, 4 task, 5 push, 6 plant, 7 terrain (lets foreign-language bindings verify their struct
  * layout). */
 size_t dial_sizeof(int which);
 
@@ -649,6 +652,42 @@ typedef struct dial_plant {
  * dial_plan_set_instance_model(b) reaches b's plant with its fidelity kept.  Fails for b out of range, a field
  * out of range, and sharded or unbound plans; the error names the bad argument. */
 int dial_plan_set_instance_plant(dial_plan* plan, int b, const dial_plant* f, void* stream);
+
+/* One instance's terrain (dial_plan_set_instance_terrain): a grid of nx x ny heights h[j][i] (row-major, j the
+ * y index), 2..DIAL_MAXTERRAIN per side, spacing > 0, origin (x0, y0).  Vertex (i, j) is the world point
+ * (x0 + i spacing, y0 + j spacing, h[j][i]); heights are absolute world z. */
+typedef struct dial_terrain {
+  int32_t nx, ny;
+  float x0, y0, spacing;
+  const float* heights;   /* [ny][nx], host memory */
+} dial_terrain;
+
+/* Per-instance terrain of dial_mpc_step.  For an instance with a terrain on a side, the terrain replaces every
+ * plane geom on the world body in that side's env steps.  Each cell is split along the diagonal from (i, j) to
+ * (i+1, j+1) into two triangles; H(x, y) is the piecewise linear surface.  A sphere (centre c, radius r) of a
+ * floor pair, and each end sphere of a capsule on one, is tested against the plane of the triangle under
+ * (c.x, c.y): with that triangle's slopes (sx, sy), n = (-sx, -sy, 1) / |.| (exactly (0, 0, 1) when both are
+ * 0), dist = dot(c - (c.x, c.y, H(c.x, c.y)), n) - r, and the contact point and frame follow the plane's
+ * formulas with that n.  Outside the grid the query point is clamped into it and the plane is horizontal at H
+ * of the clamped point.  Every floor pair keeps its contact slots, so the contact counts and the solver are
+ * those of the flat floor.  The model is locally planar: it holds where the surface varies slowly at the scale
+ * of a foot, not at steps (a sphere only sees the triangle beneath its centre).  The built-in rewards measure
+ * their base height (Go2 walk, H1 walk, H1 loco) and Go2 walk's foot heights above H beneath; custom rewards
+ * read it with dial_terrain_height (include/dial_custom_reward.h).
+ * Side DIAL_TERRAIN_PLANT is read by the plant's env step (every plant-fidelity launch), side
+ * DIAL_TERRAIN_PLANNER by the planner's rollouts, the ensemble members, adaptation's member steps and the
+ * prediction launches.  Launches that read a terrain run the terrain build of the plan's solver variant (the
+ * generic star<3,6> kernel on a Go2 plan); rows without a terrain compute there bitwise what they compute in
+ * the plan's other kernels.  A plan on which no terrain is ever set launches what it launched before. */
+
+/* Instance b's terrain on `side` [host]; t = NULL makes that side flat.  The heights are copied into
+ * plan-owned device memory, stream-ordered on `stream` (the plan must be bound, dial_mpc_bind).  The first
+ * terrain on a side drops the captured graphs, and so does a table larger than b's allocation on that side;
+ * other calls keep them and take effect at the next replay.  Fails for b or side out of range, a grid size out
+ * of range, a spacing that is not finite and > 0, a height that is not finite, a model without a floor pair
+ * (a plane geom on the world body), the dense solver path, and sharded or unbound plans; the error names the
+ * bad argument. */
+int dial_plan_set_instance_terrain(dial_plan* plan, int b, int side, const dial_terrain* t, void* stream);
 
 /* Bind the state block; M_shift [host][Hn+1][Hn+1] = u2node . roll(-1, last row 0) . node2u
  * (MBDPI.shift, core/dial_core.py:160-165), shared by all instances of a batched plan.  Drops

@@ -46,6 +46,7 @@ typedef struct dial_reward_ctx {
   const int* site_bodyid;    /* [nsite]                                                */
   const float* site_pos;     /* [nsite][3] site offsets in their body frame            */
   const float* user;         /* [n_user] dial_plan_desc.user                           */
+  const void* terrain;       /* this row's terrain (read it with dial_terrain_height)  */
 } dial_reward_ctx;
 
 /* Brax xd.ang[body-1]: world angular velocity (rad/s) */
@@ -75,6 +76,13 @@ DIAL_REWARD_FN void dial_site_xpos(const dial_reward_ctx* c, int site, float out
   out[0] = p[0] + X[0] * s[0] + X[1] * s[1] + X[2] * s[2];
   out[1] = p[1] + X[3] * s[0] + X[4] * s[1] + X[5] * s[2];
   out[2] = p[2] + X[6] * s[0] + X[7] * s[1] + X[8] * s[2];
+}
+
+/* Height H(x, y) of the terrain beneath the world point (x, y) on this row (include/dial_b200.h,
+ * dial_plan_set_instance_terrain); 0 on a row without a terrain.  Lets a reward measure heights above the
+ * ground. */
+DIAL_REWARD_FN float dial_terrain_height(const dial_reward_ctx* c, float x, float y) {
+  return terrain_height(c->terrain, x, y);
 }
 
 #endif /* DIAL_CUSTOM_REWARD_H_ */

@@ -32,6 +32,10 @@ runs the push launch (use ``--env-step 1``; an entry firing in every step measur
 mapping such as ``'{substeps: 4, iterations: 100, ls_iterations: 50, tolerance: 1e-8}'`` applied to every instance,
 or a YAML file with one spec or a list of one per instance (null: none), so that a step with an env step runs one
 plant launch per distinct substep count (use ``--env-step 1``).
+``--terrain SPEC``: every instance's ground (``DeviceLoop(..., terrain=...)``): a YAML flow mapping such as
+``'{kind: rough, amplitude: 0.03, wavelength: 0.3, seed: 1, planner: true}'`` applied to every instance, or a YAML
+file with one spec or a list of one per instance (null: none); the launches that read a terrain run the terrain
+build of the rollout kernel.
 ``--profile-kernels``: instead of the timing, run the steps without graph capture under torch.profiler and
 print the mean device time per launch of the rollout, update, ensemble reduction, delay queue, observe and push
 kernels."""
@@ -110,6 +114,10 @@ def main():
     ap.add_argument("--plant", default=None, metavar="SPEC_OR_FILE",
                     help="a plant spec for every instance (a YAML flow mapping such as '{substeps: 4}') or a YAML file "
                          "with one spec or a list of one per instance (DeviceLoop(..., plant=...))")
+    ap.add_argument("--terrain", default=None, metavar="SPEC_OR_FILE",
+                    help="a terrain spec for every instance (a YAML flow mapping such as '{kind: slope, angle: 10, "
+                         "planner: true}') or a YAML file with one spec or a list of one per instance "
+                         "(DeviceLoop(..., terrain=...))")
     ap.add_argument("--profile-kernels", action="store_true",
                     help="print per-kernel device times (eager launches under torch.profiler) instead of the step time")
     args = ap.parse_args()
@@ -169,7 +177,7 @@ def main():
     given, settings = {}, {}
     for key, opt, text in (("schedule", "--schedules", args.schedules), ("delay", "--delays", args.delays),
                            ("observe", "--observe", args.observe), ("pushes", "--pushes", args.pushes),
-                           ("plant", "--plant", args.plant)):
+                           ("plant", "--plant", args.plant), ("terrain", "--terrain", args.terrain)):
         if text is not None:
             try:
                 given[key] = yaml.safe_load(open(text) if os.path.isfile(text) else text)
@@ -222,7 +230,7 @@ def main():
             n, tot = acc.get(key, (0, 0.0))
             acc[key] = (n + 1, tot + us)
         print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, ensemble=args.ensemble,
-                              risk=args.risk, adapt=args.adapt, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
+                              risk=args.risk, adapt=args.adapt, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, terrain=args.terrain, env_step=es, kernels_us_per_launch={k: tot / n for k, (n, tot) in acc.items()},
                               launches_per_step={k: n / args.steps for k, (n, tot) in acc.items()}, gpu=gpu_info())))
         return
     evs = []
@@ -239,7 +247,7 @@ def main():
     print(json.dumps(dict(config=f"{b['name']} (BASELINE configs[{args.config}])", instances=B, distinct_tasks=args.distinct_tasks,
                           distinct_models=args.distinct_models, ensemble=args.ensemble, risk=args.risk, adapt=args.adapt, env_step=es, rows_per_rollout=rows,
                           Nsample=cfg.Nsample, Hsample=cfg.Hsample, Ndiffuse=cfg.Ndiffuse, steps=args.steps,
-                          schedules=args.schedules, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, Ndiffuse_per_instance=n_diffuse if "schedule" in given else None,
+                          schedules=args.schedules, delays=args.delays, observe=args.observe, pushes=args.pushes, plant=args.plant, terrain=args.terrain, Ndiffuse_per_instance=n_diffuse if "schedule" in given else None,
                           value=sum(n_diffuse) * cfg.Nsample * cfg.Hsample / t, unit="sample-steps/s",
                           ms_per_step=1e3 * t, gpu=gpu_info())))
 
