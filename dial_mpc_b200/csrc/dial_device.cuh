@@ -316,6 +316,13 @@ HD int cta_instance(const RolloutArgs& A, int cta, int wpc) {
   return r0 / A.rows_per_inst == r1 / A.rows_per_inst ? r0 / A.rows_per_inst : -1;
 }
 
+// The CTAs of a rollout_kernel launch at `wpc` warps per CTA: one per wpc rows, or with `models`
+// ceil(model_rows / wpc) per model slot (the kernel's row mapping)
+HD int rollout_grid(const RolloutArgs& A, int wpc) {
+  if (A.models && model_rows(A) > 0) return (A.nrows / model_rows(A)) * ((model_rows(A) + wpc - 1) / wpc);
+  return (A.nrows + wpc - 1) / wpc;
+}
+
 // ---------------------------------------------------------------------------------
 // Risk measure of an ensemble plan (dial_plan_set_ensemble_risk): how the K >= 2 member rewards of one
 // sample become its score.  The host derives the setting once (ens_risk_derive); the reduction kernel

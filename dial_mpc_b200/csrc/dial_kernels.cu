@@ -1013,9 +1013,7 @@ extern "C" size_t dial_sizeof(int which) {
 static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, cudaStream_t st,
                                   const DevPlan* dP = nullptr, bool generic = false) {
   const size_t smem = sizeof(DevModel) + sizeof(DevPlan) + (size_t)wpc * p->hM.warp_floats * sizeof(float);
-  int grid = (A.nrows + wpc - 1) / wpc;
-  // per-instance or member models: ceil(model_rows / wpc) CTAs per model slot (rollout_kernel's row mapping)
-  if (A.models && model_rows(A) > 0) grid = (A.nrows / model_rows(A)) * ((model_rows(A) + wpc - 1) / wpc);
+  int grid = rollout_grid(A, wpc);
   if (A.row_counter) {
     const int resident = p->num_sms * (wpc > 8 ? 1 : 16 / wpc);
     grid = grid < resident ? grid : resident;

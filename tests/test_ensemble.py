@@ -2,8 +2,6 @@
 ``--ensemble`` file, and, through the warp emulator, ensemble rollout launches whose member rows are bitwise
 single-instance launches on each member's model."""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import numpy as np
@@ -14,8 +12,8 @@ from dial_mpc_b200 import _capi
 from dial_mpc_b200 import random as drandom
 from dial_mpc_b200.utils.spline import interp_matrix
 from tests.conftest import make_pair
+from tests.emul import emul
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 FEET = ("FR", "FL", "RR", "RL")
 
 
@@ -105,19 +103,6 @@ def test_cli_reports_ensemble_errors(tmp_path, monkeypatch, capsys, text, extra,
 
 
 # ---- emulator: ensemble launches -----------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    """g++ build of tests/emul/emul_ensemble.cpp (the device code under the lock-step warp emulator)."""
-    so = str(tmp_path_factory.mktemp("emul_ensemble") / "libdial_emul_ensemble.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_ensemble.cpp")])
-    return C.CDLL(so)
-
-
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
 def _desc_with_task(desc, t):
     d = _capi.dial_plan_desc.from_buffer_copy(desc)
     for name in _capi.TASK_FIELDS:
@@ -129,24 +114,19 @@ def _desc_with_task(desc, t):
     return d
 
 
-def rollout(lib, base_model, models, desc, wpc, nrows, rows_per_inst, rows_per_model, tasks, task_rows, qpos, qvel,
-            warm, counters, rng, Ybar, noise, H):
+def rollout(base_model, models, desc, wpc, nrows, rows_per_inst, rows_per_model, tasks, task_rows, qpos, qvel, warm,
+            counters, rng, Ybar, noise, H):
     md = _capi.fill_model_desc(base_model)
     nq, nv, nb = md.nq, md.nv, md.nbody
     f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
-    qpos, qvel, warm, Ybar, noise = map(f32, (qpos, qvel, warm, Ybar, noise))
-    arr = None if models is None else (_capi.dial_model_desc * len(models))(*[_capi.fill_model_desc(m) for m in models])
-    tarr = None if tasks is None else (_capi.dial_task * len(tasks))(*tasks)
-    cin = np.ascontiguousarray(counters, dtype=np.int32)
-    rng = np.ascontiguousarray(rng, dtype=np.uint32)
     out = dict(rewss=np.zeros((nrows, H), np.float32), rews=np.zeros(nrows, np.float32),
                q=np.zeros((nrows, H, nq), np.float32), qd=np.zeros((nrows, H, nv), np.float32),
                xpos=np.zeros((nrows, H, nb - 1, 3), np.float32))
-    rc = lib.emul_rollout_ensemble(C.byref(md), arr, 0 if models is None else len(models), C.byref(desc), wpc, nrows, H,
-                                   rows_per_inst, rows_per_model, tarr, task_rows, _p(qpos), _p(qvel), _p(warm), _p(cin),
-                                   _p(rng), _p(Ybar), _p(noise), _p(out["rewss"]), _p(out["rews"]), _p(out["q"]),
-                                   _p(out["qd"]), _p(out["xpos"]))
-    assert rc == 0
+    emul.launch(md, desc, wpc=wpc, models=models, mode=1, nrows=nrows, H=H, rows_per_inst=rows_per_inst,
+                rows_per_model=rows_per_model, tasks=None if tasks is None else (_capi.dial_task * len(tasks))(*tasks),
+                task_rows=task_rows, qpos0=f32(qpos), qvel0=f32(qvel), warm0=f32(warm),
+                counters_in=np.ascontiguousarray(counters, dtype=np.int32),
+                rng_dev=np.ascontiguousarray(rng, dtype=np.uint32), Ybar=f32(Ybar), noise=f32(noise), **out)
     return out
 
 
@@ -159,7 +139,7 @@ def member_mean(r):
     return (s / np.float32(r.shape[1])).astype(np.float32)
 
 
-def test_seq_jump_ensemble_rows_equal_single_instance_launches(lib):
+def test_seq_jump_ensemble_rows_equal_single_instance_launches():
     env, o = make_pair("unitree_go2_seq_jump")
     m0 = env.sys.model
     fr = [0.4, 0.4, 0.02, 0.01, 0.01]
@@ -189,12 +169,12 @@ def test_seq_jump_ensemble_rows_equal_single_instance_launches(lib):
     counters = np.array([[45, 0], [49, 0]], np.int32)
     slots = [members[k] for b in range(B) for k in range(K)]          # member (b, k) at slot b K + k
     # mpc_enqueue's launch: rows ((b K) + k)(N+1) + i, tasks per instance
-    outs = {wpc: rollout(lib, m0, slots, desc, wpc, B * K * n1, K * n1, n1, tasks, K * n1, qpos, qvel, warm, counters,
+    outs = {wpc: rollout(m0, slots, desc, wpc, B * K * n1, K * n1, n1, tasks, K * n1, qpos, qvel, warm, counters,
                          keys, Y, noise, H) for wpc in (2, 5)}   # 2 warps: three CTAs per member, the last repeats a row
     for wpc, ens in outs.items():
         for b in range(B):
             for k in range(K):
-                one = rollout(lib, members[k], None, _desc_with_task(single, tasks[b]), 1, n1, 0, 0, None, 0,
+                one = rollout(members[k], None, _desc_with_task(single, tasks[b]), 1, n1, 0, 0, None, 0,
                               qpos[b:b + 1], qvel[b:b + 1], warm[b:b + 1], counters[b:b + 1], keys[b:b + 1],
                               Y[b:b + 1], noise, H)
                 sl = slice((b * K + k) * n1, (b * K + k + 1) * n1)
@@ -214,7 +194,7 @@ def test_seq_jump_ensemble_rows_equal_single_instance_launches(lib):
     np.testing.assert_allclose(rbar, r.astype(np.float64).mean(1), rtol=1e-6)
 
 
-def test_one_member_with_the_plan_model_equals_no_ensemble(lib):
+def test_one_member_with_the_plan_model_equals_no_ensemble():
     env, o = make_pair("unitree_go2_walk")
     m0 = env.sys.model
     B, N, Hs, Hn = 2, 4, 6, 3
@@ -231,10 +211,10 @@ def test_one_member_with_the_plan_model_equals_no_ensemble(lib):
     kw = dict(Nsample=N, Hsample=Hs, Hnode=Hn, temp_sample=0.05,
               M_n2u=interp_matrix(np.linspace(0, 1, Hn + 1), np.linspace(0, 1, Hs + 1)))
     counters = np.array([[0, 0], [17, 0]], np.int32)
-    plain = rollout(lib, m0, None, env.plan_desc(n_inst=B, **kw), 4, B * n1, n1, 0, None, 0, qpos, qvel, warm, counters,
+    plain = rollout(m0, None, env.plan_desc(n_inst=B, **kw), 4, B * n1, n1, 0, None, 0, qpos, qvel, warm, counters,
                     keys, Y, noise, H)
     desc = env.plan_desc(n_inst=B, n_ens=1, **kw)
     for models in (None, [m0] * B):    # no member set, and every member set to the plan's model
-        one = rollout(lib, m0, models, desc, 4, B * n1, n1, n1, None, 0, qpos, qvel, warm, counters, keys, Y, noise, H)
+        one = rollout(m0, models, desc, 4, B * n1, n1, n1, None, 0, qpos, qvel, warm, counters, keys, Y, noise, H)
         for f in plain:
             assert np.array_equal(one[f], plain[f]), f

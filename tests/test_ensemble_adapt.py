@@ -8,21 +8,18 @@ Subnormal weights and rewards are not covered: the library is built with -use_fa
 them to zero on the GPU, while the g++ build keeps them.  The restatement of the update uses Python's
 ``math.exp`` / ``math.log``, the C library's, as the g++ build does; the GPU's fp64 exp and log may
 differ from them in the last bit (tests/test_gpu_ensemble_adapt.py states its tolerance)."""
-import ctypes as C
 import math
-import os
 import re
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 from dial_mpc_b200 import _capi
+from tests.emul import emul
 from tests.test_ensemble import FEET, _go2
 from tests.test_ensemble_risk import CVAR, KMAX, MEAN, alphas, derive, same_bits, samples
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 CAP = 1.0e4
 f32 = np.float32
 
@@ -104,15 +101,8 @@ def belief_update(L, ell, forget):
 
 # ---- the g++ build of the device code ------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("emul_adapt") / "libdial_emul_adapt.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-ffp-contract=off", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_adapt.cpp")])
-    L = C.CDLL(so)
-    V = C.c_void_p
-    L.emul_adapt_reduce.argtypes = [V, C.c_int, C.c_int, C.c_int, C.c_float, V, C.c_float, V]
-    L.emul_adapt_update.argtypes = [V, V, V, C.c_int, C.c_int, C.c_float, V, V, V]
-    return L
+def lib():
+    return emul.build()
 
 
 def emul_reduce(lib, r, mode, alpha, w, prune):
@@ -310,21 +300,18 @@ def test_prediction_rows_equal_single_instance_env_steps(lib):
     desc = env.plan_desc(n_inst=B, n_ens=K, Nsample=4, Hsample=6, Hnode=3)
     single = env.plan_desc(Nsample=4, Hsample=6, Hnode=3)
     md = _capi.fill_model_desc(m0)
-    slots = (_capi.dial_model_desc * (B * K))(*[_capi.fill_model_desc(members[k]) for b in range(B) for k in range(K)])
+    slots = [members[k] for b in range(B) for k in range(K)]
     tarr = (_capi.dial_task * B)(*tasks)
     us = np.ascontiguousarray(np.repeat(Y0, K, 0))                     # the gather: row b K + k = Y[b][0]
     qd = np.zeros((B * K, nv), f32)
-    p = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-    assert lib.emul_env_step_rows(C.byref(md), slots, B * K, C.byref(desc), B * K, K, 1, tarr, K, p(qpos), p(qvel),
-                                  p(warm), p(counters), p(us), p(qd), None) == 0
+    emul.launch(md, desc, models=slots, mode=0, nrows=B * K, H=1, rows_per_inst=K, rows_per_model=1, tasks=tarr,
+                task_rows=K, qpos0=qpos, qvel0=qvel, warm0=warm, counters_in=counters, us=us, qd=qd)
     for b in range(B):
         for k in range(K):
             one = np.zeros((1, nv), f32)
-            mk = _capi.fill_model_desc(members[k])
-            assert lib.emul_env_step_rows(C.byref(mk), None, 0, C.byref(_desc_with_task(single, tasks[b])), 1, 0, 0,
-                                          None, 0, p(qpos[b:b + 1].copy()), p(qvel[b:b + 1].copy()),
-                                          p(warm[b:b + 1].copy()), p(counters[b:b + 1].copy()),
-                                          p(Y0[b:b + 1].copy()), None, p(one)) == 0
+            emul.launch(members[k], _desc_with_task(single, tasks[b]), mode=0, nrows=1, H=1,
+                        qpos0=qpos[b:b + 1].copy(), qvel0=qvel[b:b + 1].copy(), warm0=warm[b:b + 1].copy(),
+                        counters_in=counters[b:b + 1].copy(), us=Y0[b:b + 1].copy(), qvel_out=one)
             assert np.array_equal(qd[b * K + k], one[0]), (b, k)
         # the members were read: their predictions differ from one another
         assert not np.array_equal(qd[b * K], qd[b * K + 1]) and not np.array_equal(qd[b * K], qd[b * K + 2]), b

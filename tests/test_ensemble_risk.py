@@ -5,20 +5,17 @@ of the ``--ensemble`` file and of ``--instance-overrides``.
 
 Subnormal rewards are not covered: the library is built with -use_fast_math, which flushes them to zero
 on the GPU, while the g++ build keeps them."""
-import ctypes as C
 import math
-import os
 import re
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 from dial_mpc_b200 import _capi
+from tests.emul import emul
 from tests.test_ensemble import member_mean
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 MEAN, CVAR = _capi.DEFINES["DIAL_ENS_MEAN"], _capi.DEFINES["DIAL_ENS_CVAR"]
 KMAX = _capi.DEFINES["DIAL_MAXENS"]
 f32 = np.float32
@@ -66,14 +63,8 @@ def same_bits(a, b):
 
 # ---- the g++ build of the device code ------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("emul_risk") / "libdial_emul_risk.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_risk.cpp")])
-    L = C.CDLL(so)
-    L.emul_risk_derive.argtypes = [C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
-    L.emul_risk_reduce.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
-    return L
+def lib():
+    return emul.build()
 
 
 def emul_derive(lib, K, mode, alpha):

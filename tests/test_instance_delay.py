@@ -3,9 +3,7 @@
 queue step the kernels run (delay_queue_step, on the warp emulator), and the prediction launches with
 per-instance lengths against chains of single-row env steps."""
 import ctypes as C
-import os
 import re
-import subprocess
 import sys
 
 import numpy as np
@@ -14,9 +12,9 @@ import pytest
 from dial_mpc_b200 import _capi
 from dial_mpc_b200.utils.spline import interp_matrix
 from tests.conftest import make_pair
+from tests.emul import emul
 from tests.test_emul_batch import _instances
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 DMAX = _capi.DEFINES["DIAL_MAXDELAY"]
 
 
@@ -86,19 +84,23 @@ def test_cli_instance_override_delay_errors(tmp_path, monkeypatch, capsys, entry
 
 # ---- warp emulator ---------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    """g++ build of tests/emul/emul_delay.cpp (the device code under the lock-step warp emulator)."""
-    so = str(tmp_path_factory.mktemp("emul_delay") / "libdial_emul_delay.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_delay.cpp")])
-    lib = C.CDLL(so)
-    lib.emul_sizeof_delay.restype = C.c_size_t
-    assert lib.emul_sizeof_delay() == 8
+def lib():
+    lib = emul.build()
+    assert lib.emul_sizeof(emul.SIZEOF["DelaySetting"]) == 8
     return lib
 
 
 def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def env_launch(env, desc, nrows, rows_per_inst, us, us_row, iter_lim, iter_, s, rews):
+    """One env-step launch (mode 0, H = 1) as dial_mpc_step issues it, in place on the instance-major state s
+    (qpos, qvel, warm, cnt): nrows rows, rows_per_inst per instance, action row r at us + r us_row; with
+    iter_lim, the rows of an instance with iter_ >= iter_lim[b] do not run."""
+    emul.launch(env, desc, mode=0, nrows=nrows, H=1, rows_per_inst=rows_per_inst, us=us, us_row=us_row,
+                iter_lim=iter_lim, iter=iter_, qpos0=s["qpos"], qvel0=s["qvel"], warm0=s["warm"], counters_in=s["cnt"],
+                qpos_out=s["qpos"], qvel_out=s["qvel"], warm_out=s["warm"], counters_out=s["cnt"], rewss=rews)
 
 
 class Queue:
@@ -186,7 +188,7 @@ def test_queue_change_of_delay_refills(lib):
                 assert np.array_equal(ra, cur), (d, t)     # the refill's copies come out first
 
 
-def test_prediction_launches_equal_single_row_chains(lib):
+def test_prediction_launches_equal_single_row_chains():
     """The prediction launches of one graph step: launch j rolls one row per instance with action pending[b][j],
     in place, and instance b runs only while j < its prediction length.  Three Go2 seq-jump instances with
     delays 0, 2 and 5 equal, bit for bit, chains of d single-instance env steps; the chains of the delayed
@@ -204,20 +206,17 @@ def test_prediction_launches_equal_single_row_chains(lib):
         pending[b, :lens[b]] = rng.uniform(-1, 1, (lens[b], nu))
     desc = env.plan_desc(Nsample=4, Hsample=6, Hnode=Hn, temp_sample=0.05,
                          M_n2u=interp_matrix(np.linspace(0, 1, Hn + 1), np.linspace(0, 1, 7)), n_inst=B)
-    md = _capi.fill_model_desc(env.sys.model)
     bat = dict(qpos=qpos.copy(), qvel=qvel.copy(), warm=warm.copy(), cnt=counters.copy())
     rew = np.zeros(B, np.float32)
     for j in range(int(lens.max())):
-        assert lib.emul_env_launch(C.byref(md), C.byref(desc), B, 1, _p(pending[:, j:]), DMAX * nu, _p(lens), j,
-                                   _p(bat["qpos"]), _p(bat["qvel"]), _p(bat["warm"]), _p(bat["cnt"]), _p(rew)) == 0
+        env_launch(env, desc, B, 1, pending.reshape(-1)[j * nu:], DMAX * nu, lens, j, bat, rew)
     for b in range(B):
         one = dict(qpos=qpos[b:b + 1].copy(), qvel=qvel[b:b + 1].copy(), warm=warm[b:b + 1].copy(),
                    cnt=counters[b:b + 1].copy())
         r1 = np.zeros(1, np.float32)
         for j in range(lens[b]):
             act = np.ascontiguousarray(pending[b, j][None])
-            assert lib.emul_env_launch(C.byref(md), C.byref(desc), 1, 0, _p(act), 0, None, 0, _p(one["qpos"]),
-                                       _p(one["qvel"]), _p(one["warm"]), _p(one["cnt"]), _p(r1)) == 0
+            env_launch(env, desc, 1, 0, act, 0, None, 0, one, r1)
         for k in ("qpos", "qvel", "warm", "cnt"):
             assert np.array_equal(bat[k][b], one[k][0]), (b, k)
         assert bat["cnt"][b, 0] == counters[b, 0] + lens[b]

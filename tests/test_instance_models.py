@@ -3,7 +3,6 @@
 own models (bitwise equal to single-instance launches on each model)."""
 import ctypes as C
 import os
-import subprocess
 import xml.etree.ElementTree as ET
 
 import numpy as np
@@ -13,9 +12,10 @@ from dial_mpc_b200 import _capi
 from dial_mpc_b200.modelc.mjcf import compile_mjcf
 from dial_mpc_b200.utils.spline import interp_matrix
 from tests.conftest import make_pair
+from tests.emul import emul
+from tests.test_emul_batch import rollout_batched
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-EMUL = os.path.join(HERE, "emul")
 GO2_XML = os.path.join(HERE, "golden", "unitree_go2")
 FEET = ("FR", "FL", "RR", "RL")
 DERIVED = ("body_invweight0", "dof_invweight0")
@@ -108,12 +108,8 @@ def test_assigning_sys_drops_the_cached_plan():
 
 # ---- emulator: the set_instance_model check and batched launches ---------------------------------------
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    """g++ build of tests/emul/emul_models.cpp (the device code under the lock-step warp emulator)."""
-    so = str(tmp_path_factory.mktemp("emul_models") / "libdial_emul_models.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_models.cpp")])
-    return C.CDLL(so)
+def lib():
+    return emul.build()
 
 
 def _difference(lib, a, b):
@@ -145,40 +141,13 @@ def test_instance_model_check_names_the_field(lib):
     assert _difference(lib, d0, par) == "pair_geom2"
 
 
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
+def rollout_models(base_model, models, desc, wpc, *args, **kw):
+    """Rows as dial_mpc_step launches them (tests/test_emul_batch.py), instance b on models[b] (None: the plan's
+    model), in CTAs of ``wpc`` warps."""
+    return rollout_batched(base_model, desc, *args, models=models, wpc=wpc, **kw)
 
 
-def rollout_models(lib, base_model, models, desc, wpc, qpos, qvel, warm, counters, rng=None, us=None, Ybar=None,
-                   noise=None, mode=1, H=None, us_row=0, single=False):
-    """Rows as dial_mpc_step launches them, instance b on models[b] (None: the plan's model), in CTAs of
-    ``wpc`` warps.  single=True: one instance as a single-instance plan (rows_per_inst = 0)."""
-    md = _capi.fill_model_desc(base_model)
-    nq, nv, nu, nb = md.nq, md.nv, md.nu, md.nbody
-    f32 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float32)
-    qpos, qvel, warm, us, Ybar, noise = map(f32, (qpos, qvel, warm, us, Ybar, noise))
-    B = qpos.shape[0]
-    rpi = desc.Nsample + 1 if mode == 1 else 1
-    nrows = B * rpi
-    arr = None if models is None else (_capi.dial_model_desc * len(models))(*[_capi.fill_model_desc(m) for m in models])
-    cin = np.ascontiguousarray(counters, dtype=np.int32)
-    rng = None if rng is None else np.ascontiguousarray(rng, dtype=np.uint32)
-    out = dict(rewss=np.zeros((nrows, H), np.float32), rews=np.zeros(nrows, np.float32),
-               q=np.zeros((nrows, H, nq), np.float32), qd=np.zeros((nrows, H, nv), np.float32),
-               xpos=np.zeros((nrows, H, nb - 1, 3), np.float32), qpos_out=np.zeros((B, nq), np.float32),
-               qvel_out=np.zeros((B, nv), np.float32), warm_out=np.zeros((B, nv), np.float32),
-               ctrl_out=np.zeros((B, nu), np.float32), counters=cin.copy())
-    fin = mode == 0
-    rc = lib.emul_rollout_models(C.byref(md), arr, 0 if models is None else len(models), C.byref(desc), wpc, mode,
-                                 nrows, H, 0 if single else rpi, int(us_row), _p(qpos), _p(qvel), _p(warm), _p(cin),
-                                 _p(out["counters"]) if fin else None, _p(rng), _p(us), _p(Ybar), _p(noise),
-                                 _p(out["rewss"]), _p(out["rews"]), _p(out["q"]), _p(out["qd"]), _p(out["xpos"]),
-                                 *(_p(out[k]) if fin else None for k in ("qpos_out", "qvel_out", "warm_out", "ctrl_out")))
-    assert rc == 0
-    return out
-
-
-def test_seq_jump_instance_models_equal_single_instance_plans(lib):
+def test_seq_jump_instance_models_equal_single_instance_plans():
     env, o = make_pair("unitree_go2_seq_jump")
     m0 = env.sys.model
     fr = [0.4, 0.4, 0.02, 0.01, 0.01]
@@ -203,13 +172,13 @@ def test_seq_jump_instance_models_equal_single_instance_plans(lib):
     # the counters straddle the first stage boundary (the env step from step 49 enters stage 1)
     counters = np.array([[45, 0], [49, 0], [50, 1]], np.int32)
     rows = N + 1
-    plain = rollout_models(lib, m0, None, desc, 4, qpos, qvel, warm, counters, rng=keys, Ybar=Y, noise=noise, H=Hs + 1)
+    plain = rollout_models(m0, None, desc, 4, qpos, qvel, warm, counters, rng=keys, Ybar=Y, noise=noise, H=Hs + 1)
     # 3 warps per CTA: two CTAs per instance, the second repeats the instance's last row; 5: one each
     for wpc in (3, 5):
-        bat = rollout_models(lib, m0, models, desc, wpc, qpos, qvel, warm, counters, rng=keys, Ybar=Y, noise=noise,
+        bat = rollout_models(m0, models, desc, wpc, qpos, qvel, warm, counters, rng=keys, Ybar=Y, noise=noise,
                              H=Hs + 1)
         for b in range(B):
-            one = rollout_models(lib, models[b], None, single, 1, qpos[b:b + 1], qvel[b:b + 1], warm[b:b + 1],
+            one = rollout_models(models[b], None, single, 1, qpos[b:b + 1], qvel[b:b + 1], warm[b:b + 1],
                                  counters[b:b + 1], rng=keys[b:b + 1], Ybar=Y[b:b + 1], noise=noise, H=Hs + 1,
                                  single=True)
             sl = slice(b * rows, (b + 1) * rows)
@@ -220,9 +189,9 @@ def test_seq_jump_instance_models_equal_single_instance_plans(lib):
             assert not np.array_equal(bat["rewss"][b * rows:(b + 1) * rows], plain["rewss"][b * rows:(b + 1) * rows]), b
     # env step (mode 0): one row per instance, action Y[b][0], one CTA of one warp per instance
     us_row = (Hn + 1) * nu
-    bat0 = rollout_models(lib, m0, models, desc, 1, qpos, qvel, warm, counters, us=Y, mode=0, H=1, us_row=us_row)
+    bat0 = rollout_models(m0, models, desc, 1, qpos, qvel, warm, counters, us=Y, mode=0, H=1, us_row=us_row)
     for b in range(B):
-        one = rollout_models(lib, models[b], None, single, 1, qpos[b:b + 1], qvel[b:b + 1], warm[b:b + 1],
+        one = rollout_models(models[b], None, single, 1, qpos[b:b + 1], qvel[b:b + 1], warm[b:b + 1],
                              counters[b:b + 1], us=Y[b:b + 1, :1], mode=0, H=1, single=True)
         for k in ("qpos_out", "qvel_out", "warm_out", "ctrl_out", "counters"):
             assert np.array_equal(bat0[k][b], one[k][0]), (b, k)

@@ -6,7 +6,6 @@ prediction launches of lengths age + d against chains of single-row env steps.""
 import ctypes as C
 import os
 import re
-import subprocess
 import sys
 
 import numpy as np
@@ -16,10 +15,10 @@ from dial_mpc_b200 import _capi
 from dial_mpc_b200 import random as drandom
 from dial_mpc_b200.utils.spline import interp_matrix
 from tests.conftest import make_pair
+from tests.emul import emul
 from tests.test_emul_batch import _instances
-from tests.test_instance_delay import Queue
+from tests.test_instance_delay import Queue, env_launch
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 DMAX = _capi.DEFINES["DIAL_MAXDELAY"]
 R = DMAX + 1                      # records of one ring (ages 0..16)
 MAXV = _capi.DEFINES["DIAL_MAXV"]
@@ -160,14 +159,10 @@ class ObsRing(C.Structure):
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    """g++ build of tests/emul/emul_observe.cpp (the device code under the emulator)."""
-    so = str(tmp_path_factory.mktemp("emul_observe") / "libdial_emul_observe.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_observe.cpp")])
-    lib = C.CDLL(so)
-    lib.emul_sizeof_obs.restype = C.c_size_t
-    assert lib.emul_sizeof_obs(0) == C.sizeof(ObsSetting) and lib.emul_sizeof_obs(1) == C.sizeof(ObsRing)
+def lib():
+    lib = emul.build()
+    assert lib.emul_sizeof(emul.SIZEOF["ObsSetting"]) == C.sizeof(ObsSetting)
+    assert lib.emul_sizeof(emul.SIZEOF["ObsRing"]) == C.sizeof(ObsRing)
     return lib
 
 
@@ -443,21 +438,11 @@ def test_zero_rotation_sigma_keeps_the_quaternion(lib):
             assert np.array_equal(z["oq"], zero.rq[(zero.r.head - 1) % R])
 
 
-@pytest.fixture(scope="module")
-def delay_lib(tmp_path_factory):
-    """g++ build of tests/emul/emul_delay.cpp (its env-step launch)."""
-    so = str(tmp_path_factory.mktemp("emul_delay") / "libdial_emul_delay.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_delay.cpp")])
-    return C.CDLL(so)
-
-
-def test_prediction_launches_over_history_and_queue(delay_lib):
+def test_prediction_launches_over_history_and_queue():
     """The prediction launches of an observing step: instance b starts from its observed record and takes
     age_b + d_b single-row env steps with its sequence (history rows, then pending rows).  Three Go2 seq-jump
     instances with (age, d) = (0, 0), (2, 1), (3, 2) equal, bit for bit, chains of single-instance env steps,
     across the first stage boundary of the jump sequence (the step from 49)."""
-    dl = delay_lib
     env, o = make_pair("unitree_go2_seq_jump")
     B, Hn = 3, 3
     nu = env.action_size
@@ -471,20 +456,17 @@ def test_prediction_launches_over_history_and_queue(delay_lib):
         seq[b, :lens[b]] = rng.uniform(-1, 1, (lens[b], nu))
     desc = env.plan_desc(Nsample=4, Hsample=6, Hnode=Hn, temp_sample=0.05,
                          M_n2u=interp_matrix(np.linspace(0, 1, Hn + 1), np.linspace(0, 1, 7)), n_inst=B)
-    md = _capi.fill_model_desc(env.sys.model)
     bat = dict(qpos=qpos.copy(), qvel=qvel.copy(), warm=warm.copy(), cnt=counters.copy())
     rew = np.zeros(B, np.float32)
     for j in range(int(lens.max())):
-        assert dl.emul_env_launch(C.byref(md), C.byref(desc), B, 1, _p(seq[:, j:]), DMAX * nu, _p(lens), j,
-                                  _p(bat["qpos"]), _p(bat["qvel"]), _p(bat["warm"]), _p(bat["cnt"]), _p(rew)) == 0
+        env_launch(env, desc, B, 1, seq.reshape(-1)[j * nu:], DMAX * nu, lens, j, bat, rew)
     for b in range(B):
         one = dict(qpos=qpos[b:b + 1].copy(), qvel=qvel[b:b + 1].copy(), warm=warm[b:b + 1].copy(),
                    cnt=counters[b:b + 1].copy())
         r1 = np.zeros(1, np.float32)
         for j in range(lens[b]):
             act = np.ascontiguousarray(seq[b, j][None])
-            assert dl.emul_env_launch(C.byref(md), C.byref(desc), 1, 0, _p(act), 0, None, 0, _p(one["qpos"]),
-                                      _p(one["qvel"]), _p(one["warm"]), _p(one["cnt"]), _p(r1)) == 0
+            env_launch(env, desc, 1, 0, act, 0, None, 0, one, r1)
         for k in ("qpos", "qvel", "warm", "cnt"):
             assert np.array_equal(bat[k][b], one[k][0]), (b, k)
         assert bat["cnt"][b, 0] == counters[b, 0] + lens[b]

@@ -16,10 +16,6 @@ from tests.emul import emul
 KMAX = _capi.DEFINES["DIAL_MAXSUBSTEPS"]
 
 
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
 def plant_descs(env, k, iterations=None, ls_iterations=None, tolerance=None):
     """The plant's model and plan descriptors as the library derives them: the model's timestep / k in fp32 and
     the given solver settings, n_frames * k; everything else the plan's."""
@@ -32,21 +28,16 @@ def plant_descs(env, k, iterations=None, ls_iterations=None, tolerance=None):
     return md, desc
 
 
-def emul_env_step(env, md, desc, q, v, w, a, step0):
-    """One env step (mode 0, one row, H = 1) of the device code on the descriptors given."""
-    lib = emul.build(reward_source=getattr(env, "reward_source", None) or None)
+def emul_env_step(env, md, desc, q, v, w, a, step0, **kw):
+    """One env step (mode 0, one row, H = 1) of the device code on the descriptors given; ``kw``: emul.launch's."""
     nq, nv, nu, nb = md.nq, md.nv, md.nu, md.nbody
     f32 = lambda x: np.ascontiguousarray(x, dtype=np.float32)
-    q, v, w, us = f32(q), f32(v), f32(w), f32(np.asarray(a).reshape(1, 1, nu))
     out = dict(rewss=np.zeros((1, 1), np.float32), rews=np.zeros(1, np.float32), q=np.zeros((1, 1, nq), np.float32),
                qd=np.zeros((1, 1, nv), np.float32), xpos=np.zeros((1, 1, nb - 1, 3), np.float32),
                qpos_out=np.zeros(nq, np.float32), qvel_out=np.zeros(nv, np.float32), warm_out=np.zeros(nv, np.float32),
                ctrl_out=np.zeros(nu, np.float32))
-    rc = lib.emul_rollout(C.byref(md), C.byref(desc), 0, 1, 1, int(step0), 0, _p(q), _p(v), _p(w), _p(us), None, None,
-                          None, C.c_uint32(0), C.c_uint32(0), _p(out["rewss"]), _p(out["rews"]), _p(out["q"]),
-                          _p(out["qd"]), _p(out["xpos"]), _p(out["qpos_out"]), _p(out["qvel_out"]),
-                          _p(out["warm_out"]), _p(out["ctrl_out"]), None)
-    assert rc == 0
+    emul.launch(md, desc, reward_source=getattr(env, "reward_source", None) or None, mode=0, nrows=1, H=1, step0=step0,
+                qpos0=f32(q), qvel0=f32(v), warm0=f32(w), us=f32(np.asarray(a).reshape(1, 1, nu)), **out, **kw)
     return out
 
 

@@ -6,9 +6,7 @@ and Allegro's ball, at many states, for points off the COM and torque-only impul
 spatial momentum of the pushed tree changes by exactly the spatial impulse; a zero impulse leaves qvel bit for
 bit; and the firing window of an entry."""
 import ctypes as C
-import os
 import re
-import subprocess
 import sys
 
 import numpy as np
@@ -16,8 +14,8 @@ import pytest
 
 from dial_mpc_b200 import _capi
 from tests.conftest import make_pair
+from tests.emul import emul
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 PMAX = _capi.DEFINES["DIAL_MAXPUSH"]
 MODELS = ["unitree_go2_walk", "unitree_h1_walk", "branchpod", "hexapod", "longchain", "slidepod", "allegro_reorient"]
 # Delta qvel of the emulator (fp64 throughout) against the oracle's np.linalg.solve: both fp64, in other
@@ -132,15 +130,10 @@ class PushTable(C.Structure):
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    """g++ build of tests/emul/emul_push.cpp (the device code under the emulator)."""
-    so = str(tmp_path_factory.mktemp("emul_push") / "libdial_emul_push.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_push.cpp")])
-    lib = C.CDLL(so)
-    lib.emul_sizeof_push.restype = C.c_size_t
-    assert lib.emul_sizeof_push(0) == C.sizeof(_capi.dial_push) and lib.emul_sizeof_push(1) == C.sizeof(PushTable)
-    lib.emul_push_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double] + [C.c_void_p] * 4 + [C.c_int]
+def lib():
+    lib = emul.build()
+    assert lib.emul_sizeof(emul.SIZEOF["dial_push"]) == C.sizeof(_capi.dial_push)
+    assert lib.emul_sizeof(emul.SIZEOF["PushTable"]) == C.sizeof(PushTable)
     return lib
 
 

@@ -2,10 +2,7 @@
 table (schedule_table) against MBDPI.schedule of the updated config, the --instance-overrides errors, and on
 the warp emulator the planner rows of a batched launch with per-instance noise rows against single-instance
 launches bound to that row, and the CTA -> instance mapping the skipped instances exit by (cta_instance)."""
-import ctypes as C
 import dataclasses
-import os
-import subprocess
 import sys
 
 import numpy as np
@@ -16,9 +13,9 @@ from dial_mpc_b200 import _capi
 from dial_mpc_b200.core.dial_config import DialConfig
 from dial_mpc_b200.utils.spline import interp_matrix
 from tests.conftest import make_pair
+from tests.emul import emul
 from tests.test_emul_batch import _instances
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 BASE = DialConfig(env_name="unitree_go2_walk", Nsample=64, Hsample=12, Hnode=4, Ndiffuse=2, Ndiffuse_init=3,
                   temp_sample=0.05, horizon_diffuse_factor=0.9, traj_diffuse_factor=0.5)
 
@@ -115,35 +112,23 @@ SCHED = np.dtype([("on", "<i4"), ("temp", "<f4"), ("n_rows", "<i4"), ("pad", "<i
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    """g++ build of tests/emul/emul_schedule.cpp (the device code under the lock-step warp emulator)."""
-    so = str(tmp_path_factory.mktemp("emul_schedule") / "libdial_emul_schedule.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC", "-o", so,
-                           os.path.join(EMUL, "emul_schedule.cpp")])
-    lib = C.CDLL(so)
-    lib.emul_sizeof_schedule.restype = C.c_size_t
-    assert lib.emul_sizeof_schedule() == SCHED.itemsize
+def lib():
+    lib = emul.build()
+    assert lib.emul_sizeof(emul.SIZEOF["InstSchedule"]) == SCHED.itemsize
     return lib
 
 
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
-def _rows(lib, env, desc, qpos, qvel, warm, counters, keys, Y, noise, iter_, sched, single):
-    md = _capi.fill_model_desc(env.sys.model)
+def _rows(env, desc, qpos, qvel, warm, counters, keys, Y, noise, iter_, sched, single):
     f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
-    qpos, qvel, warm, Y, noise = map(f32, (qpos, qvel, warm, Y, noise))
-    B, rows, H = qpos.shape[0], desc.Nsample + 1, desc.Hsample + 1
-    rews, q = np.zeros(B * rows, np.float32), np.zeros((B * rows, H, md.nq), np.float32)
-    rc = lib.emul_rollout_schedule(C.byref(md), C.byref(desc), B * rows, H, 0 if single else rows, iter_, _p(sched),
-                                   _p(qpos), _p(qvel), _p(warm), _p(np.ascontiguousarray(counters, np.int32)),
-                                   _p(np.ascontiguousarray(keys, np.uint32)), _p(Y), _p(noise), _p(rews), _p(q))
-    assert rc == 0
+    B, rows, H, nq = qpos.shape[0], desc.Nsample + 1, desc.Hsample + 1, env.sys.nq
+    rews, q = np.zeros(B * rows, np.float32), np.zeros((B * rows, H, nq), np.float32)
+    emul.launch(env, desc, mode=1, nrows=B * rows, H=H, rows_per_inst=0 if single else rows, iter=iter_, sched=sched,
+                qpos0=f32(qpos), qvel0=f32(qvel), warm0=f32(warm), counters_in=np.ascontiguousarray(counters, np.int32),
+                rng_dev=np.ascontiguousarray(keys, np.uint32), Ybar=f32(Y), noise=f32(noise), rews=rews, q=q)
     return rews, q
 
 
-def test_batched_rows_take_their_instance_noise_row(lib):
+def test_batched_rows_take_their_instance_noise_row():
     """Instance b's planner rows at iteration i with its own table equal a single-instance launch bound to
     row i of that table; an instance whose schedule is off takes the bound row."""
     env, o = make_pair("unitree_go2_walk")
@@ -160,16 +145,16 @@ def test_batched_rows_take_their_instance_noise_row(lib):
     for b, scale in ((1, 0.3), (2, 1.7)):
         sched["on"][b], sched["temp"][b], sched["n_rows"][b] = 1, 0.1, it + 1
         sched["noise"][b, :it + 1, :Hn + 1] = rng.uniform(0.1, 1.0, (it + 1, Hn + 1)) * scale
-    bat = _rows(lib, env, desc, qpos, qvel, warm, counters, keys, Y, bound, it, sched, single=False)
+    bat = _rows(env, desc, qpos, qvel, warm, counters, keys, Y, bound, it, sched, single=False)
     rows = N + 1
     for b in range(B):
         row = sched["noise"][b, it, :Hn + 1] if sched["on"][b] else bound
-        one = _rows(lib, env, desc, qpos[b:b + 1], qvel[b:b + 1], warm[b:b + 1], counters[b:b + 1], keys[b:b + 1],
+        one = _rows(env, desc, qpos[b:b + 1], qvel[b:b + 1], warm[b:b + 1], counters[b:b + 1], keys[b:b + 1],
                     Y[b:b + 1], row, 0, None, single=True)
         sl = slice(b * rows, (b + 1) * rows)
         assert np.array_equal(bat[0][sl], one[0]) and np.array_equal(bat[1][sl], one[1]), b
     # the table row was read: instance 1 bound to the plan's row differs
-    other = _rows(lib, env, desc, qpos[1:2], qvel[1:2], warm[1:2], counters[1:2], keys[1:2], Y[1:2], bound, 0, None,
+    other = _rows(env, desc, qpos[1:2], qvel[1:2], warm[1:2], counters[1:2], keys[1:2], Y[1:2], bound, 0, None,
                   single=True)
     assert not np.array_equal(bat[0][rows:2 * rows], other[0])
 

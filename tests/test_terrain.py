@@ -4,7 +4,6 @@ step of the terrain build in the warp emulator against the oracle's env step on 
 terrain_oracle.py), at the emulator's parity bounds (tests/test_instance_plant.py); a flat terrain at z = 0
 bitwise equal to no terrain; ``dial_terrain_height``; the spec and CLI errors; the struct layout."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -13,16 +12,11 @@ import pytest
 from dial_mpc_b200 import _capi
 from dial_mpc_b200 import terrain as T
 from tests.conftest import make_pair
+from tests.emul import emul
 from tests.terrain_oracle import collision, floor_pairs, on_terrain
 from tests.test_instance_plant import emul_env_step, mid_run_states
 
 import oracle.mjx_oracle as mo
-
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
-
-
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 # ---- generators and the surface --------------------------------------------------------------------------------
@@ -152,38 +146,10 @@ def test_uniform_slope_is_a_tilted_plane_geom(name):
 
 
 # ---- the emulator's terrain build ------------------------------------------------------------------------------
-_LIBS = {}
-
-
-def _lib(reward_source=None):
-    key = reward_source or ""
-    if key not in _LIBS:
-        so = os.path.join(EMUL, f"libdial_emul_terrain{'_' + os.path.basename(key).split('.')[0] if key else ''}.so")
-        extra = [f'-DDIAL_CUSTOM_REWARD_FILE="{os.path.abspath(reward_source)}"'] if reward_source else []
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-I", EMUL, "-shared", "-fPIC"] + extra +
-                              ["-o", so, os.path.join(EMUL, "emul_terrain.cpp")])
-        lib = C.CDLL(so)
-        lib.emul_terrain_height.restype = C.c_float
-        lib.emul_terrain_height.argtypes = [C.c_void_p, C.c_float, C.c_float]
-        _LIBS[key] = lib
-    return _LIBS[key]
-
-
 def emul_terrain_step(env, t, q, v, w, a, step0):
-    lib = _lib(getattr(env, "reward_source", None) or None)
-    md, desc = _capi.fill_model_desc(env.sys.model), env.plan_desc()
-    f32 = lambda x: np.ascontiguousarray(x, dtype=np.float32)
-    q, v, w, us = f32(q), f32(v), f32(w), f32(np.asarray(a).reshape(1, 1, md.nu))
-    out = dict(rewss=np.zeros((1, 1), np.float32), q=np.zeros((1, 1, md.nq), np.float32),
-               qd=np.zeros((1, 1, md.nv), np.float32), qpos_out=np.zeros(md.nq, np.float32),
-               qvel_out=np.zeros(md.nv, np.float32), warm_out=np.zeros(md.nv, np.float32),
-               ctrl_out=np.zeros(md.nu, np.float32))
-    ct = None if t is None else t.c_struct()
-    rc = lib.emul_rollout_terrain(C.byref(md), C.byref(desc), None if ct is None else C.byref(ct), 0, 1, 1, int(step0),
-                                  _p(q), _p(v), _p(w), _p(us), _p(out["rewss"]), _p(out["q"]), _p(out["qd"]),
-                                  _p(out["qpos_out"]), _p(out["qvel_out"]), _p(out["warm_out"]), _p(out["ctrl_out"]))
-    assert rc == 0
-    return out
+    """One env step of the terrain build on the terrain `t` (None: a row without a terrain)."""
+    return emul_env_step(env, _capi.fill_model_desc(env.sys.model), env.plan_desc(), q, v, w, a, step0,
+                         terrain=None if t is None else [t.c_struct()], defines=("DIAL_TERRAIN",))
 
 
 def _pair(name):
@@ -274,7 +240,7 @@ def test_no_floor_pair_is_rejected(tmp_path):
 
 
 def test_custom_reward_terrain_height():
-    lib = _lib()
+    lib = emul.build(("DIAL_TERRAIN",))
     rng = np.random.default_rng(4)
     t = T.grid(rng.normal(size=(6, 8)) * 0.2, 0.3, (-1.0, -0.5))
     ct = t.c_struct()
