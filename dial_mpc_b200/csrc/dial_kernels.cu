@@ -28,59 +28,22 @@ static int fail(const std::string& s) { g_err = s; return -1; }
 
 // The rollout kernel lives in dial_rollout_variant.cu, compiled once per solver variant
 // (-DDIAL_VARIANT=v) so that the five instantiations build in parallel; each object exports
-// one launcher.  Custom-reward builds (-DDIAL_ONLY_VARIANT=v) compile a single translation unit.
+// one launcher.  Custom-reward builds (-DDIAL_ONLY_VARIANT=v) compile a single translation unit, whose one
+// launcher (DIAL_V_LAUNCHER) is the terrain build when compiled with DIAL_TERRAIN.
+typedef cudaError_t (*dial_launch_fn)(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t);
 #ifdef DIAL_ONLY_VARIANT
-#define DIAL_HAS_VARIANT(v) ((v) == DIAL_ONLY_VARIANT)
 #define DIAL_VARIANT DIAL_ONLY_VARIANT
 #include "dial_rollout_variant.cu"
 #else
-#define DIAL_HAS_VARIANT(v) 1
-#endif
-#define DIAL_DECL_LAUNCH(v) cudaError_t dial_launch_rollout_v##v(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t);
-#if DIAL_HAS_VARIANT(0)
-DIAL_DECL_LAUNCH(0)
-#endif
-#if DIAL_HAS_VARIANT(1)
-DIAL_DECL_LAUNCH(1)
-#endif
-#if DIAL_HAS_VARIANT(2)
-DIAL_DECL_LAUNCH(2)
-#endif
-#if DIAL_HAS_VARIANT(3)
-DIAL_DECL_LAUNCH(3)
-#endif
-#if DIAL_HAS_VARIANT(4)
-DIAL_DECL_LAUNCH(4)
-#endif
-// Terrain builds (dial_rollout_variant.cu with -DDIAL_TERRAIN) of every stock variant but the dense one, which
-// has none: the launches that read a terrain (dial_plan_set_instance_terrain) run them.  A custom build holds
-// one when compiled with DIAL_TERRAIN, and its one kernel then serves every launch.
-#if defined(DIAL_ONLY_VARIANT) && !defined(DIAL_TERRAIN)
-#define DIAL_HAS_TERRAIN(v) 0
-#else
-#define DIAL_HAS_TERRAIN(v) (DIAL_HAS_VARIANT(v) && (v) != 3)
-#endif
-#define DIAL_DECL_TERRAIN(v) cudaError_t dial_launch_rollout_v##v##_terrain(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t);
-#if DIAL_HAS_TERRAIN(0)
-DIAL_DECL_TERRAIN(0)
-#endif
-#if DIAL_HAS_TERRAIN(1)
-DIAL_DECL_TERRAIN(1)
-#endif
-#if DIAL_HAS_TERRAIN(2)
-DIAL_DECL_TERRAIN(2)
-#endif
-#if DIAL_HAS_TERRAIN(4)
-DIAL_DECL_TERRAIN(4)
-#endif
+#define DIAL_DECL_LAUNCH(s) cudaError_t dial_launch_rollout_##s(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t);
+DIAL_DECL_LAUNCH(v0) DIAL_DECL_LAUNCH(v1) DIAL_DECL_LAUNCH(v2) DIAL_DECL_LAUNCH(v3) DIAL_DECL_LAUNCH(v4)
+// Terrain builds (dial_rollout_variant.cu with -DDIAL_TERRAIN) of every variant but the dense one, which has
+// none: the launches that read a terrain (dial_plan_set_instance_terrain) run them.
+DIAL_DECL_LAUNCH(v0_terrain) DIAL_DECL_LAUNCH(v1_terrain) DIAL_DECL_LAUNCH(v2_terrain) DIAL_DECL_LAUNCH(v4_terrain)
 // Shape-specialised star<3,6> kernels (dial_rollout_variant.cu with -DDIAL_SHAPE_NAME=s): the stock Go2
 // scene, with the structure values that dial_mpc_b200.modelc.shape derives from its model.  A plan launches one only when dial_shape_matches_<s> finds every fixed
 // value equal to its own model and plan.  Custom-reward builds hold none.
-#ifndef DIAL_ONLY_VARIANT
-typedef cudaError_t (*dial_launch_fn)(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t);
-#define DIAL_DECL_SHAPE(s) \
-  cudaError_t dial_launch_rollout_##s(const DevModel*, const DevPlan*, const RolloutArgs&, int, int, size_t, cudaStream_t); \
-  bool dial_shape_matches_##s(const DevModel&, const dial_plan_desc&);
+#define DIAL_DECL_SHAPE(s) DIAL_DECL_LAUNCH(s) bool dial_shape_matches_##s(const DevModel&, const dial_plan_desc&);
 DIAL_DECL_SHAPE(go2)
 static const struct {
   const char* name;
@@ -820,7 +783,13 @@ struct dial_plan {
   DevModel* dM = nullptr;
   DevPlan* dP = nullptr;
   int variant = 0;
-  int shape = 0;                // 1 + index into kShapes: the shape-specialised kernel of the variant; 0: generic
+  // the rollout launchers (resolve_kernels): `flat` serves the launches without a terrain, `generic` those on
+  // the plant's plan descriptors, `terrain` (null: none) those that read a terrain table; `name` names `flat`
+  struct { dial_launch_fn flat, generic, terrain; const char* name; } kernels{};
+  // lock-step level of a launch of 2 or more warps per CTA (RolloutArgs.lockstep): a CTA barrier per env step
+  // shares the instruction fetch on every path; the generic tree adds one before the constraint solve, and the
+  // dense path, whose unrolled solver is hundreds of KB of SASS, one per Newton iteration
+  int lockstep = 1;
   int n_inst = 1;               // independent planner instances (dial_plan_desc.n_inst)
   int n_ens = 0;                // planning models per instance (dial_plan_desc.n_ens)
   int num_sms = 132;
@@ -837,7 +806,6 @@ struct dial_plan {
   float* partial = nullptr;
   float* tb_partial = nullptr;
   unsigned int* counter = nullptr;
-  unsigned int* row_counter = nullptr;
   float* zeros = nullptr;                                          // [nv]
   int ybar_grid = 0;
   int upd_grid = 0;             // grid of the fused update kernel: about 8 samples per thread slot
@@ -1006,60 +974,41 @@ extern "C" size_t dial_sizeof(int which) {
        : which == 6 ? sizeof(dial_plant) : which == 7 ? sizeof(dial_terrain) : 0;
 }
 
-// solver instantiation by tree shape: star<3,6> (quadruped), star<5,7> (humanoid), star<5,6>,
-// dense<22> (elliptic cones), generic tree.  `wpc` warps per CTA (1..16; one kernel serves all).
-// `dP`: the plan descriptor the launch reads (null: the plan's own); `generic`: the generic kernel of the
-// plan's variant even where a shape-specialised one matches (whose solver counts and n_frames are fixed).
+// The plan's rollout launchers, fixed by its model, variant and plan descriptor.  Solver instantiation by tree
+// shape: star<3,6> (quadruped), star<5,7> (humanoid), star<5,6>, dense<22> (elliptic cones), generic tree.
+// `flat` is the shape-specialised kernel of the variant when one matches (not with DIAL_FORCE_GENERIC_SHAPE=1:
+// it computes bit for bit what the generic one does, and tests compare the two), else the variant's.
+static void resolve_kernels(dial_plan* p) {
+  static const char* const names[] = {"v0", "v1", "v2", "v3", "v4"};
+  p->kernels.name = names[p->variant];
+#ifdef DIAL_ONLY_VARIANT
+  p->kernels.flat = p->kernels.generic = DIAL_V_LAUNCHER;   // the variant was checked against DIAL_ONLY_VARIANT
+#ifdef DIAL_TERRAIN
+  p->kernels.terrain = DIAL_V_LAUNCHER;
+#endif
+#else
+  static const dial_launch_fn generic[] = {dial_launch_rollout_v0, dial_launch_rollout_v1, dial_launch_rollout_v2,
+                                           dial_launch_rollout_v3, dial_launch_rollout_v4};
+  static const dial_launch_fn terrain[] = {dial_launch_rollout_v0_terrain, dial_launch_rollout_v1_terrain,
+                                           dial_launch_rollout_v2_terrain, nullptr, dial_launch_rollout_v4_terrain};
+  p->kernels.flat = p->kernels.generic = generic[p->variant];
+  p->kernels.terrain = terrain[p->variant];
+  if (p->variant == 1 && !getenv("DIAL_FORCE_GENERIC_SHAPE"))
+    for (const auto& s : kShapes)
+      if (s.matches(p->hM, p->hP.c)) { p->kernels.flat = s.launch; p->kernels.name = s.name; break; }
+#endif
+}
+
+// One rollout launch of `wpc` warps per CTA (1..16; one kernel serves all).  `dP`: the plan descriptor the
+// launch reads (null: the plan's own); `generic`: the generic kernel of the plan's variant even where a
+// shape-specialised one matches (whose solver counts and n_frames are fixed).
 static cudaError_t launch_rollout(dial_plan* p, const RolloutArgs& A, int wpc, cudaStream_t st,
                                   const DevPlan* dP = nullptr, bool generic = false) {
   const size_t smem = sizeof(DevModel) + sizeof(DevPlan) + (size_t)wpc * p->hM.warp_floats * sizeof(float);
-  int grid = rollout_grid(A, wpc);
-  if (A.row_counter) {
-    const int resident = p->num_sms * (wpc > 8 ? 1 : 16 / wpc);
-    grid = grid < resident ? grid : resident;
-    cudaError_t e = cudaMemsetAsync(A.row_counter, 0, sizeof(unsigned int), st);
-    if (e != cudaSuccess) return e;
-  }
   p->launches++;
-  if (!dP) dP = p->dP;
-  if (A.terrain) {   // a launch that reads a terrain table: the terrain build of the plan's variant
-    switch (p->variant) {
-#if DIAL_HAS_TERRAIN(1)
-      case 1: return dial_launch_rollout_v1_terrain(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-#if DIAL_HAS_TERRAIN(2)
-      case 2: return dial_launch_rollout_v2_terrain(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-#if DIAL_HAS_TERRAIN(4)
-      case 4: return dial_launch_rollout_v4_terrain(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-#if DIAL_HAS_TERRAIN(0)
-      case 0: return dial_launch_rollout_v0_terrain(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-      default: return cudaErrorInvalidDeviceFunction;
-    }
-  }
-#ifndef DIAL_ONLY_VARIANT
-  if (p->shape > 0 && !generic) return kShapes[p->shape - 1].launch(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-  switch (p->variant) {
-#if DIAL_HAS_VARIANT(1)
-    case 1: return dial_launch_rollout_v1(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-#if DIAL_HAS_VARIANT(2)
-    case 2: return dial_launch_rollout_v2(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-#if DIAL_HAS_VARIANT(3)
-    case 3: return dial_launch_rollout_v3(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-#if DIAL_HAS_VARIANT(4)
-    case 4: return dial_launch_rollout_v4(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-#if DIAL_HAS_VARIANT(0)
-    case 0: return dial_launch_rollout_v0(p->dM, dP, A, grid, wpc, smem, st);
-#endif
-    default: return cudaErrorInvalidDeviceFunction;
-  }
+  const dial_launch_fn launch = A.terrain ? p->kernels.terrain : generic ? p->kernels.generic : p->kernels.flat;
+  if (!launch) return cudaErrorInvalidDeviceFunction;
+  return launch(p->dM, dP ? dP : p->dP, A, rollout_grid(A, wpc), wpc, smem, st);
 }
 
 // Launch shape.  One CTA per SM with up to 16 warps that re-converge at every env step
@@ -1095,23 +1044,8 @@ static cudaError_t launch_rollout_any(dial_plan* p, const RolloutArgs& A0, cudaS
     }
   }
   if (wpc < 1 || wpc > DIAL_MAXTHREADS / 32) return cudaErrorInvalidValue;
-  // lock-step pays off on both solver paths.  The dense (elliptic) path used to run free with
-  // dynamic row assignment because MJX's 50-iteration line searches made its rows heavy-tailed;
-  // since the line search stops at the detected cycle, sharing the instruction fetch wins there
-  // too, and the finer the better (slowest to fastest: free-running with dynamic rows, a barrier per
-  // env step, per physics substep, per Newton iteration = level 3, the dense default).  DIAL_NO_LOCKSTEP=1 restores the free-running
-  // warps, DIAL_NO_MIDSYNC=1 / DIAL_DENSE_LOCKSTEP=2 select the coarser levels.
-  A.lockstep = (wpc >= 2 && !getenv("DIAL_NO_LOCKSTEP")) ? 1 : 0;
-  // (not with per-instance models: a persistent warp takes rows of any instance)
-  if (p->hM.dense && !A.lockstep && !A.models && A.nrows > wpc * p->num_sms && !getenv("DIAL_NO_DYNAMIC_ROWS")) A.row_counter = p->row_counter;
-  // second barrier before the constraint solve: the dense path needs it (and a third per Newton
-  // iteration); on the star paths it stopped paying once the solver shrank — DIAL_MIDSYNC=1 /
-  // DIAL_NO_MIDSYNC=1 override
-  const bool mid = getenv("DIAL_MIDSYNC") ? true : (getenv("DIAL_NO_MIDSYNC") ? false : (p->hM.dense || !p->hM.s_on));
-  if (A.lockstep && mid) A.lockstep = 2;
-  { const char* se = getenv("DIAL_SYNC_EVERY"); A.sync_every = se ? atoi(se) : 1; if (A.sync_every < 1) A.sync_every = 1; }
-  const char* dl = getenv("DIAL_DENSE_LOCKSTEP");
-  if (A.lockstep == 2 && p->hM.dense && !(dl && atoi(dl) == 2)) A.lockstep = 3;
+  // sync_every (0) and row_counter (null) stay unset: a barrier at every env step, and every warp on its own row
+  A.lockstep = wpc >= 2 ? p->lockstep : 0;
   return launch_rollout(p, A, wpc, st);
 }
 
@@ -1168,13 +1102,8 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
     if ((int64_t)p->n_inst * c.n_ens * (c.Nsample + 1) > 0x7fffffff) { g_err = "n_inst * n_ens * (Nsample + 1) exceeds 2^31 - 1 rows per rollout launch"; delete p; return nullptr; }
   }
   p->n_ens = c.n_ens;
-#ifndef DIAL_ONLY_VARIANT
-  // the specialised kernel computes bit for bit what the generic one does; DIAL_FORCE_GENERIC_SHAPE=1
-  // keeps the generic kernel (tests compare the two)
-  if (p->variant == 1 && !getenv("DIAL_FORCE_GENERIC_SHAPE"))
-    for (int s = 0; s < (int)(sizeof(kShapes) / sizeof(kShapes[0])); ++s)
-      if (kShapes[s].matches(p->hM, p->hP.c)) { p->shape = s + 1; break; }
-#endif
+  resolve_kernels(p);
+  p->lockstep = p->hM.dense ? 3 : p->hM.s_on ? 1 : 2;
   auto bad = [&](cudaError_t e, const char* what) {
     g_err = std::string(what) + ": " + cudaGetErrorString(e);
     dial_plan_destroy(p);
@@ -1223,7 +1152,6 @@ extern "C" dial_plan* dial_plan_create(const dial_model_desc* model, const dial_
   if (p->own(e, p->tb_partial, B * TB_CHUNKS * H * (m.nq + m.nv + 3 * (m.nbody - 1)) * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(tb_partial)");
   if (p->own(e, p->counter, B * sizeof(unsigned int)) != cudaSuccess) return bad(e, "cudaMalloc(counter)");
   if ((e = cudaMemset(p->counter, 0, B * sizeof(unsigned int))) != cudaSuccess) return bad(e, "cudaMemset(counter)");
-  if (p->own(e, p->row_counter, sizeof(unsigned int)) != cudaSuccess) return bad(e, "cudaMalloc(row_counter)");
   if (getenv("DIAL_DEBUG_COUNTERS")) {
     if (p->own(e, p->dbg, 8 * sizeof(float)) != cudaSuccess) return bad(e, "cudaMalloc(dbg)");
     cudaMemset(p->dbg, 0, 8 * sizeof(float));
@@ -1800,7 +1728,7 @@ extern "C" int dial_plan_set_instance_terrain(dial_plan* p, int b, int side, con
     floor |= (m.pair_kind[k] == PAIR_PLANE_SPHERE || m.pair_kind[k] == PAIR_PLANE_CAPSULE) && m.geom_bodyid[m.pair_geom1[k]] == 0;
   if (!floor) return fail(at + "the model has no floor pair (a plane geom on the world body against a sphere or capsule)");
   if (p->hM.dense) return fail(at + "the dense solver path has no terrain build");
-  if (!DIAL_HAS_TERRAIN(p->variant)) return fail(at + "this custom build has no terrain kernel (compile it with DIAL_TERRAIN)");
+  if (!p->kernels.terrain) return fail(at + "this custom build has no terrain kernel (compile it with DIAL_TERRAIN)");
   const dial_plan_desc& c = p->hP.c;
   if (c.Ntotal != c.Nsample || p->xch.on) return fail(at + "sharded plans (Ntotal != Nsample) have no per-instance terrain");
   if (!p->mpc_bound) return fail(at + "call dial_mpc_bind first");
@@ -2419,12 +2347,7 @@ extern "C" int dial_solver_variant(const dial_model_desc* model) {
 }
 
 extern "C" const char* dial_plan_rollout_kernel(const dial_plan* p) {
-  static const char* const generic[] = {"v0", "v1", "v2", "v3", "v4"};
-  if (!p) return "";
-#ifndef DIAL_ONLY_VARIANT
-  if (p->shape > 0) return kShapes[p->shape - 1].name;
-#endif
-  return p->variant >= 0 && p->variant <= 4 ? generic[p->variant] : "";
+  return p ? p->kernels.name : "";
 }
 
 extern "C" const char* dial_custom_reward_id(void) {

@@ -22,4 +22,4 @@ e0.record()
 for i in range(20): mb.plan.reverse_rollout(st, None, key, Y, mb.sigma_control, mb._rews_local)
 e1.record(); torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / 20
-print(f"{name} N={N} Hs={Hs} WPC={os.environ.get('DIAL_WPC','auto')} lockstep={'off' if os.environ.get('DIAL_NO_LOCKSTEP') else 'on'}: rollout kernel {ms:.3f} ms -> {N*Hs/ms*1e3:.3e} sample-steps/s  rews {float(mb._rews_local.mean()):.5f}")
+print(f"{name} N={N} Hs={Hs} WPC={os.environ.get('DIAL_WPC','auto')}: rollout kernel {ms:.3f} ms -> {N*Hs/ms*1e3:.3e} sample-steps/s  rews {float(mb._rews_local.mean()):.5f}")
